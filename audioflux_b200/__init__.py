@@ -1,4 +1,4 @@
-"""audioflux_b200: B200-native (sm_100a) drop-in for audioFlux's time-frequency hot path.
+"""audioflux_b200: H100-native (sm_90a) drop-in for audioFlux's time-frequency hot path.
 
 Host-side mirror of the reference's operator interface (same class / method / argument
 names as python/audioflux/{stft,bft,cqt,cwt,spectrogram}.py and feature/xxcc.py) over the C-ABI

@@ -217,12 +217,13 @@ int af_launch_cqt_octave_tc(const float *sig, int sigStride, int batch, int vali
                             int padLeft, int timeLength, const float *bfrag, const float *scale, int num, int colOff,
                             float *outRe, float *outIm, void *stream);
 
-/* tcgen05 octave kernel (kernels/cqt_umma.cu): the staged signal itself is the Hankel A operand; hops 4 .. 128 */
-int af_cqt_umma_supported(int fftLength, int hop, int bpo);
-void af_cqt_umma_bimage(const float *kappa2, int fftLength, unsigned char *out /* fftLength/128 * 32768 bytes */);
-int af_launch_cqt_octave_umma(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
-                              int padLeft, int timeLength, const unsigned char *bimg, const float *scale, int num, int colOff,
-                              float *outRe, float *outIm, void *stream);
+/* wgmma octave kernel (kernels/cqt_wgmma.cu): Hankel A fragments from the staged signal, B images in swizzled shared
+ * memory; power-of-two hops 2 .. 128 */
+int af_cqt_wgmma_supported(int fftLength, int hop, int bpo);
+void af_cqt_wgmma_bimage(const float *kappa2, int fftLength, unsigned char *out /* fftLength/128 * 32768 bytes */);
+int af_launch_cqt_octave_wgmma(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
+                               int padLeft, int timeLength, const unsigned char *bimg, const float *scale, int num, int colOff,
+                               float *outRe, float *outIm, void *stream);
 
 typedef struct {
     int log2n, num, batch, padLength, dataLength;

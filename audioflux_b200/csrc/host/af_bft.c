@@ -1,5 +1,5 @@
 /* af_bft.c -- BFT object of the C ABI: STFT -> power / magnitude -> filter bank (-> fused MFCC).
- * Interface spec: /root/reference/src/bft_algorithm.h:14-57; behaviour src/bft_algorithm.c:87-276
+ * Interface spec: src/bft_algorithm.h:14-57; behaviour src/bft_algorithm.c:87-276
  * (parameter rules), :397-540 (compute).  Compute = kernels/stft_generic.cu + kernels/bank_xxcc.cu,
  * or kernels/mfcc_fused.cu for the fftLength=2048 MFCC path. */
 #include <math.h>

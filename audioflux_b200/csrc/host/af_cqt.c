@@ -1,5 +1,5 @@
 /* af_cqt.c -- CQT object of the C ABI (host C; compute = kernels/cqt.cu).
- * Interface spec: /root/reference/src/cqt_algorithm.h:14-62; behaviour src/cqt_algorithm.c:110-247
+ * Interface spec: src/cqt_algorithm.h:14-62; behaviour src/cqt_algorithm.c:110-247
  * (parameters), :266-299 (time length), :845-1061 (octave recursion). */
 #include <math.h>
 #include <stdio.h>
@@ -17,7 +17,7 @@ struct OpaqueCQT {
     int devReady;
     void *stream;
     float *dBfrag;                               /* tensor-core octave kernel: pre-split kernel fragments */
-    unsigned char *dBimg;                        /* tcgen05 octave kernel: pre-swizzled shared-memory images of the kernels */
+    unsigned char *dBimg;                        /* wgmma octave kernel: pre-swizzled shared-memory images of the kernels */
     float *dKappa2, *dLeft, *dRight, *dScale;    /* dScale: octaveNum x bpo, rebuilt when isScale flips */
     int scaleDirty;
     AfDevBuf dIn, dSigA, dSigB, dOutRe, dOutIm;
@@ -123,7 +123,7 @@ static int cqt_device(CQTObj c) {
             const size_t nb = (size_t)(c->fftLength / 128) * 32768;
             unsigned char *img = (unsigned char *)malloc(nb * sets);
             if (!img) return AF_ERR_NOMEM;
-            for (int s = 0; s < sets; s++) af_cqt_umma_bimage(c->kappa2 + setFloats * s, c->fftLength, img + nb * s);
+            for (int s = 0; s < sets; s++) af_cqt_wgmma_bimage(c->kappa2 + setFloats * s, c->fftLength, img + nb * s);
             rc = af_dev_upload((void **)&c->dBimg, img, nb * sets);
             free(img);
             if (rc) return rc;
@@ -181,9 +181,9 @@ static int cqt_compute_ex(CQTObj c, const float *dData, int dataLength, int batc
         const unsigned char *bimg = c->dBimg ? c->dBimg + set * (size_t)(c->fftLength / 128) * 32768 : NULL;
         const float *bfrag = c->dBfrag ? c->dBfrag + set * (size_t)(c->fftLength / 8) * 96 * 4 : NULL;
         const float *kappa = c->dKappa2 + set * 2 * (size_t)c->binPerOctave * c->fftLength;
-        /* tcgen05 (default where the hop allows it) > mma.sync 3xTF32 > FP32 loop; AFB200_CQT_KERNEL = mma | fp32 forces the older ones */
-        if (c->dBimg && af_cqt_umma_supported(c->fftLength, hop, c->binPerOctave) && !kq) {
-            if ((rc = af_launch_cqt_octave_umma(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bimg,
+        /* wgmma (default where the hop allows it) > mma.sync 3xTF32 > FP32 loop; AFB200_CQT_KERNEL = mma | fp32 forces the older ones */
+        if (c->dBimg && af_cqt_wgmma_supported(c->fftLength, hop, c->binPerOctave) && !kq) {
+            if ((rc = af_launch_cqt_octave_wgmma(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bimg,
                                                 c->dScale + (size_t)k * c->binPerOctave, c->num, o * c->binPerOctave, dRe, dIm, st))) return rc;
             continue;
         }

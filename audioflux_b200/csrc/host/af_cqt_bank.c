@@ -1,12 +1,12 @@
 /* af_cqt_bank.c -- constant-Q kernels and the fixed /2 decimator taps (setup time, host).
  *
  * Behavioural spec:
- *   bin frequencies   /root/reference/src/filterbank/cqt_filterBank.c:159-184 (float32 running product:
+ *   bin frequencies   src/filterbank/cqt_filterBank.c:159-184 (float32 running product:
  *                     the kernel phase 2*pi*j*f/sr reaches ~250 rad, so a 1-ulp change of f moves
  *                     kernel entries by ~2e-5 -- the float evaluation order is therefore kept)
  *   kernel lengths    :187-244      temporal kernels :253-336      spectral kernels + threshold :57-148
- *   object wiring     /root/reference/src/cqt_algorithm.c:1181-1265
- *   decimator         /root/reference/src/dsp/resample_algorithm.c:60-98 (quality Fast), :430-521, :546-634
+ *   object wiring     src/cqt_algorithm.c:1181-1265
+ *   decimator         src/dsp/resample_algorithm.c:60-98 (quality Fast), :430-521, :546-634
  */
 #include <math.h>
 #include <stdlib.h>

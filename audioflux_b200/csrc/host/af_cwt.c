@@ -1,5 +1,5 @@
 /* af_cwt.c -- CWT object of the C ABI (host C; compute = kernels/cwt.cu).
- * Interface spec: /root/reference/src/cwt_algorithm.h:14-45; behaviour src/cwt_algorithm.c:73-334
+ * Interface spec: src/cwt_algorithm.h:14-45; behaviour src/cwt_algorithm.c:73-334
  * (parameters), :361-483 (compute). */
 #include <math.h>
 #include <stdio.h>

@@ -1,7 +1,7 @@
 /* af_cwt_bank.c -- analytic wavelets in the frequency domain and the scale ladder (setup time, host).
  *
- * Behavioural spec: /root/reference/src/filterbank/cwt_filterBank.c:85-290 (scales, omega grid),
- * :361-640 (psi_hat of each family), /root/reference/src/cwt_algorithm.c:198-244 (family defaults).
+ * Behavioural spec: src/filterbank/cwt_filterBank.c:85-290 (scales, omega grid),
+ * :361-640 (psi_hat of each family), src/cwt_algorithm.c:198-244 (family defaults).
  * The bank is a closed form in s*omega, so the device evaluates `af_wavelet_eval`'s twin on the
  * fly instead of reading a num x N table (176 MB per clip at N = 2^19).
  */

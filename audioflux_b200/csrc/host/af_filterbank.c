@@ -3,9 +3,9 @@
  * Behavioural spec (constants the device kernels consume; every integer outcome -- band-edge
  * bins, supports -- must equal the reference's, so the float32 evaluation order of the
  * published scale formulas is kept):
- *   scales      /root/reference/src/filterbank/auditory_filterBank.c:1023-1190
+ *   scales      src/filterbank/auditory_filterBank.c:1023-1190
  *   band edges  :594-677      range revision :946-1021     bank styles :210-500
- *   range rules /root/reference/src/bft_algorithm.c:158-230, src/cwt_algorithm.c:137-196
+ *   range rules src/bft_algorithm.c:158-230, src/cwt_algorithm.c:137-196
  * Unlike the reference, writes are clipped to the bank's columns (the reference writes out of
  * bounds when a revised edge leaves [0, samplate/2], e.g. Linspace/Log with the default range).
  */
@@ -169,8 +169,8 @@ static void window_half_fill(float *bank, int width, int row, int style, int fro
 
 /* Gammatone bank: magnitude response of Slaney's 4th-order gammatone filter (four cascaded biquads,
  * "An efficient implementation of the Patterson-Holdsworth auditory filter bank", 1993) at the FFT bins.
- * Behavioural spec: /root/reference/src/filterbank/auditory_filterBank.c:509-591 (bank, norms, x2 interior),
- * :691-924 (coefficients), /root/reference/src/dsp/filterDesign_freqz.c:8-118 (response on
+ * Behavioural spec: src/filterbank/auditory_filterBank.c:509-591 (bank, norms, x2 interior),
+ * :691-924 (coefficients), src/dsp/filterDesign_freqz.c:8-118 (response on
  * omega = linspace(0, 2 pi - 2 pi/n, n)[0 .. n/2]).
  * The lowest bands (centre frequency below ~100 Hz) are numerically degenerate: the gain and the biquad
  * responses lose most of their float32 digits to cancellation, and the reference's values there are what a

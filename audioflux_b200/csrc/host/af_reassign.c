@@ -1,5 +1,5 @@
 /* af_reassign.c -- ReassignObj of the C ABI (host C; compute = kernels/stft_generic.cu x 3 + kernels/reassign.cu).
- * Interface spec: /root/reference/src/reassign_algorithm.h:26-55; behaviour src/reassign_algorithm.c:83-451, 587-822.
+ * Interface spec: src/reassign_algorithm.h:26-55; behaviour src/reassign_algorithm.c:83-451, 587-822.
  * Three STFTs of the clip -- window h, its wrapped central difference dh and the ramp-weighted t.h -- give per cell the
  * reassigned frequency f - Im(S_dh / S_h) sr / 2 pi and time t + Re(S_th / S_h) / sr; cells are rounded to the grid and
  * the sign-alternated S_h is scatter-added.  Cell indices are integer outcomes of float32 divides: a cell within an ulp

@@ -1,5 +1,5 @@
 /* af_spectrogram.c -- SpectrogramObj front door of the C ABI (host C).
- * Interface spec: /root/reference/src/spectrogram_algorithm.h:40-119; behaviour
+ * Interface spec: src/spectrogram_algorithm.h:40-119; behaviour
  * src/spectrogram_algorithm.c:326-583 (parameters), :584-791 (tables), :864-1395 (spectrogram), :1409-1525 (xxcc).
  * For the scale types on the time-frequency path the spectrogram is mathematically bftObj_bft in real mode, so
  * the object owns a BFT core (same kernels, including the fused MFCC kernel) and only restates the reference's

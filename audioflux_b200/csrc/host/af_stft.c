@@ -1,5 +1,5 @@
 /* af_stft.c -- STFT object of the C ABI (host C; compute = kernels/stft_generic.cu).
- * Interface spec: /root/reference/src/stft_algorithm.h:14-40, behaviour src/stft_algorithm.c. */
+ * Interface spec: src/stft_algorithm.h:14-40, behaviour src/stft_algorithm.c. */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -1,6 +1,6 @@
 /* af_window.c -- FFT analysis windows (setup time, host).
  *
- * Behavioural spec: /root/reference/src/dsp/flux_window.c:890-940 (`window_calFFTWindow`):
+ * Behavioural spec: src/dsp/flux_window.c:890-940 (`window_calFFTWindow`):
  * "periodic" = symmetric window of length n+1 with the last sample dropped, except
  * Bartlett / Triang / Bartlett-Hann / Bohman which stay symmetric.  Formulas are the textbook
  * ones, evaluated in double and rounded once to float (the reference evaluates in float; the

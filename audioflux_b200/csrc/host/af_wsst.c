@@ -1,6 +1,6 @@
 /* af_wsst.c -- synchrosqueezing objects of the C ABI: WSSTObj (wavelet synchrosqueezed transform) and SynsqObj
  * (phase-difference synchrosqueezing of any time-frequency matrix).
- * Interface spec: /root/reference/src/wsst_algorithm.h:12-49, src/synsq_algorithm.h:12-33; behaviour
+ * Interface spec: src/wsst_algorithm.h:12-49, src/synsq_algorithm.h:12-33; behaviour
  * src/wsst_algorithm.c:64-352 and src/synsq_algorithm.c:38-300.  Compute = the CWT core (kernels/cwt.cu: W and the
  * derivative transform W' from one forward spectrum) + kernels/squeeze.cu (frequency index, row scatter).
  * Row indices are integer outcomes of float32 transcendental math (log2f / atan2f): cells whose value sits within a

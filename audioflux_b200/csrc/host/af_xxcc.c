@@ -1,5 +1,5 @@
 /* af_xxcc.c -- XXCC object of the C ABI (host C; compute = kernels/bank_xxcc.cu `k_xxcc`).
- * Interface spec: /root/reference/src/feature/xxcc_algorithm.h:12-39, behaviour src/feature/xxcc_algorithm.c. */
+ * Interface spec: src/feature/xxcc_algorithm.h:12-39, behaviour src/feature/xxcc_algorithm.c. */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>

@@ -1,7 +1,7 @@
-// c64.cuh -- complex fp32 values packed in one 64-bit register pair, operated on with the
-// sm_100 packed-fp32 instructions (PTX add/sub/mul/fma.rn.f32x2 -> SASS FADD2 / FMUL2 / FFMA2).
-// ptxas folds the half swaps / sign flips below into operand modifiers (.LO_HI, .NP), so a complex
-// add is one instruction and a complex multiply by a constant is two.
+// c64.cuh -- complex fp32 values packed in one 64-bit register pair.  sm_90 has no packed-fp32 instructions, so each
+// helper is two scalar IEEE operations with explicit rounding (__fadd_rn / __fmul_rn / __fmaf_rn): the compiler may
+// not contract a separate multiply and add into an FMA, so every result is the one the element-wise (re, im) arithmetic
+// below defines, bit for bit.
 #pragma once
 #include <stdint.h>
 
@@ -13,10 +13,22 @@ __device__ __forceinline__ c64 c_from(float2 v) { return c_pack(v.x, v.y); }
 __device__ __forceinline__ float c_re(c64 v) { float a, b; c_unpack(v, a, b); return a; }
 __device__ __forceinline__ float c_im(c64 v) { float a, b; c_unpack(v, a, b); return b; }
 
-__device__ __forceinline__ c64 c_add(c64 a, c64 b) { c64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ c64 c_sub(c64 a, c64 b) { c64 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ c64 v_mul(c64 a, c64 b) { c64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }   // element-wise
-__device__ __forceinline__ c64 v_fma(c64 a, c64 b, c64 c) { c64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+__device__ __forceinline__ c64 c_add(c64 a, c64 b) {
+    float ar, ai, br, bi; c_unpack(a, ar, ai); c_unpack(b, br, bi);
+    return c_pack(__fadd_rn(ar, br), __fadd_rn(ai, bi));
+}
+__device__ __forceinline__ c64 c_sub(c64 a, c64 b) {
+    float ar, ai, br, bi; c_unpack(a, ar, ai); c_unpack(b, br, bi);
+    return c_pack(__fsub_rn(ar, br), __fsub_rn(ai, bi));
+}
+__device__ __forceinline__ c64 v_mul(c64 a, c64 b) {     // element-wise
+    float ar, ai, br, bi; c_unpack(a, ar, ai); c_unpack(b, br, bi);
+    return c_pack(__fmul_rn(ar, br), __fmul_rn(ai, bi));
+}
+__device__ __forceinline__ c64 v_fma(c64 a, c64 b, c64 c) {
+    float ar, ai, br, bi, cr, ci; c_unpack(a, ar, ai); c_unpack(b, br, bi); c_unpack(c, cr, ci);
+    return c_pack(__fmaf_rn(ar, br, cr), __fmaf_rn(ai, bi, ci));
+}
 
 __device__ __forceinline__ c64 c_swap(c64 v) { float a, b; c_unpack(v, a, b); return c_pack(b, a); }
 __device__ __forceinline__ c64 c_conj(c64 v) { float a, b; c_unpack(v, a, b); return c_pack(a, -b); }

@@ -1,4 +1,4 @@
-// common.cuh -- small device/host helpers shared by the kernels (sm_100a only).
+// common.cuh -- small device/host helpers shared by the kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

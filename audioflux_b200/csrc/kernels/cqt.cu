@@ -5,7 +5,7 @@
 //   rect window and centre zero padding (src/stft_algorithm.c:601-694) ; compaction ; `__mcdot1` of the
 //   half spectrum with the thresholded spectral kernels ; scaling (:972-989, 1020-1041).
 //
-// B200-first restatement: for a real frame x, sum_k X[k] K_b[k] == sum_n x[n] kappa_b[n] with
+// GPU restatement: for a real frame x, sum_k X[k] K_b[k] == sum_n x[n] kappa_b[n] with
 // kappa_b = DFT of the (thresholded, half-spectrum) kernel row, so one octave is a strided complex
 // correlation  out[t][b] = sum_n xpad[t*hop + n] * kappa_b[n]  -- dense FP32 FMA work on data that
 // stays in shared memory, with no per-frame FFT, no T x 512 spectra in HBM and no compaction pass.
@@ -31,7 +31,7 @@ __device__ __forceinline__ int dec_slot(int i) { return i + 4 * (i >> 5); }
 // out[i] = (sum_{j<32} L[j] x[2i-j] + sum_{j<31} R[j] x[2i+1+j]) / sqrt(1/2), zero outside the clip: a 64-tap FIR
 // h[k] over the window x[2i-32+k] (h[0] = 0, h[32-j] = L[j], h[33+j] = R[j] = c_decTaps[32+j]).  Each thread keeps an 80-sample window in
 // registers (20 LDS.128) and produces 8 outputs; the taps are consumed as (even, odd) PAIRS against the aligned sample
-// pairs of the window with packed fp32x2 FMAs -- 32 FFMA2 per output, the two halves of the accumulator added at the end.
+// pairs of the window with (even, odd) pair FMAs (c64.cuh) -- 32 per output, the two halves of the accumulator added at the end.
 __global__ void __launch_bounds__(kDecThreads, 2) k_decimate2(const float *__restrict__ in, int inLength, long long inStride,
                                                               float *__restrict__ out, long long outStride) {
     __shared__ __align__(16) float sx[kDecSpan + 4 * (kDecSpan / 32) + 8];
@@ -80,8 +80,7 @@ __global__ void __launch_bounds__(kDecThreads, 2) k_decimate2(const float *__res
     for (int q = 0; q < kDecPer; q++) acc[q] = 0ull;
 #pragma unroll
     for (int u = 0; u < 32; u++) {
-        const c64 h = reinterpret_cast<const c64 *>(sh)[u];   // (h[2u], h[2u+1]): vector registers, so the FFMA2 take no
-                                                              // uniform-register operands (those cost two UMOV each)
+        const c64 h = reinterpret_cast<const c64 *>(sh)[u];   // (h[2u], h[2u+1])
 #pragma unroll
         for (int q = 0; q < kDecPer; q++) acc[q] = v_fma(h, w[q + u], acc[q]);
     }
@@ -139,8 +138,8 @@ __global__ void k_cqt_octave(OctParams p) {
     const int span = (p.TT - 1) * h + N;
     const long long m0 = (long long)t0 * h - p.padLeft;      // signal index of padded position t0*h
     // (4 independent loads in flight per thread: at the top octave the staging moves 3x more data per MAC than
-    //  lower down and was load-latency bound, 28 % of that launch's stall samples; hop is a power of two in every
-    //  default configuration, then the polyphase split is a shift and a mask)
+    //  lower down and is load-latency bound; hop is a power of two in every default configuration, then the
+    //  polyphase split is a shift and a mask)
     const int hShift = (h & (h - 1)) == 0 ? __ffs(h) - 1 : -1;
     for (int i0 = threadIdx.x; i0 < span; i0 += 4 * blockDim.x) {
         float v[4];

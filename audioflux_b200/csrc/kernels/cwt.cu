@@ -146,7 +146,7 @@ __device__ __forceinline__ float2 bank_times_spec(const CwtParams &p, float s, i
     if (k <= p.N / 2) {
         // omega_k = float(2 pi k / N) as the reference tabulates it (double product, rounded once): k * (hi + lo) with
         // hi + lo = 2 pi / N split into two floats gives the same value without the int->double->float conversion chain
-        // and FP64 multiplies per element (measured: 29 % of the columns kernel's stall samples sat on them)
+        // and FP64 multiplies per element
         omega = fmaf((float)k, p.omegaHi, (float)k * p.omegaLo);
         if (p.bankTable) wv = k < p.bankWidth ? p.bankTable[(size_t)sIdx * p.bankWidth + k] : 0.0f;   // pwtObj_pwt
         else wv = wavelet_eval(p.wType, p.g, p.b, p.factor, s * omega);
@@ -255,7 +255,7 @@ __global__ void k_cwt_rows(CwtParams p) {
 
 // ---- support of every bank row: bins [lo, hi) where psi_hat(s omega_k) exceeds 2^-28 of the row's peak.  Outside, the
 // fast path treats the row as zero (relative error <= 4e-9, far inside the 1e-4 tolerance): low scales touch a sliver of
-// the spectrum, and loading / evaluating the wavelet over all N/2 bins was 27 % of the fused kernel's time (ncu r2).
+// the spectrum, and loading / evaluating the wavelet over all N/2 bins would dominate their columns units.
 __device__ __forceinline__ float bank_value(const CwtParams &p, int sIdx, int k) {
     if (p.bankTable) return k < p.bankWidth ? fabsf(p.bankTable[(size_t)sIdx * p.bankWidth + k]) : 0.0f;
     const float omega = fmaf((float)k, p.omegaHi, (float)k * p.omegaLo);
@@ -278,7 +278,7 @@ __global__ void k_cwt_support_range(CwtParams p, const unsigned *peakBits, int *
 
 // ============================================================================================
 // Fast path for N = 2^19 (BASELINE config 4): N1 = 1024 columns leg, N2 = 512 rows leg, every
-// transform done by ONE WARP in registers (generated packed-fp32 32/16-point DFTs, warp-private
+// transform done by ONE WARP in registers (generated 32/16-point DFTs on (re, im) register pairs, warp-private
 // shared-memory transposes, __syncwarp only) -- the CTA synchronises three times instead of once per
 // radix pass, and 2-3 CTAs share an SM so the load / transform / store phases of different CTAs overlap.
 // Both directions run the forward transform; the inverse is conj . DFT . conj with the conjugations
@@ -292,8 +292,7 @@ constexpr int kWRowPitch = 520;       // c64 per row slot
 // warps walk ALONG one slot.  The slot pitches are multiples of 16 c64 (the float transpose planes inside a slot
 // rely on it), so the across-walk would hit one 8-byte bank pair 8 times; XOR-ing the low index bits with the slot
 // number makes it conflict-free and leaves the along-walk (16 consecutive entries of one slot) a permutation of the
-// same 128 bytes.  (ncu before: 66 % / 59 % of the shared wavefronts of the two kernels were conflict replays; the
-// kernels are latency-bound though, so this bought only 1.4 %.)
+// same 128 bytes.
 __device__ __forceinline__ int wcol_idx(int c, int i) { return c * kWColPitch + (i ^ (2 * c)); }
 __device__ __forceinline__ int wrow_idx(int r, int k) { return r * kWRowPitch + (k ^ (r & 15)); }
 
@@ -391,8 +390,8 @@ __device__ void cwt_cols_w_unit(const CwtParams &p, c64 *tile, const float2 *tw1
         const int col = col0 + warp;
         // inter-leg twiddle W_N^(col k1), k1 = lane + 32 kb: W_N^(col lane) . (W_N^(32 col))^kb.  Two table products per lane
         // (W_N^j = W_1024^(j / N2) . W_N^(j % N2)) and a running product over kb in groups of 8, re-anchored at kb = 0, 8, 16, 24
-        // by exact table values: 10 table look-ups per lane instead of 64 (ncu r2: 10.4 % of the kernel sat on them), and at
-        // most 7 chained float products (relative error < 1e-6).
+        // by exact table values: 10 table look-ups per lane instead of 64, and at most 7 chained float products (relative
+        // error < 1e-6).
         auto wN = [&](int j) { return c_mul(c_from(t1k[(j >> p.log2N2) & 1023]), c_from(tf[j & (N2 - 1)])); };
         const c64 step = N2 > 1 ? wN((32 * col) & (p.N - 1)) : c_pack(1.0f, 0.0f);
 #pragma unroll
@@ -522,9 +521,9 @@ __global__ void __launch_bounds__(kWRows * 16) k_cwt_rows_w(CwtParams p) {
 // ============================================================================================
 // Both inverse legs in ONE persistent kernel (N = 2^19 fast path).  The inter-leg buffer of an item (4 MB) used to be
 // written by a columns launch over ALL items of the chunk and read back by a rows launch: 352 MB per clip to HBM and
-// back (ncu r1: 1036 MB of DRAM traffic per clip for 354 MB of results).  Here the (clip, scale) items are taken in
+// back, about three times the 354 MB of results per clip.  Here the (clip, scale) items are taken in
 // groups of `groupItems`; a group's inter-leg data lives in one slot of a small ring (kRing slots, tens of MB: it stays
-// in the 126 MB L2), the rows units of group g are queued right behind the columns units of group g + 1, and a slot is
+// in the 50 MB L2), the rows units of group g are queued right behind the columns units of group g + 1, and a slot is
 // rewritten -- in L2, before its dirty lines are ever evicted -- as soon as the rows units of its previous group are
 // done.  CTAs claim units from one global counter; two per-group counters carry the dependencies (columns done -> rows
 // may start; rows done -> the slot may be reused).  Unit order guarantees progress: whatever a unit waits for was
@@ -648,7 +647,7 @@ static int cwt_fused_enabled(const AfCwtArgs *a) {
 static int cwt_group_items(void) {
     const char *e = getenv("AFB200_CWT_GROUP");
     const int g = e ? atoi(e) : 0;
-    return g > 0 && g <= 64 ? g : 4;                     // 3 slots x 4 items x 4 MB = 48 MB of the 126 MB L2 (sweep r2: 4 > 3 > 6 > 8 > 2)
+    return g > 0 && g <= 64 ? g : 2;                     // 3 slots x 2 items x 4 MB = 24 MB: half of the 50 MB L2 of an H100
 }
 
 // workspace = forward spectrum (batch x N float2) + inter-leg buffer: batch x num x N float2 when N > 4096, or -- fused
@@ -720,11 +719,10 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
             const size_t smF = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (2048 + p.N2 + 512);
             if ((rc = set_smem(k_cwt_fused_w, smF, "smem k_cwt_fused_w"))) return rc;
             int sms = af_sm_count();
-            if (sms <= 0) sms = 148;
-            // Optional (AFB200_CWT_L2PERSIST=1): pin the ring in L2 with a persisting access-policy window on this stream.  Measured
-            // (r2, 8 clips): DRAM writes drop from 415 to 348 MB / clip (= the compulsory 352 MB) but the kernel gets 10 % SLOWER
-            // (0.39 vs 0.354 ms / clip: the set-aside takes L2 away from the spectrum reads and the result stores), so the default is
-            // off: streaming result stores + a 48 MB ring already keep the traffic at 1.17x compulsory.
+            if (sms <= 0) sms = 132;
+            // Optional (AFB200_CWT_L2PERSIST=1): pin the ring in L2 with a persisting access-policy window on this stream.  The
+            // set-aside takes L2 away from the spectrum reads and the result stores, so the default is off: streaming result
+            // stores already keep the ring's lines in L2 for most of their life.
             const char *pe = getenv("AFB200_CWT_L2PERSIST");
             const bool persist = pe && pe[0] == '1';
             const size_t ringBytes = sizeof(float2) * (size_t)p.N * kRing * f.groupItems;

@@ -15,7 +15,7 @@
 //     double buffered through a full/empty mbarrier ring fed by a dedicated producer warp;
 //   * the 2048 real samples are packed as 1024 complex points and transformed as 32 x 32:
 //     lane n1 holds z[n1 + 32*n2] in registers (one complex value per 64-bit register pair, all
-//     butterflies in packed FADD2/FMUL2/FFMA2), a generated straight-line 32-point DFT runs over n2,
+//     butterflies on (re, im) register pairs, c64.cuh), a generated straight-line 32-point DFT runs over n2,
 //     twiddles W_1024^(n1*k) come half from a conflict-free transposed shared table and half from one
 //     extra multiply by W_64^n1, a 33-padded shared transpose regroups the data (warp-private,
 //     __syncwarp only), a second 32-point DFT runs over n1;  lane l then holds Z[l + 32*kb];
@@ -41,7 +41,7 @@ constexpr int kNC = 1024;           // packed complex points
 #ifndef AF_FRAME_WARPS
 #define AF_FRAME_WARPS 13
 #endif
-constexpr int kFrameWarps = AF_FRAME_WARPS;     // consumer warps = max frames per tile (<= 16: one mma M tile); 13 measured best (tools/sweep_frame_warps.sh)
+constexpr int kFrameWarps = AF_FRAME_WARPS;     // consumer warps = max frames per tile (<= 16: one mma M tile); 13 by default
 #ifndef AF_ABLATE
 #define AF_ABLATE 0     // diagnostic timing builds: 1 no bank loop, 2 no post-pass, 4 no FFTs, 8 no transposes, 16 no window/sample loads
 #endif
@@ -62,8 +62,8 @@ constexpr int kStages = 2;
 #ifndef AF_LBUFS
 #define AF_LBUFS 3
 #endif
-constexpr int kLBufs = AF_LBUFS;    // log-mel tiles in flight between the frame warps and the DCT epilogue (2 measured 4 % of
-                                    // frame-warp time waiting for the epilogue, profiles/r1_final_hotspots.txt)
+constexpr int kLBufs = AF_LBUFS;    // log-mel tiles in flight between the frame warps and the DCT epilogue (2 leaves frame
+                                    // warps waiting for the epilogue)
 constexpr int kMaxNum = 128;        // filters (padded)
 constexpr int kScratchFloats = 1152;            // per warp: 33x32 float transpose plane, later Ps[0..1024] + zero pad
 constexpr int kPsPad = 1152;        // Ps[0..1024], zeros up to kPsPad (padded band reads)
@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
             // C fragment: rows g and g+8, columns n*8 + 2t, +1.  Destination 0 is this GPU's buffer, 1..nPeer the
             // peers' (the all-gather of the result rides on the epilogue, tile by tile).  The tile is a contiguous run of
             // nf * ccNum floats in every destination: it is staged in shared memory and leaves as ONE TMA bulk store per
-            // destination (full lines over NVLink; r1 wrote 32-bit scalars, 0.85 scaling efficiency at 8 GPUs).
+            // destination (full lines over NVLink rather than 32-bit scalars).
             const long long tileOff = ((long long)clip * p.timeLength + f0) * p.ccNum;
             if (p.bulkStore) {
                 float *stage = reinterpret_cast<float *>(smem + L.stageOff + epi * kStageBytes);
@@ -483,7 +483,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
                 float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f, acc3 = 0.0f;
                 // software pipelined: the loads of stage i+1 are in flight while stage i is accumulated
                 // (the final prefetch over-reads one stage: the tables carry the padding).  A two-stage-deep
-                // pipeline was measured slower (1.93 vs 1.78 ms: 128 registers, longer prologue per group).
+                // pipeline needs 128 registers and a longer prologue per group.
                 float4 w = wg4[0];
                 float2 p0 = ps2[0], p1 = ps2[1];
 #pragma unroll 2
@@ -695,10 +695,9 @@ extern "C" int af_mfcc_plan_build(void **planOut, int fftLength, int num, int cc
     pl->melGroups = (num + 31) / 32;
     int starts[kMaxNum];
     Intervals *iv = static_cast<Intervals *>(malloc(sizeof(Intervals)));
-    // The interval loop is opt-in (AFB200_MFCC_BANK_MODE=1): it halves the bank loop's shared-memory traffic, but on
-    // B200 it measured SLOWER (2.01 ms vs 1.78 ms at config 2, profiles/r1_bankmode_ablation.txt): the kernel is bound by
-    // the latency of queued MIO operations per warp, and the interval form adds a serial tail (warp reduction of the
-    // last interval + neighbour exchange by shuffles, 0.29 ms) that outweighs the shorter loop (0.43 vs 0.49 ms).
+    // The interval loop is opt-in (AFB200_MFCC_BANK_MODE=1): it halves the bank loop's shared-memory traffic, but the
+    // kernel is bound by the latency of queued MIO operations per warp, and the interval form adds a serial tail (warp
+    // reduction of the last interval + neighbour exchange by shuffles) that can outweigh the shorter loop.
     const char *force = getenv("AFB200_MFCC_BANK_MODE");
     float ones[kMaxNum];
     for (int m = 0; m < kMaxNum; m++) ones[m] = 1.0f;
@@ -818,7 +817,7 @@ static int launch_fused(void *plan, const float *data, int dataLength, int batch
     const int smemBytes = carve(p.spanFloats, pl->melWFloats, pl->ct).total;
 
     int sms = af_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     long long grid = p.totalTiles < (long long)sms * kCtasPerSm ? p.totalTiles : (long long)sms * kCtasPerSm;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaSuccess;

@@ -7,7 +7,7 @@
 //   -> __mcsquare / sqrtf (src/bft_algorithm.c:489-497) -> __mdot1 (:515-518, src/vector/flux_vector.c:55-86)
 //   -> log10f clamp / powf(1/3) (src/feature/xxcc_algorithm.c:124-140) -> fftObj_dct (:142-149) -> cut (:151-155)
 //
-// What changed against v1 (profiles/r1_final_hotspots.txt: bank loop 28 %, post-pass shuffles 15 % of frame-warp time):
+// What changed against v1 (whose frame warps spend most of their time in the bank loop and the post-pass shuffles):
 //  * the real 2048-point FFT is split as 64 (real, in registers) x 32 (complex, in registers): lane n2 transforms the
 //    64 real samples x[32 n1 + n2] (packed complex 32-point DFT + an IN-LANE post-pass, compile-time twiddles), the
 //    columns k1 = 1..31 are twiddled, transposed through shared memory and transformed again; lane k1 then holds the
@@ -19,7 +19,7 @@
 //  * the filter bank is applied per TILE by the helper warps, not per frame by the frame warps: the power spectra of
 //    the tile's frames sit in shared memory as [bin pair][frame], lane = frame, and every bin pair is multiplied
 //    ONCE for the two filters that overlap on it (interval form: rising slope of filter i, falling slope of filter
-//    i-1, the reference's own float weights, no re-normalisation) with packed FFMA2.  The intervals are cut into PIECES of
+//    i-1, the reference's own float weights, no re-normalisation) with two FMAs per lane.  The intervals are cut into PIECES of
 //    at most Lmax bin pairs (host-planned, Lmax = 3 for the 128-band mel bank) so that the 128 helper lanes carry equal
 //    work (the longest interval is 15 pairs, the mean 4.5); a piece's partial sums go into a slot that ALIASES the power
 //    tile rows its pass has finished reading, and are added up per band in a fixed order (bit-stable);
@@ -281,7 +281,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             if (!p.rawMel) wait_cls<2>(&lEmpty[lbuf], ((uint32_t)(it >> 1) & 1u) ^ 1u);    // DCT done with tile it - 2
             // ---- phase 1: ONE PIECE (<= Lmax bin pairs of one interval) PER LANE AND PASS, all frames of the tile in
             // registers: one LDS.128 of weights (rise of filter i, fall of filter i-1) and, per frame, one LDS.64 of the
-            // power pair + two FFMA2 -- kFW independent accumulator chains per lane.  Pass 0 walks the low rows of the
+            // power pair + two complex-pair FMAs -- kFW independent accumulator chains per lane.  Pass 0 walks the low rows of the
             // power tile, pass 1 the rest; once every helper warp is through a pass the rows it read are dead and take
             // the pieces' partial sums S[piece][frame] = (rise part, fall part), piece index = row index.
             c64 *sS = reinterpret_cast<c64 *>(sP);
@@ -877,7 +877,7 @@ static int launch_fused2(void *plan, const float *data, int dataLength, int batc
     pp->totalTiles = (unsigned)((long long)pp->tilesPerClip * batch);
 
     int sms = af_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     const long long grid = (long long)pp->totalTiles < (long long)sms ? (long long)pp->totalTiles : (long long)sms;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaSuccess;

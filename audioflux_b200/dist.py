@@ -54,7 +54,7 @@ def mfcc_sharded(bft, clips, cc_num=13, rectify_type=0, total=None, group=None, 
 
 class OverlappedGather:
     """Chunked compute + all-gather with the collective of chunk k running on a side stream while chunk k+1
-    is being transformed (SURVEY.md section 8e: the gather costs the same order as the compute at B200 speed).
+    is being transformed (SURVEY.md section 8e: the gather costs the same order as the compute at this library's speed).
 
     out[k] is the gathered (world * B_chunk, T, cc) block of chunk k: rank r's clips of that chunk sit at rows
     [r * B_chunk, (r + 1) * B_chunk).  Buffers are allocated once and reused, so steady-state steps allocate nothing."""

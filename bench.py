@@ -1,18 +1,24 @@
 #!/usr/bin/env python3
-"""bench.py -- MFCC frames/s (48 kHz, n_fft=2048, hop=512, 128 mel, 40 coefficients) on N B200s.
+"""bench.py -- MFCC frames/s (48 kHz, n_fft=2048, hop=512, 128 mel, 40 coefficients) on N H100s.
 
-Contract (see the task statement / DESIGN.md section 6):
+Usage (DESIGN.md section 6):
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank per GPU)
   python bench.py --impl reference ...                     (the reference's own CPU path, oracle/_ref)
+  python bench.py ... --dump-outputs DIR                   (N=1: also write what the last timed step computed, as .npy)
 One JSON line on stdout from rank 0.
 
 A "step" is one pass of the fused STFT->mel->log->DCT path over one synthetic batch:
-  N=1 : BASELINE config 2 = 1024 clips x 5 s (983 MB of samples, larger than the 126 MB L2).
+  N=1 : BASELINE config 2 = 1024 clips x 5 s (983 MB of samples, larger than the 50 MB L2).
   N>1 : the same 1024 clips PER GPU (weak scaling, config 5 at N=8) with the all-gather of the (1024, 465, 40)
         result blocks -- the path's only exchange step -- fused into the kernel epilogue as NVLink P2P stores
         (--gather peer, default) or done by NCCL on a side stream (--gather nccl).
 `value` is device-timed (CUDA events on the launching stream) with inputs resident in HBM;
 `e2e` goes through the public call with pinned HOST buffers, H2D and D2H inside the timed region.
+--steps sets the number of timed steps of the MFCC, CQT and CWT device-timed loops, of the MFCC and CQT e2e loops and of
+the reference arm.  The CWT e2e figure is a sample instead: AFB200_CWT_E2E_CHUNKS (default 8) of the 32 chunks of one step,
+each of which moves 5.6 GB of planes to the host.
+Inputs come from fixed seeds, so two builds given the same arguments see the same samples and their
+--dump-outputs files can be compared array for array.
 """
 import argparse
 import json
@@ -53,22 +59,26 @@ FLOP_PER_FRAME = 75e3
 CQT_BATCH, CQT_NUM = 1024, 84
 CWT_BATCH, CWT_NUM, CWT_RADIX, CWT_SAMPLES = 512, 84, 19, SR * 10      # 10 s = 480 000 samples, zero-padded to 2^19
 
+# --dump-outputs: at most this many bytes in all; larger outputs are dumped as a fixed, seeded sample
+DUMP_SEED = 20240611
 
-def ncu_traffic(summary_name):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch, parsed from a committed ncu summary under profiles/
-    (Mbyte / Gbyte units as ncu prints them); None when the file or the two metrics are missing."""
-    path = os.path.join(ROOT, "profiles", summary_name)
-    try:
-        tot, seen = 0.0, 0
-        for line in open(path):
-            f = line.split()
-            if len(f) >= 3 and f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[f[2]]
-                tot += float(f[1]) * unit
-                seen += 1
-        return int(tot) if seen == 2 else None
-    except Exception:
-        return None
+
+def dump_array(dirpath, name, arr):
+    """one output array as DIR/<name>.npy: float64 stays float64 (large indices), everything else becomes float32"""
+    if dirpath is None:
+        return 0
+    os.makedirs(dirpath, exist_ok=True)
+    arr = np.asarray(arr)
+    a = np.ascontiguousarray(arr, dtype=np.float64 if arr.dtype == np.float64 else np.float32)
+    np.save(os.path.join(dirpath, name + ".npy"), a)
+    return a.nbytes
+
+
+def seeded_rows(n, k, salt):
+    """k of n row indices (sorted), the same for every run"""
+    if k >= n:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(DUMP_SEED + salt).choice(n, size=k, replace=False))
 
 
 def measured_peaks():
@@ -78,7 +88,7 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"    # H100 SXM data sheet (700 W)
 
 
 class ClockSampler:
@@ -351,7 +361,7 @@ def run_reference_arm(args):
     per = max(2, int(os.environ.get("AFB200_CPU_CLIPS_PER_WORKER", "16")))
     vals, runs = [], []
     t_all = time.perf_counter()
-    for _ in range(max(1, min(args.steps, 3))):
+    for _ in range(args.steps):
         r = cpu_reference_rate(per, cores)
         if r is None:
             emit({"impl": "reference", "unavailable": "oracle/_ref/libaudioflux_ref.so not built"})
@@ -365,7 +375,7 @@ def run_reference_arm(args):
         "metric": "mfcc_frames_per_s", "value": v, "unit": "frames/s", "impl": "reference", "n_gpus": args.gpus,
         "steps": len(vals), "warmup": 1, "ms_per_step": 1e3 * frames_step / v, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-        # the B200 arm's workload (same clips, same transform); each reference step is a bounded sample of it
+        # the GPU arm's workload (same clips, same transform); each reference step is a bounded sample of it
         "config": {"workload": f"BASELINE config {'2' if args.gpus == 1 else '5-shaped'}: batch={args.batch} x 5 s 48 kHz clips per GPU, "
                                "STFT(2048,hop 512,hann)->mel128(slaney)->log10->DCT MFCC(40)",
                    "batch_per_gpu": args.batch, "clip_samples": L, "frames_per_clip": T,
@@ -423,8 +433,18 @@ def bench_cqt_c3(dev, peaks, args, cores):
         return {"error": f"CQT parity gate failed: rel err {errs}"}
     del re, im
     n0 = lib.afb200_kernelLaunchCount()
-    ms = _timed_ms(lambda: c.cqt_batch(x), steps=max(3, min(args.steps, 10)), warm=3)
+    last = {}
+
+    def cqt_step():
+        last["out"] = c.cqt_batch(x)
+    ms = _timed_ms(cqt_step, steps=args.steps, warm=3)
     launches = (lib.afb200_kernelLaunchCount() - n0) // (len(ms) + 3)
+    if args.dump_outputs:
+        rows = torch.from_numpy(seeded_rows(B, 16, 3)).to(dev)
+        dump_array(args.dump_outputs, "cqt_re_sample", last["out"][0].index_select(0, rows).cpu().numpy())
+        dump_array(args.dump_outputs, "cqt_im_sample", last["out"][1].index_select(0, rows).cpu().numpy())
+        dump_array(args.dump_outputs, "cqt_sample_clip_index", rows.cpu().numpy())
+    del last
     ms_step = float(np.mean(ms))
     # end to end: the C-ABI call with page-locked HOST buffers (chunked copy-in / transform / copy-out inside)
     xh = torch.empty((B, L), dtype=torch.float32).pin_memory()
@@ -441,7 +461,7 @@ def bench_cqt_c3(dev, peaks, args, cores):
                     C.c_void_p(ih.numpy().ctypes.data), 0, None), "cqtObj_cqtBatch(host)")
     e2e()
     t0 = time.perf_counter()
-    n_e = 3
+    n_e = args.steps
     for _ in range(n_e):
         e2e()
     e2e_s = (time.perf_counter() - t0) / n_e
@@ -505,8 +525,15 @@ def bench_cwt_c4(dev, peaks, args, cores):
     if not err < 1e-4:
         return {"error": f"CWT parity gate failed: rel err {err}"}
     n0 = lib.afb200_kernelLaunchCount()
-    ms = _timed_ms(step, steps=3, warm=1)
-    launches = (lib.afb200_kernelLaunchCount() - n0) // 4
+    ms = _timed_ms(step, steps=args.steps, warm=1)
+    launches = (lib.afb200_kernelLaunchCount() - n0) // (args.steps + 1)
+    if args.dump_outputs:
+        # the last chunk of the last step: a seeded sample of 2^20 (clip, scale, sample) positions of each plane
+        nb = B - (B - 1) // chunk * chunk
+        pos = torch.from_numpy(np.sort(np.random.default_rng(DUMP_SEED + 4).choice(nb * CWT_NUM * N, size=1 << 20, replace=False))).to(dev)
+        dump_array(args.dump_outputs, "cwt_re_sample", re.reshape(-1).index_select(0, pos).cpu().numpy())
+        dump_array(args.dump_outputs, "cwt_im_sample", im.reshape(-1).index_select(0, pos).cpu().numpy())
+        dump_array(args.dump_outputs, "cwt_sample_flat_index", pos.cpu().numpy().astype(np.float64))
     ms_step = float(np.mean(ms))
     # end to end: cwtObj_cwtBatch with HOST pointers, chunk by chunk (inputs from and planes to page-locked host memory)
     xh = torch.empty((chunk, N), dtype=torch.float32).pin_memory()
@@ -525,11 +552,6 @@ def bench_cwt_c4(dev, peaks, args, cores):
     e2e_s_per_clip = (time.perf_counter() - t0) / (n_chunks * chunk)
     bytes_clip = 4 * CWT_SAMPLES + 2 * 4 * CWT_NUM * N
     achieved = B * bytes_clip / (ms_step * 1e-3) / 1e9
-    # DRAM bytes of the dominant kernel (k_cwt_fused_w) from the committed ncu capture: tools/cwt_prof.py transforms 4 clips per
-    # launch, the bench chunk-size clips -- the kernel walks (clip, scale) items in groups of 4, so its traffic scales with the clips
-    cwt_summary, cwt_capture_clips = "r2_final_cwt_ncu.txt", 4
-    t4 = ncu_traffic(cwt_summary)
-    cwt_traffic = int(t4 / cwt_capture_clips * chunk) if t4 else None
     out = {"metric": "cwt_clips_per_s", "value": B / (ms_step * 1e-3), "unit": "clips/s", "ms_per_step": ms_step, "per_step_ms": ms,
            "config": {"workload": f"BASELINE config 4: batch={B} x 10 s 48 kHz clips (480000 samples zero-padded to 2^19), CWT morlet {CWT_NUM} scales (octave)",
                       "chunk_clips": chunk, "output": "two planes of 352 MB per clip; each chunk's planes overwrite one device buffer",
@@ -538,8 +560,7 @@ def bench_cwt_c4(dev, peaks, args, cores):
                    "sample": f"{n_chunks} of the {B // chunk} chunks of a step, each through cwtObj_cwtBatch with HOST pointers"},
            "gpu_launches": int(launches),
            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                        "traffic": cwt_traffic, "traffic_source": f"profiles/{cwt_summary} ({cwt_capture_clips} clips per launch) scaled to the bench's {chunk}-clip launches" if cwt_traffic else None,
-                        "kernel": "k_cwt_fused_w", "algorithmic_bytes_per_launch": chunk * bytes_clip,
+                        "traffic": None, "kernel": "k_cwt_fused_w", "algorithmic_bytes_per_launch": chunk * bytes_clip,
                         "algorithmic_bytes_per_step": B * bytes_clip}}
     del x, re, im
     if not args.no_cpu_baseline:
@@ -552,8 +573,8 @@ def bench_cwt_c4(dev, peaks, args, cores):
     return out
 
 
-# --------------------------------------------------------------------------- B200 arm
-def run_b200_arm(args):
+# --------------------------------------------------------------------------- GPU arm
+def run_gpu_arm(args):
     import torch
     import audioflux_b200 as af
     from audioflux_b200 import lib as L_
@@ -659,8 +680,9 @@ def run_b200_arm(args):
     torch.cuda.synchronize()
     sampler.mark(True)
     ev[0].record()
+    last_out = None
     for i in range(args.steps):
-        step()
+        last_out = step()
         ev[i + 1].record()
     torch.cuda.synchronize()
     sampler.mark(False)
@@ -668,6 +690,12 @@ def run_b200_arm(args):
         dist.barrier()
     launches = lib.afb200_kernelLaunchCount() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0 and world == 1:
+        # (B, T, 40) MFCC of the last timed step: 76 MB at the default batch, so a seeded sample of 256 clips
+        rows = seeded_rows(B, 256, 2)
+        dump_array(args.dump_outputs, "mfcc_sample", last_out.index_select(0, torch.from_numpy(rows).to(dev)).cpu().numpy())
+        dump_array(args.dump_outputs, "mfcc_sample_clip_index", rows)
+    del last_out
     total_ms = ev[0].elapsed_time(ev[-1])
     per_step = [ev[i].elapsed_time(ev[i + 1]) for i in range(args.steps)]
     if world > 1:                      # kernel-only duration for the roofline: one untimed-by-the-metric extra pass
@@ -735,7 +763,7 @@ def run_b200_arm(args):
     if dist:
         dist.barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    n_e2e = max(3, min(args.steps, 10))
+    n_e2e = args.steps
     e0.record()
     for _ in range(n_e2e):
         e2e_step()
@@ -763,12 +791,6 @@ def run_b200_arm(args):
     if world == 1 and not args.no_cpu_baseline:
         cpu = cpu_reference_rate(per_cpu, cores)
     kernel_name = "k_mfcc_fused<5,0>" if os.environ.get("AFB200_MFCC_KERNEL") == "v1" else "k_mfcc_fused2<5>"
-    summary = os.environ.get("AFB200_NCU_SUMMARY", "r1_final_mfcc_fused_ncu_summary.txt" if "fused<" in kernel_name
-                             else "r2_final_mfcc_fused2_ncu_summary.txt")
-    traffic = ncu_traffic(summary) if (B == 1024 and L == 240000) else None
-    if traffic is None and "fused2" in kernel_name and B == 1024 and L == 240000:
-        summary = "r2_mfcc_fused2_ncu_summary.txt"                   # the capture at the start of the round
-        traffic = ncu_traffic(summary)
     line = {
         "metric": "mfcc_frames_per_s", "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
@@ -776,7 +798,7 @@ def run_b200_arm(args):
         "config": {"workload": f"BASELINE config {'2' if world == 1 else '5-shaped'}: batch={B} x 5 s 48 kHz clips per GPU, "
                                "STFT(2048,hop 512,hann)->mel128(slaney)->log10->DCT MFCC(40), fused kernel",
                    "batch_per_gpu": B, "clip_samples": L, "frames_per_clip": T,
-                   "l2": "inputs (983 MB per GPU) exceed the 126 MB L2; no explicit flush needed",
+                   "l2": "inputs (983 MB per GPU) exceed the 50 MB L2; no explicit flush needed",
                    "collective": {"none": "none",
                                   "peer": "fused: the kernel epilogue stores each tile into every rank's gathered (world,B,T,40) array "
                                           "over NVLink P2P (cudaIpc-mapped), then a 4-byte NCCL all-reduce as the cross-rank fence",
@@ -791,9 +813,7 @@ def run_b200_arm(args):
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                      "frac": achieved / peaks["hbm_gbs"],
-                     # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of this kernel at this configuration, parsed at
-                     # run time from the committed ncu --set full summary under profiles/ (None if that file is absent)
-                     "traffic": traffic, "traffic_source": f"profiles/{summary}" if traffic else None, "peak_kind": peak_kind,
+                     "traffic": None, "peak_kind": peak_kind,
                      "kernel": kernel_name, "kernel_ms": kernel_ms, "algorithmic_bytes_per_launch": B * BYTES_PER_CLIP,
                      "frame_read_model_frac": (B * T * BYTES_PER_FRAME_READ_MODEL / (kernel_ms * 1e-3) / 1e9) / peaks["hbm_gbs"],
                      "fp32_tflops": B * T * FLOP_PER_FRAME / (kernel_ms * 1e-3) / 1e12},
@@ -827,17 +847,22 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="gpu", choices=["gpu", "reference"])
     ap.add_argument("--batch", type=int, default=BATCH_PER_GPU, help="clips per GPU (default: BASELINE config 2)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the CQT (config 3) / CWT (config 4) keys")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N=1: write what the last timed step of each workload computed to DIR/<name>.npy (float32; "
+                         "seeded samples of the larger outputs, under 64 MB in all)")
     ap.add_argument("--gather-chunks", type=int, default=4, help="N>1, --gather nccl: chunks per step for compute/all-gather overlap")
     ap.add_argument("--gather", choices=("peer", "nccl"), default="peer",
                     help="N>1: 'peer' = all-gather fused into the kernel epilogue (NVLink P2P stores); 'nccl' = overlapped NCCL all-gather")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference_arm(args)
-    return run_b200_arm(args)
+    return run_gpu_arm(args)
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 /* afb200_bft.h -- BFT object: STFT -> power/magnitude -> mel/bark/erb/... filter bank.
- * Replaces /root/reference/src/bft_algorithm.h:14-57 (implementation src/bft_algorithm.c). */
+ * Replaces src/bft_algorithm.h:14-57 (implementation src/bft_algorithm.c). */
 #ifndef AFB200_BFT_H
 #define AFB200_BFT_H
 #include "afb200_types.h"

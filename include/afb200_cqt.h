@@ -1,4 +1,4 @@
-/* afb200_cqt.h -- constant-Q transform.  Replaces /root/reference/src/cqt_algorithm.h:14-62
+/* afb200_cqt.h -- constant-Q transform.  Replaces src/cqt_algorithm.h:14-62
  * (src/cqt_algorithm.c).   */
 #ifndef AFB200_CQT_H
 #define AFB200_CQT_H

@@ -1,4 +1,4 @@
-/* afb200_cwt.h -- continuous wavelet transform.  Replaces /root/reference/src/cwt_algorithm.h:14-45
+/* afb200_cwt.h -- continuous wavelet transform.  Replaces src/cwt_algorithm.h:14-45
  * (src/cwt_algorithm.c); cwtDet is a "next" row. */
 #ifndef AFB200_CWT_H
 #define AFB200_CWT_H

@@ -1,7 +1,7 @@
 /* afb200_ext.h -- ADDITIVE entry points of libaudioflux_b200.so (no reference counterpart).
  *
  * The reference API is one clip per call with host pointers (python/audioflux/bft.py:349-365
- * loops channels in Python); fed that way a B200 is PCIe/launch bound.  These entry points
+ * loops channels in Python); fed that way a GPU is PCIe/launch bound.  These entry points
  * take a whole batch and either host or device pointers.
  *
  *   memKind 0: host pointers (pageable or pinned) -- copies + sync happen inside the call.

@@ -1,5 +1,5 @@
 /* afb200_pwt.h -- pseudo wavelet transform: FFT -> auditory filter bank x spectrum -> IFFT per band.
- * Replaces /root/reference/src/pwt_algorithm.h:16-31 (src/pwt_algorithm.c). */
+ * Replaces src/pwt_algorithm.h:16-31 (src/pwt_algorithm.c). */
 #ifndef AFB200_PWT_H
 #define AFB200_PWT_H
 #include "afb200_types.h"

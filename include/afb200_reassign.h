@@ -1,4 +1,4 @@
-/* afb200_reassign.h -- time-frequency reassignment object: drop-in for /root/reference/src/reassign_algorithm.h:26-55
+/* afb200_reassign.h -- time-frequency reassignment object: drop-in for src/reassign_algorithm.h:26-55
  * (same names, argument meaning and defaults). */
 #ifndef AFB200_REASSIGN_H
 #define AFB200_REASSIGN_H

@@ -1,6 +1,6 @@
 /* afb200_spectrogram.h -- SpectrogramObj: the reference's general spectrogram front door (the class its own
  * benchmark times, benchmark/run_audioflux.py:14-29).  Replaces the part of
- * /root/reference/src/spectrogram_algorithm.h:40-119 that lies on the time-frequency path:
+ * src/spectrogram_algorithm.h:40-119 that lies on the time-frequency path:
  * construction, spectrogram (STFT -> power/magnitude -> Linear slice or mel/bark/erb/... bank) and the cepstral
  * calls and the cepstral deconvolution.  Chroma / Deep scale types and the spectral-descriptor functions (flatness,
  * centroid, ...) are outside the path: `_new` rejects those scale types with -2, the functions are not exported. */

@@ -1,4 +1,4 @@
-/* afb200_stft.h -- framed STFT object.  Replaces /root/reference/src/stft_algorithm.h:14-40
+/* afb200_stft.h -- framed STFT object.  Replaces src/stft_algorithm.h:14-40
  * (implementation src/stft_algorithm.c).  Host pointers, one clip per call, caller-allocated
  * outputs that are fully overwritten. */
 #ifndef AFB200_STFT_H

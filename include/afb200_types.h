@@ -1,6 +1,6 @@
 /* afb200_types.h -- enum ints of the audioFlux C ABI used by the time-frequency hot path.
  *
- * Replaces: /root/reference/src/flux_base.h:14-168 (same identifiers and values, so native
+ * Replaces: src/flux_base.h:14-168 (same identifiers and values, so native
  * callers compile unchanged and python/audioflux/type/basic.py:25-353 keeps passing the same
  * ints).  Only the enums the hot path consumes are declared.
  */

@@ -1,4 +1,4 @@
-/* afb200_wsst.h -- synchrosqueezing objects: drop-in for /root/reference/src/wsst_algorithm.h:12-49 and
+/* afb200_wsst.h -- synchrosqueezing objects: drop-in for src/wsst_algorithm.h:12-49 and
  * src/synsq_algorithm.h:12-33 (same names, argument meaning and defaults). */
 #ifndef AFB200_WSST_H
 #define AFB200_WSST_H

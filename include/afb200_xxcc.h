@@ -1,5 +1,5 @@
 /* afb200_xxcc.h -- cepstral coefficients (rectify -> ortho DCT-II -> first ccNum).
- * Replaces /root/reference/src/feature/xxcc_algorithm.h:12-39 (src/feature/xxcc_algorithm.c). */
+ * Replaces src/feature/xxcc_algorithm.h:12-39 (src/feature/xxcc_algorithm.c). */
 #ifndef AFB200_XXCC_H
 #define AFB200_XXCC_H
 #include "afb200_types.h"

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE ONLY.  Nothing under ``audioflux_b200/`` may import this
 module; it is the checker used by ``tests/``, ``__graft_entry__.smoke()`` and
 the ``cpu_baseline`` leg of ``bench.py``.
 
-Every function cites the reference file:line (relative to /root/reference) it
+Every function cites the reference file:line (relative to the audioFlux source tree) it
 restates.  Arithmetic is done in float64 unless the reference's float32
 rounding decides an *integer* outcome (band-edge bin indices, kernel lengths),
 in which case the float32 steps are reproduced explicitly.

@@ -1,8 +1,7 @@
 """ctypes handle on the UNMODIFIED reference build in oracle/_ref (test infrastructure only).
 
-The library is produced by `make -C oracle` from /root/reference/src (in the build
-container); it travels to the GPU box as a prebuilt file.  It is never loaded by the
-product package."""
+The library is produced by `make -C oracle REF=<audioFlux tree>` (or by build() when
+the audioFlux tree is present).  It is never loaded by the product package."""
 from __future__ import annotations
 
 import ctypes
@@ -26,7 +25,7 @@ def get_ref_lib(omp: bool = False, asan: bool = False):
     path = REF_ASAN_PATH if asan else REF_OMP_PATH if omp else REF_PATH
     if path not in _cache:
         if not os.path.exists(path):
-            raise FileNotFoundError(f"{path} missing: run `make -C oracle` where /root/reference exists")
+            raise FileNotFoundError(f"{path} missing: run `make -C oracle REF=<audioFlux tree>`")
         lib = ctypes.CDLL(path)
         capi.bind(lib)
         _cache[path] = lib

@@ -34,7 +34,7 @@ def load(default_lib: str, b200_lib: str):
     if "mod" in _state:
         return _state["mod"]
     if not available():
-        raise FileNotFoundError(f"{PYREF} missing: run `make -C oracle` where /root/reference exists")
+        raise FileNotFoundError(f"{PYREF} missing: run `make -C oracle REF=<audioFlux tree>`")
     tmp = tempfile.mkdtemp(prefix="af_pyref_")
     pkg = os.path.join(tmp, "audioflux")
     shutil.copytree(PYREF, pkg)

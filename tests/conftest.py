@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def rel_max(a, b):
@@ -44,7 +44,7 @@ def golden():
 def ref_lib():
     from oracle import ref_lib as R
     if not R.available():
-        pytest.skip("oracle/_ref/libaudioflux_ref.so not built (needs /root/reference: make -C oracle)")
+        pytest.skip("oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
     return R.get_ref_lib()
 
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Generate tests/golden/*.npz from the UNMODIFIED reference build (oracle/_ref).
 
-Run in the build container (needs /root/reference to have been compiled by `make -C oracle`):
+Run where the reference has been compiled by `make -C oracle REF=<audioFlux tree>`:
     python tests/golden/make_golden.py
 The fixtures pin both the numpy oracle (tests/test_golden.py) and the CUDA path
 (tests/test_gpu_parity.py) to outputs of the reference itself.  Inputs are seeded

@@ -13,7 +13,7 @@ from oracle import ref_python as RP
 @pytest.fixture(scope="module")
 def raf(ref_lib):
     if not RP.available():
-        pytest.skip("oracle/_ref/pyref not built (needs /root/reference: make -C oracle)")
+        pytest.skip("oracle/_ref/pyref not built (make -C oracle REF=<audioFlux tree>)")
     import os
     from conftest import ROOT
     mod = RP.load(R.REF_PATH, os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so"))

@@ -21,7 +21,7 @@ B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 def raf(product_lib):
     """the reference package, default library = the reference build, lib_ext 'b200' = the product"""
     if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (needs /root/reference: make -C oracle)")
+        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
     mod = RP.load(R.REF_PATH, B200)
     yield mod
     mod.fftlib.set_fft_lib(None)

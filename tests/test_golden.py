@@ -1,5 +1,5 @@
 """The numpy oracle against fixtures generated from the reference itself
-(tests/golden/make_golden.py).  Runs everywhere (no GPU, no /root/reference)."""
+(tests/golden/make_golden.py).  Runs everywhere (no GPU, no reference build)."""
 import numpy as np
 
 from conftest import rel_max

@@ -36,7 +36,7 @@ TOL = 1e-4
 
 def reference_results(kind, seed, cases):
     if not R.available():
-        pytest.skip("oracle/_ref/libaudioflux_ref.so not built (needs /root/reference: make -C oracle)")
+        pytest.skip("oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
     with tempfile.TemporaryDirectory() as d:
         out = os.path.join(d, "ref.pkl")
         env = dict(os.environ, CUDA_VISIBLE_DEVICES="")

@@ -99,7 +99,7 @@ def test_peer_scatter_two_gpus(torch_cuda):
     torch = torch_cuda
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     n = 2 if n < 4 else 4 if n < 8 else 8
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={n}",
            "--master-addr", "127.0.0.1", "--master-port", "29533", os.path.join(ROOT, "tests", "_peer_scatter_worker.py")]

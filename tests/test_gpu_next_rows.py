@@ -421,7 +421,7 @@ def test_cqt_streaming_matches_oracle_and_reference(cuda_device, ref_lib, chunks
 @pytest.mark.parametrize("num,sr,beta,norm,bpo", [(84, 32000, 5.0, 0, 12), (48, 44100, 2.0, 1, 12), (72, 22050, 10.0, 2, 12),
                                                    (48, 16000, 3.0, 0, 24)])
 def test_vqt_vs_oracle_and_reference(cuda_device, ref_lib, num, sr, beta, norm, bpo):
-    """VQT (beta != 0, VERDICT r1 missing #5): per-octave kernel sets through the tcgen05 / mma / FP32 octave kernels"""
+    """VQT (beta != 0, VERDICT r1 missing #5): per-octave kernel sets through the wgmma / mma / FP32 octave kernels"""
     import audioflux_b200 as af
     x = (0.1 * np.random.default_rng(3).standard_normal(30000)).astype(np.float32)
     kw = dict(bin_per_octave=bpo, beta=beta, normal_type=af.SpectralFilterBankNormalType(norm))

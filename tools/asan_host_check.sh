@@ -10,7 +10,7 @@ ASAN=$(gcc -print-file-name=libasan.so)
 for f in "$ROOT"/audioflux_b200/csrc/host/*.c; do
   gcc -std=gnu99 -O1 -g -fPIC -fsanitize=address -fno-omit-frame-pointer -ffp-contract=off -I/usr/local/cuda/include -c "$f" -o "$TMP/$(basename "$f" .c).o"
 done
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -shared -Xlinker -Bsymbolic -o "$TMP/libaudioflux_b200.so" \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -Xlinker -Bsymbolic -o "$TMP/libaudioflux_b200.so" \
   "$TMP"/*.o "$ROOT"/audioflux_b200/csrc/build/*.cu.o -lm -Xlinker -lasan
 cd "$ROOT"
 export AFB200_LIB_PATH="$TMP/libaudioflux_b200.so"

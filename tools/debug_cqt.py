@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Per-octave comparison of the CQT octave kernels (tcgen05 / mma.sync / fp32) against each other and the oracle."""
+"""Per-octave comparison of the CQT octave kernels (wgmma / mma.sync / fp32) against each other and the oracle."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.realpath(__file__)))
@@ -25,8 +25,7 @@ def main():
     wr, wi = O.cqt(xh[1], 84, 48000, norm=O.NORM_AREA)
     want = wr + 1j * wi
     print("fp32 vs oracle", float(np.abs(ref[1] - want).max() / np.abs(want).max()))
-    for name, k, bo in (("mma.sync", "mma", "0"), ("tcgen05 bo=0", None, "0"), ("tcgen05 bo=1", None, "1"), ("tcgen05 bo=2", None, "2")):
-        os.environ["AFB200_UMMA_BO"] = bo
+    for name, k in (("mma.sync", "mma"), ("wgmma", None)):
         got = run(k, x)
         for o in range(7):
             sl = slice(12 * o, 12 * o + 12)

@@ -14,6 +14,7 @@ from .pwt import PWT  # noqa: F401
 from .wsst import WSST, Synsq  # noqa: F401
 from .reassign import Reassign  # noqa: F401
 from .spectrogram import Spectrogram, MelSpectrogram, BarkSpectrogram, ErbSpectrogram  # noqa: F401
+from .spectral import Spectral  # noqa: F401
 from . import lib  # noqa: F401
 
 __version__ = "0.1.0"

@@ -178,6 +178,49 @@ EXTENSION_API = {
     "afb200_chromaCqtFilterBank": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, vp]),
 }
 
+# spectral descriptors (src/feature/spectral_algorithm.h:16-81, include/afb200_spectral.h) and the additive batched
+# entry point (include/afb200_ext.h)
+_SPEC1 = (None, [vp, vp, vp])                       # (obj, mDataArr, dataArr)
+_SPEC_PH = (None, [vp, vp, vp, vp])                 # (obj, mSpecArr, mPhaseArr, dataArr)
+SPECTRAL_API = {
+    "spectralObj_new": (C.c_int, [P(vp), C.c_int, vp]),
+    "spectralObj_setEdge": (None, [vp, C.c_int, C.c_int]),
+    "spectralObj_setEdgeArr": (None, [vp, vp, C.c_int]),
+    "spectralObj_setTimeLength": (None, [vp, C.c_int]),
+    "spectralObj_flatness": _SPEC1,
+    "spectralObj_flux": (None, [vp, vp, C.c_int, C.c_float, C.c_int, c_int_p, c_int_p, vp]),
+    "spectralObj_rolloff": (None, [vp, vp, C.c_float, vp]),
+    "spectralObj_centroid": _SPEC1,
+    "spectralObj_spread": _SPEC1,
+    "spectralObj_skewness": _SPEC1,
+    "spectralObj_kurtosis": _SPEC1,
+    "spectralObj_entropy": (None, [vp, vp, C.c_int, vp]),
+    "spectralObj_crest": _SPEC1,
+    "spectralObj_slope": _SPEC1,
+    "spectralObj_decrease": _SPEC1,
+    "spectralObj_bandWidth": (None, [vp, vp, C.c_float, vp]),
+    "spectralObj_rms": _SPEC1,
+    "spectralObj_energy": (None, [vp, vp, C.c_int, C.c_float, vp]),
+    "spectralObj_hfc": _SPEC1,
+    "spectralObj_sd": (None, [vp, vp, C.c_int, C.c_int, vp]),
+    "spectralObj_sf": (None, [vp, vp, C.c_int, C.c_int, vp]),
+    "spectralObj_mkl": (None, [vp, vp, C.c_int, vp]),
+    "spectralObj_pd": _SPEC_PH,
+    "spectralObj_wpd": _SPEC_PH,
+    "spectralObj_nwpd": _SPEC_PH,
+    "spectralObj_cd": _SPEC_PH,
+    "spectralObj_rcd": _SPEC_PH,
+    "spectralObj_broadband": (None, [vp, vp, C.c_float, vp]),
+    "spectralObj_novelty": (None, [vp, vp, C.c_int, C.c_float, c_int_p, c_int_p, vp]),
+    "spectralObj_eef": (None, [vp, vp, C.c_int, vp]),
+    "spectralObj_eer": (None, [vp, vp, C.c_int, C.c_float, vp]),
+    "spectralObj_max": _SPEC_PH,
+    "spectralObj_mean": _SPEC_PH,
+    "spectralObj_var": _SPEC_PH,
+    "spectralObj_free": (None, [vp]),
+    "spectralObj_spectralBatch": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -188,7 +231,7 @@ REFERENCE_BUILDERS = {
 }
 
 
-def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, REFERENCE_BUILDERS)) -> dict:
+def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -281,6 +281,19 @@ int af_launch_cq_deconv(const float *in, int rows, int num, int mode, int hcNum,
 int af_launch_temporal(const float *data, int fftLength, int slideLength, int timeLength, const float *window,
                        float *energy, float *rms, float *zcr, void *stream);
 
+/* spectral descriptors (kernels/spectral.cu): all requests of one spectralObj_spectralBatch call in one launch */
+typedef struct {
+    const float *spec, *phase;    /* device, batch x T x num */
+    const float *fre;             /* device, num (NULL when no frequency feature is requested) */
+    const int *idx;               /* device bin list (NULL: the contiguous range start .. start+nb-1) */
+    float *out;                   /* device, planes of batch x T */
+    int num, T, batch, start, nb, nReq;
+    float meanFre;                /* float mean of fre over the bins, summed in list order (spectral_algorithm.c:1124-1130) */
+    int req[AFB200_SPECTRAL_MAX_REQ], plane[AFB200_SPECTRAL_MAX_REQ];
+    float par[4 * AFB200_SPECTRAL_MAX_REQ];
+} AfSpectralArgs;
+int af_launch_spectral(const AfSpectralArgs *a, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

@@ -74,6 +74,18 @@ class ChromaDataNormalType(Enum):
     P1 = 4
 
 
+class SpectralNoveltyMethodType(Enum):
+    SUB = 0
+    ENTROY = 1      # the reference's spelling
+    KL = 2
+    IS = 3
+
+
+class SpectralNoveltyDataType(Enum):
+    VALUE = 0
+    NUMBER = 1
+
+
 class PaddingPositionType(Enum):
     CENTER = 0
     RIGHT = 1

@@ -20,6 +20,7 @@
 #include "afb200_cwt.h"
 #include "afb200_spectrogram.h"
 #include "afb200_pwt.h"
+#include "afb200_spectral.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -137,6 +138,35 @@ int cqtObj_deconvBatch(CQTObj cqtObj, const float *in, int rows, float *timbre, 
                        int memKind, void *stream);
 /* chroma_cqtFilterBank (src/filterbank/chroma_filterBank.c:176-262): bank num x cqtLength */
 int afb200_chromaCqtFilterBank(int num, int cqtLength, int binPerOctave, float minFre, float *bank);
+
+/* Feature ids of spectralObj_spectralBatch and their parameters par[4*i .. 4*i+3] = {step, p, threshold, flags}
+ * (unused slots ignored; flags is an integer held in a float):
+ *   FLUX       step, p, -, flags bit0 isPositive, bit1 isExp, bit2 type (mean)
+ *   ROLLOFF    threshold                          ENTROPY / EEF   flags bit0 isNorm
+ *   BANDWIDTH  p                                  ENERGY          p = gamma, flags bit0 isLog
+ *   SD / SF    step, flags bit0 isPositive        MKL             flags bit2 type (mean)
+ *   BROADBAND  threshold                          EER             p = gamma, flags bit0 isNorm
+ *   NOVELTY    step, threshold, flags bits0-1 methodType, bit2 dataType (Number)
+ * MAX / MEAN / VAR write two consecutive planes: value, then frequency. */
+enum {
+    AFB200_SPECTRAL_FLATNESS = 0, AFB200_SPECTRAL_FLUX, AFB200_SPECTRAL_ROLLOFF, AFB200_SPECTRAL_CENTROID,
+    AFB200_SPECTRAL_SPREAD, AFB200_SPECTRAL_SKEWNESS, AFB200_SPECTRAL_KURTOSIS, AFB200_SPECTRAL_ENTROPY,
+    AFB200_SPECTRAL_CREST, AFB200_SPECTRAL_SLOPE, AFB200_SPECTRAL_DECREASE, AFB200_SPECTRAL_BANDWIDTH,
+    AFB200_SPECTRAL_RMS, AFB200_SPECTRAL_ENERGY, AFB200_SPECTRAL_HFC, AFB200_SPECTRAL_SD, AFB200_SPECTRAL_SF,
+    AFB200_SPECTRAL_MKL, AFB200_SPECTRAL_PD, AFB200_SPECTRAL_WPD, AFB200_SPECTRAL_NWPD, AFB200_SPECTRAL_CD,
+    AFB200_SPECTRAL_RCD, AFB200_SPECTRAL_BROADBAND, AFB200_SPECTRAL_NOVELTY, AFB200_SPECTRAL_EEF,
+    AFB200_SPECTRAL_EER, AFB200_SPECTRAL_MAX, AFB200_SPECTRAL_MEAN, AFB200_SPECTRAL_VAR,
+    AFB200_SPECTRAL_COUNT
+};
+#define AFB200_SPECTRAL_MAX_REQ 64
+/* spec (and phase, NULL unless PD / WPD / NWPD / CD / RCD is requested): batch x timeLength x num, time-major.
+ * req[i]: AFB200_SPECTRAL_* id, par[4*i .. 4*i+3] its parameters; 1 <= nReq <= AFB200_SPECTRAL_MAX_REQ.
+ * out: one plane of batch x timeLength per request (two for MAX / MEAN / VAR), in request order.  Frames that the
+ * reference leaves unwritten stay as they were in `out` (frame 1 of PD / WPD / NWPD, VAR with fewer than 2 bins) and
+ * BROADBAND adds its counts to what `out` holds.  req / par are host arrays; one kernel launch per call.  Each clip's
+ * temporal features start afresh (frame 0 of clip b never looks at clip b-1). */
+int spectralObj_spectralBatch(SpectralObj spectralObj, const float *spec, const float *phase, int timeLength, int batch,
+                              int nReq, const int *req, const float *par, float *out, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

@@ -40,6 +40,11 @@ typedef enum { ChromaDataNormal_None = 0, ChromaDataNormal_Max, ChromaDataNormal
 typedef enum { CepstralRectify_Log = 0, CepstralRectify_CubicRoot } CepstralRectifyType;
 typedef enum { CepstralEnergy_Replace = 0, CepstralEnergy_Append, CepstralEnergy_Ignore } CepstralEnergyType;
 
+/* src/flux_base.h:103-116 (spectral novelty; "Entroy" is the reference's spelling) */
+typedef enum { SpectralNoveltyMethod_Sub = 0, SpectralNoveltyMethod_Entroy, SpectralNoveltyMethod_KL,
+               SpectralNoveltyMethod_IS } SpectralNoveltyMethodType;
+typedef enum { SpectralNoveltyData_Value = 0, SpectralNoveltyData_Number } SpectralNoveltyDataType;
+
 typedef enum { PaddingPosition_Center = 0, PaddingPosition_Right, PaddingPosition_Left } PaddingPositionType;
 typedef enum { PaddingMode_Constant = 0, PaddingMode_Reflect, PaddingMode_Wrap } PaddingModeType;
 

@@ -1,0 +1,170 @@
+"""Spectral descriptors without a GPU: the numpy oracle against the reference build (or its stored outputs in
+tests/golden/spectral.npz), the argument rules of SpectralObj, the exported C API and the loud failure without a GPU."""
+import ctypes as C
+import os
+import re
+
+import numpy as np
+import pytest
+
+from conftest import ROOT, GOLDEN
+import _spectral_cases as SC
+
+import audioflux_b200 as af
+from audioflux_b200 import capi
+
+GOLD = os.path.join(GOLDEN, "spectral.npz")
+
+
+def _key(setname, mode, vi, part=0):
+    return f"{setname}/{mode}/{vi}/{part}"
+
+
+def _cases():
+    for setname, x, ph, fre in SC.spectrogram_sets():
+        for mode in ("full", "range", "list"):
+            for vi, (name, kw) in enumerate(SC.VARIANTS):
+                if name in SC.SO.PHASE and ph is None:
+                    continue
+                yield setname, x, ph, fre, mode, vi, name, kw
+
+
+def _reference_outputs():
+    """{key: reference output}: from the reference build when present, else the stored golden file"""
+    from oracle import ref_lib as R
+    if R.available():
+        lib = R.get_ref_lib()
+        res = {}
+        for setname, x, ph, fre, mode, vi, name, kw in _cases():
+            out = SC.call_c(lib, name, x, fre, mode, ph, **kw)
+            for part, o in enumerate(out if isinstance(out, tuple) else (out,)):
+                res[_key(setname, mode, vi, part)] = o
+        return res
+    if not os.path.exists(GOLD):
+        pytest.skip("no reference build and no tests/golden/spectral.npz")
+    g = np.load(GOLD)
+    return {k: g[k] for k in g.files}
+
+
+@pytest.fixture(scope="module")
+def ref_out():
+    return _reference_outputs()
+
+
+def test_oracle_matches_reference(ref_out):
+    bad = []
+    for setname, x, ph, fre, mode, vi, name, kw in _cases():
+        want = SC.oracle(name, x, fre, mode, ph, **kw)
+        for part, w in enumerate(want if isinstance(want, tuple) else (want,)):
+            r = ref_out[_key(setname, mode, vi, part)]
+            msg = SC.agree(w, r, exact=SC.is_exact(name, kw) or (name == "max" and part == 1))
+            if msg:
+                bad.append(f"{setname}/{mode}/{name}{kw}[{part}]: {msg}")
+    assert not bad, "\n".join(bad[:20])
+
+
+def test_golden_file_matches_reference_build():
+    from oracle import ref_lib as R
+    if not (R.available() and os.path.exists(GOLD)):
+        pytest.skip("needs both the reference build and tests/golden/spectral.npz")
+    g = np.load(GOLD)
+    live = _reference_outputs()
+    assert sorted(g.files) == sorted(live)
+    for k in g.files:
+        assert SC.agree(live[k], g[k], exact=True) is None, k
+
+
+def test_constructor_and_edge_rules(product_lib):
+    lib = product_lib
+    obj = C.c_void_p()
+    assert lib.spectralObj_new(C.byref(obj), 1, None) == -1
+    fre = np.arange(16, dtype=np.float32)
+    assert lib.spectralObj_new(C.byref(obj), 16, fre.ctypes.data) == 0
+    lib.spectralObj_setEdge(obj, 5, 16)          # end > num-1: ignored
+    lib.spectralObj_setEdge(obj, 4, 4)           # empty: ignored
+    lib.spectralObj_setEdge(obj, -1, 3)          # ignored
+    lib.spectralObj_setEdge(obj, 2, 9)           # accepted
+    # setEdgeArr takes ownership: an invalid list is freed and ignored, a valid one replaces (and frees) the old one
+    for idx in ([3, 99], [5, 1, 5, 0], [15, -1], [2, 2]):
+        p = SC._libc.calloc(len(idx), 4)
+        (C.c_int * len(idx)).from_address(p)[:] = idx
+        lib.spectralObj_setEdgeArr(obj, C.c_void_p(p), len(idx))
+    lib.spectralObj_free(obj)
+    with pytest.raises(ValueError):
+        af.Spectral(1, np.zeros(1, np.float32))
+    s = af.Spectral(16, fre)
+    with pytest.raises(ValueError):
+        s.set_edge(3, 16)
+    with pytest.raises(ValueError):
+        s.set_edge(5, 5)
+    s.set_edge_arr([4, 2, 2, 9])
+    with pytest.raises(ValueError):
+        s.spectral_batch(np.zeros((3, 15), np.float32), ["centroid"])
+    with pytest.raises(ValueError):
+        s.spectral_batch(np.zeros((3, 16), np.float32), ["pd"])
+    with pytest.raises(ValueError):
+        s.spectral_batch(np.zeros((3, 16), np.float32), ["nope"])
+
+
+def test_batch_rejects_bad_requests(product_lib):
+    lib = product_lib
+    obj = C.c_void_p()
+    assert lib.spectralObj_new(C.byref(obj), 8, None) == 0
+    x = np.ones((2, 8), np.float32)
+    out = np.full(4, 7.0, np.float32)
+    par = np.zeros(4, np.float32)
+    for req in (99, 3):      # unknown id; centroid without freBandArr
+        r = np.array([req], np.int32)
+        assert lib.spectralObj_spectralBatch(obj, x.ctypes.data, None, 2, 1, 1, r.ctypes.data, par.ctypes.data,
+                                             out.ctypes.data, 0, None) != 0
+    r = np.array([18], np.int32)  # pd without phase planes
+    assert lib.spectralObj_spectralBatch(obj, x.ctypes.data, None, 2, 1, 1, r.ctypes.data, par.ctypes.data,
+                                         out.ctypes.data, 0, None) != 0
+    assert (out == 7.0).all()
+    lib.spectralObj_free(obj)
+
+
+def _spectral_declared():
+    src = open(os.path.join(ROOT, "include", "afb200_spectral.h")).read() + \
+        open(os.path.join(ROOT, "include", "afb200_ext.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    return {m.group(1) for m in re.finditer(r"\b(spectralObj_[A-Za-z0-9_]*)\s*\(", src)}
+
+
+def test_spectral_api_declared_and_exported(product_lib):
+    declared = _spectral_declared()
+    assert set(capi.SPECTRAL_API) == declared
+    for name in capi.SPECTRAL_API:
+        assert hasattr(product_lib, name), name
+    from oracle import ref_lib as R
+    if R.available():
+        lib = R.get_ref_lib()
+        for name in capi.SPECTRAL_API:
+            if name != "spectralObj_spectralBatch":
+                assert hasattr(lib, name), name
+
+
+def test_feature_ids_match_header():
+    src = open(os.path.join(ROOT, "include", "afb200_ext.h")).read()
+    body = src[src.index("AFB200_SPECTRAL_FLATNESS = 0"):src.index("AFB200_SPECTRAL_COUNT")]
+    ids = [n.lower() for n in re.findall(r"AFB200_SPECTRAL_([A-Z]+)", body)]
+    from audioflux_b200 import spectral
+    assert [n.replace("_", "") for n in spectral.FEATURES] == ids
+
+
+def test_no_gpu_means_loud_failure_spectral(product_lib):
+    if product_lib.afb200_deviceCount() > 0:
+        return
+    fre = np.arange(32, dtype=np.float32)
+    s = af.Spectral(32, fre)
+    x = np.ones((2, 5, 32), np.float32)
+    with pytest.raises(af.lib.AfB200Error, match="no CUDA device"):
+        s.spectral_batch(x, ["centroid", "flux"])
+    out = np.full(5, 7.0, np.float32)
+    obj = C.c_void_p()
+    assert product_lib.spectralObj_new(C.byref(obj), 32, fre.ctypes.data) == 0
+    product_lib.spectralObj_setTimeLength(obj, 5)
+    product_lib.spectralObj_centroid(obj, x[0].ctypes.data, out.ctypes.data)
+    assert (out == 7.0).all()
+    assert b"no CUDA device" in product_lib.afb200_lastError()
+    product_lib.spectralObj_free(obj)

@@ -44,3 +44,13 @@ __device__ __forceinline__ c64 c_mul(c64 a, c64 w) {
 }
 // |v|^2
 __device__ __forceinline__ float c_norm2(c64 v) { float a, b; c_unpack(v_mul(v, v), a, b); return a + b; }
+
+// FMA forms (the fused MFCC frame path only): fewer instructions, each product rounded once inside an FMA, so results
+// differ from the helpers above in the last bits.
+// a * w: FMUL + FFMA per component
+__device__ __forceinline__ c64 c_mul_fma(c64 a, c64 w) {
+    float ar, ai, wr, wi; c_unpack(a, ar, ai); c_unpack(w, wr, wi);
+    return c_pack(__fmaf_rn(-ai, wi, __fmul_rn(ar, wr)), __fmaf_rn(ai, wr, __fmul_rn(ar, wi)));
+}
+// |v|^2: FMUL + FFMA
+__device__ __forceinline__ float c_norm2_fma(c64 v) { float a, b; c_unpack(v, a, b); return __fmaf_rn(a, a, __fmul_rn(b, b)); }

@@ -67,10 +67,13 @@ constexpr int kMaxPieces = 256;     // pieces the intervals may be cut into (slo
 constexpr int kMaxPass = kMaxPieces / (kEW * 32);   // bank passes: one piece per helper lane and pass
 constexpr int kSpecPitch = 17;      // c64 slots per n2 row of the special-column buffer (odd -> conflict-free both ways)
 constexpr int kScratchFloats = 33 * 32;
+constexpr int kPitchPairs = kFW | 1;   // power-tile row pitch (frames): odd -> conflict-free column walks; always kFW wide
+constexpr int kBarBytes = 128;      // 12 mbarriers at the start of shared memory (128 keeps the TMA span aligned)
+constexpr int kTwRows = 31;         // stage-C twiddles W_2048^(lane k1), k1 = 1..31: one complex product per column
 
 struct Plan {
     float2 *dWinPairs;              // [32 m][32 lane]  0.5 * (w[64 m + lane], w[64 m + 32 + lane])
-    float2 *dTw;                    // [17][32]  W_2048^(lane * ka), ka = 0..15; row 16: W_2048^(16 lane)
+    float2 *dTw;                    // [kTwRows][32]  W_2048^(lane * k1), k1 = 1..31 (row k1 - 1)
     float *dDct;                    // [128 m][dctPitch]
     int num, ccNum, ct, dataType;
     unsigned ivDesc[kMaxNum + 4];   // (first bin pair << 16) | table offset; entries num+1.. = end sentinels
@@ -94,10 +97,10 @@ struct Params {
     long long dataStride;
     unsigned totalTiles;            // (< 2^31: checked by the launcher) 32-bit tile arithmetic in the kernel
     int batch, timeLength, hop, framesPerTile, tilesPerClip, spanFloats, stages;
-    int num, ccNum, rectify, dataType, rawMel, pitchPairs, bulkStore, dctPitch;
+    int num, ccNum, rectify, dataType, rawMel, bulkStore, dctPitch;
     int nPeer;
     float *peerOut[kMaxPeers];
-    int offSpan, offScratch, offP, offWin, offTw, offSpec, offDct, offL, offStage, offBar, offTab, offDesc, offAssign, offPrefix, stageBytes;   // offL: two log-mel tiles
+    int offSpan, offScratch, offP, offWin, offTw, offSpec, offDct, offL, offStage, offTab, offDesc, offAssign, offPrefix, stageBytes;   // offL: two log-mel tiles
     int nPass, passLen[kMaxPass];
     const unsigned short *assign;
     int tabLen;
@@ -148,14 +151,14 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     extern __shared__ __align__(128) unsigned char smem[];
     float *span = reinterpret_cast<float *>(smem + p.offSpan);
     float *scratchAll = reinterpret_cast<float *>(smem + p.offScratch);
-    float *sP = reinterpret_cast<float *>(smem + p.offP);                 // [kPairs][pitchPairs][2]
+    float *sP = reinterpret_cast<float *>(smem + p.offP);                 // [kPairs][kPitchPairs][2]
     float2 *sWin = reinterpret_cast<float2 *>(smem + p.offWin);
     float2 *sTw = reinterpret_cast<float2 *>(smem + p.offTw);
     c64 *sSpec = reinterpret_cast<c64 *>(smem + p.offSpec);               // [2][32 n2][kSpecPitch]
     float *sDct = reinterpret_cast<float *>(smem + p.offDct);
     float *sL = reinterpret_cast<float *>(smem + p.offL);                 // [16][kLPitch]
     float *sStage = reinterpret_cast<float *>(smem + p.offStage);         // result tile(s), dense rows
-    uint64_t *fullBar = reinterpret_cast<uint64_t *>(smem + p.offBar);    // [2] TMA landed
+    uint64_t *fullBar = reinterpret_cast<uint64_t *>(smem);               // [2] TMA landed (barriers at offset 0: fixed addresses)
     uint64_t *emptyBar = fullBar + 2;                                     // [2] frame warps took their samples
     uint64_t *specFull = fullBar + 4;                                     // [2] special columns of a tile stored
     uint64_t *pFull = fullBar + 6;                                        // power-spectrum tile complete
@@ -168,11 +171,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     unsigned short *sPrefix = reinterpret_cast<unsigned short *>(smem + p.offPrefix);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pitch = p.pitchPairs;
+    constexpr int pitch = kPitchPairs;        // compile-time: the power-tile stores and walks take immediate offsets
 
     // ---- one-time: tables -> shared, zero the tiles (pad slots are multiplied by zero weights), barriers ----
     for (int i = threadIdx.x; i < 32 * 32; i += kThreads) sWin[i] = p.winPairs[i];
-    for (int i = threadIdx.x; i < 17 * 32; i += kThreads) sTw[i] = p.tw[i];
+    for (int i = threadIdx.x; i < kTwRows * 32; i += kThreads) sTw[i] = p.tw[i];
     for (int i = threadIdx.x; i < p.tabLen; i += kThreads) sTab[i] = p.bankTab[i];
     for (int i = threadIdx.x; i < kMaxPieces; i += kThreads) sDesc[i] = p.pieceDesc[i];
     for (int i = threadIdx.x; i < kMaxNum + 4; i += kThreads) sPrefix[i] = p.piecePrefix[i];
@@ -242,18 +245,18 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 u[n2] = kind ? af_mul_w64(c_pack(v, 0.0f), n2 & 15) : c_pack(v, 0.0f);
                 if (n2 >= 16 && kind) u[n2] = c_mul_mi(u[n2]);                        // W_64^16 = -i
             }
-            af_fft32(u);
+            af_fft32_fma(u);
             wait_cls<16>(pEmpty, ((uint32_t)it & 1u) ^ 1u);                   // bank done with the previous tile
             if (f < nf) {
                 float *dst = sP + 2 * f + (kind ? 32 * pitch : 0);                    // bin 64 k2 + 32 kind -> pair 32 k2 + 16 kind
 #pragma unroll
                 for (int k2 = 0; k2 < 16; k2++) {
-                    float pw = c_norm2(u[AF_BR5(k2)]);
+                    float pw = c_norm2_fma(u[AF_BR5(k2)]);
                     if (p.dataType == SpectralData_Mag) pw = sqrtf(pw);
                     dst[(size_t)k2 * 64 * pitch] = pw;
                 }
                 if (!kind) {
-                    float pw = c_norm2(u[AF_BR5(16)]);
+                    float pw = c_norm2_fma(u[AF_BR5(16)]);
                     if (p.dataType == SpectralData_Mag) pw = sqrtf(pw);
                     dst[(size_t)16 * 64 * pitch] = pw;                                // bin 1024
                 }
@@ -270,13 +273,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         const int rowFloats = p.num;
         int it = 0;
         for (unsigned tile = blockIdx.x; tile < p.totalTiles; tile += gridDim.x, ++it) {
-            const unsigned clip = tile / (unsigned)p.tilesPerClip;
-            const int f0 = (int)(tile - clip * (unsigned)p.tilesPerClip) * F;
-            const int nf = min(F, p.timeLength - f0);
             const int lbuf = it & 1;
-            float *L = sL + (size_t)lbuf * 16 * kLPitch;
-            float *stage = sStage + (size_t)lbuf * (p.stageBytes / 8);   // (filter-bank output mode: two staging tiles)
-            const int stagePitch = p.num + 4;                              // padded rows (bank conflicts)
             wait_cls<2>(pFull, (uint32_t)it & 1u);
             if (!p.rawMel) wait_cls<2>(&lEmpty[lbuf], ((uint32_t)(it >> 1) & 1u) ^ 1u);    // DCT done with tile it - 2
             // ---- phase 1: ONE PIECE (<= Lmax bin pairs of one interval) PER LANE AND PASS, all frames of the tile in
@@ -322,6 +319,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                     }
                 }
             }
+            // (tile geometry after phase 1: nothing of it stays live across the accumulator loop)
+            const unsigned clip = tile / (unsigned)p.tilesPerClip;
+            const int f0 = (int)(tile - clip * (unsigned)p.tilesPerClip) * F;
+            const int nf = min(F, p.timeLength - f0);
+            float *L = sL + (size_t)lbuf * 16 * kLPitch;
+            float *stage = sStage + (size_t)lbuf * (p.stageBytes / 8);   // (filter-bank output mode: two staging tiles)
+            const int stagePitch = p.num + 4;                              // padded rows (bank conflicts)
             if (p.rawMel && e == 0) bulk_wait_read0();             // the store of tile it - 2 has read this staging tile
             named_bar_sync(1, kBW * 32);                           // every partial sum of the tile is in shared memory
             // ---- phase 2: mel_m = sum of the rise parts of interval m + the fall parts of interval m + 1 (pieces in
@@ -486,7 +490,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     float *scratch = scratchAll + (size_t)warp * kScratchFloats;
     const c64 *sWinC = reinterpret_cast<const c64 *>(sWin);
     const c64 *sTwC = reinterpret_cast<const c64 *>(sTw);
-    const c64 w16 = sTwC[16 * 32 + lane];                          // W_2048^(16 lane)
     // power-tile addresses (floats): bin = lane + 64 k2 (k2 < 16) and 64 (32 - k2) - lane (k2 >= 16)
     const int strideK2 = 64 * pitch;
     const int offLo = (lane >> 1) * (2 * pitch) + 2 * warp + (lane & 1);
@@ -527,21 +530,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         }
 
         // ---- B: 64-point real DFT of the lane's column: packed complex 32-point DFT + in-lane post-pass ----
-        if (!(AF2_ABLATE & 4)) af_fft32(z);                        // Z[k] at AF_BR5(k)
-#pragma unroll
-        for (int k = 1; k < 16; k++) {
-            const c64 zk = z[AF_BR5(k)], zc = c_conj(z[AF_BR5(32 - k)]);
-            const c64 ev = c_add(zk, zc);
-            const c64 od = af_mul_w64(c_mul_mi(c_sub(zk, zc)), k);  // -i W_64^k (Z[k] - conj Z[32-k])
-            z[AF_BR5(k)] = c_add(ev, od);                           // R[k]   (window carries the 1/2)
-            z[AF_BR5(32 - k)] = c_conj(c_sub(ev, od));              // R[32-k]
-        }
-        z[AF_BR5(16)] = v_mul(z[AF_BR5(16)], c_pack(2.0f, -2.0f)); // R[16] = 2 conj Z[16]
-        {
-            float zr, zi;
-            c_unpack(z[0], zr, zi);
-            z[0] = c_pack(2.0f * (zr + zi), 2.0f * (zr - zi));      // (R[0], R[32]), both real
-        }
+        if (!(AF2_ABLATE & 4)) af_fft32_fma(z);                    // Z[k] at AF_BR5(k)
+        // R[k] = (Z[k] + conj Z[32-k]) - i W_64^k (Z[k] - conj Z[32-k]) at AF_BR5(k), (R[0], R[32]) in z[0]
+        af_rfft64_post_fma(z);
         sSpec[((size_t)sb * 32 + lane) * kSpecPitch + warp] = z[0];
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&specFull[sb]);
@@ -551,9 +542,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             float yr[32], yi[32];
 #pragma unroll
             for (int k1 = 1; k1 < 32; k1++) {
-                c64 y = z[AF_BR5(k1)];
-                if (k1 >= 16) y = c_mul(y, w16);
-                if (k1 & 15) y = c_mul(y, sTwC[(k1 & 15) * 32 + lane]);
+                const c64 y = c_mul_fma(z[AF_BR5(k1)], sTwC[(k1 - 1) * 32 + lane]);
                 c_unpack(y, yr[k1], yi[k1]);
             }
             if (!(AF2_ABLATE & 8)) {
@@ -576,20 +565,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             }
         }
         // ---- D: 32-point DFT over n2 in lane k1: bins k1 + 64 k2 and, mirrored, 64 (32 - k2) - k1 ----
-        if (!(AF2_ABLATE & 4)) af_fft32(z);
+        if (!(AF2_ABLATE & 4)) af_fft32_fma(z);
         wait_cls<1>(pEmpty, ((uint32_t)it & 1u) ^ 1u);      // bank done with the previous tile's spectra
         if (lane) {
             if (p.dataType == SpectralData_Mag) {                  // (uniform branch: no sqrt sequence in the power path)
 #pragma unroll
                 for (int k2 = 0; k2 < 32; k2++) {
-                    const float pw = sqrtf(c_norm2(z[AF_BR5(k2)]));
+                    const float pw = sqrtf(c_norm2_fma(z[AF_BR5(k2)]));
                     if (k2 < 16) sP[offLo + k2 * strideK2] = pw;
                     else sP[offHi + (32 - k2) * strideK2] = pw;
                 }
             } else {
 #pragma unroll
                 for (int k2 = 0; k2 < 32; k2++) {
-                    const float pw = c_norm2(z[AF_BR5(k2)]);
+                    const float pw = c_norm2_fma(z[AF_BR5(k2)]);
                     if (k2 < 16) sP[offLo + k2 * strideK2] = pw;
                     else sP[offHi + (32 - k2) * strideK2] = pw;
                 }
@@ -772,12 +761,12 @@ extern "C" int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int c
     for (int m = 0; m < 32; m++)
         for (int l = 0; l < 32; l++) wp[m * 32 + l] = make_float2(0.5f * window[64 * m + l], 0.5f * window[64 * m + 32 + l]);
     rc = af_dev_upload(reinterpret_cast<void **>(&pl->dWinPairs), wp, sizeof(float2) * 1024);
-    for (int ka = 0; ka < 17; ka++)
+    for (int k1 = 1; k1 <= kTwRows; k1++)
         for (int l = 0; l < 32; l++) {
-            const double a = -2.0 * M_PI * (double)((ka < 16 ? ka : 16) * l) / 2048.0;
-            wp[ka * 32 + l] = make_float2((float)cos(a), (float)sin(a));
+            const double a = -2.0 * M_PI * (double)(k1 * l) / 2048.0;
+            wp[(k1 - 1) * 32 + l] = make_float2((float)cos(a), (float)sin(a));
         }
-    if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dTw), wp, sizeof(float2) * 17 * 32);
+    if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dTw), wp, sizeof(float2) * kTwRows * 32);
     free(wp);
 
     Intervals *iv = static_cast<Intervals *>(malloc(sizeof(Intervals)));
@@ -846,26 +835,24 @@ static int launch_fused2(void *plan, const float *data, int dataLength, int batc
     const int budget = 227 * 1024;
     int F = kFW < timeLength ? kFW : timeLength, stages = 2, total = 0;
     for (;;) {
-        int o = 0;
+        int o = kBarBytes;                                      // the mbarriers come first
         const int spanFloats = (F - 1) * slideLength + kN;
-        const int pitchPairs = kFW | 1;                          // odd: conflict-free column walks; always kFW frames wide (bank phase)
         pp->offSpan = o;    o += stages * spanFloats * 4;
         pp->offScratch = o; o += kFW * kScratchFloats * 4;
-        pp->offP = o;       o += (kPairs * pitchPairs * 8 + 15) & ~15;
+        pp->offP = o;       o += (kPairs * kPitchPairs * 8 + 15) & ~15;
         pp->offWin = o;     o += 32 * 32 * 8;
-        pp->offTw = o;      o += 17 * 32 * 8;
+        pp->offTw = o;      o += kTwRows * 32 * 8;
         pp->offSpec = o;    o += 2 * 32 * kSpecPitch * 8;
         pp->offDct = o;     o += rawMel ? 0 : kMaxNum * pp->dctPitch * 4;
         pp->offL = o;       o += 2 * 16 * kLPitch * 4;
         pp->stageBytes = rawMel ? 2 * ((F * (pl->num + 4) * 4 + 15) & ~15) : ((F * pl->ccNum * 4 + 15) & ~15);
         pp->offStage = o;   o += pp->stageBytes;
-        pp->offBar = o;     o += 12 * 8;
         pp->offTab = o;     o += pl->tabLen * 16;
         pp->offDesc = o;    o += kMaxPieces * 4;
         pp->offAssign = o;  o += (kMaxPass * kEW * 32 * 2 + 15) & ~15;
         pp->offPrefix = o;  o += ((kMaxNum + 4) * 2 + 15) & ~15;
         total = o;
-        pp->spanFloats = spanFloats; pp->pitchPairs = pitchPairs;
+        pp->spanFloats = spanFloats;
         if (total <= budget) break;
         if (stages == 2) { stages = 1; continue; }
         stages = 2;

@@ -173,7 +173,6 @@ EXTENSION_API = {
     "afb200_auditoryFilterBank": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.c_float, C.c_float, C.c_int, vp, vp, vp]),
     "afb200_decimatorTaps": (C.c_int, [vp, vp]),
-    "afb200_mfccIntervalPlan": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
     "afb200_mfccBankPlan2": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
     "afb200_chromaCqtFilterBank": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, vp]),
 }

@@ -181,11 +181,10 @@ typedef struct {
 } AfMfccArgs;
 int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const AfBands *bands);
 int af_mfcc_plan_build(void **plan, int fftLength, int num, int ccNum, const float *window,
-                       const float *bank, const AfBands *bands, const float *dct, int dataType,
-                       const float *gain /* per-filter normalisation gains (NULL = 1) */);
+                       const float *bank, const AfBands *bands, const float *dct, int dataType);
 int af_launch_mel_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
                         int slideLength, float *out, void *stream);   /* stops after the bank: batch x T x num */
-int af_mfcc_plan_mode(void *plan);      /* 1: interval (shared product) bank loop, 0: filter-per-lane */
+int af_mfcc_plan_mode(void *plan);      /* 0: a plan (the fused kernel serves the object), -1: no plan */
 void af_mfcc_plan_free(void *plan);
 int af_launch_mfcc_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
                          int slideLength, int rectifyType, float *out, int nPeer, float *const *peerOut,

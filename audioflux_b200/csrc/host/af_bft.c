@@ -223,12 +223,11 @@ static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, 
         if (!b->melPlan) {
             float *dct = (float *)calloc((size_t)b->num, sizeof(float));      /* unused by this mode */
             if (!dct) return AF_ERR_NOMEM;
-            rc = af_mfcc_plan_build(&b->melPlan, b->fftLength, b->num, 1, b->window, b->bank, &b->bands, dct, b->dataType, NULL);
+            rc = af_mfcc_plan_build(&b->melPlan, b->fftLength, b->num, 1, b->window, b->bank, &b->bands, dct, b->dataType);
             free(dct);
             if (rc) return rc;
         }
-        if (af_mfcc_plan_mode(b->melPlan) == 0)
-            return af_launch_mel_fused(b->melPlan, dData, dataLength, batch, T, b->slideLength, dRe, st);
+        return af_launch_mel_fused(b->melPlan, dData, dataLength, batch, T, b->slideLength, dRe, st);
     }
     const int linear = b->scaleType == SpectralFilterBankScale_Linear;
     const int count = b->highIndex - b->lowIndex + 1 < b->num ? b->highIndex - b->lowIndex + 1 : b->num;
@@ -402,32 +401,7 @@ static int mfcc_compute(BFTObj b, const float *dData, int dataLength, int batch,
             float *dct = (float *)malloc(sizeof(float) * (size_t)ccNum * b->num);
             if (!dct) return AF_ERR_NOMEM;
             af_dct2_matrix(b->num, ccNum, dct);
-            /* per-filter gain of the bank normalisation (row peak over the un-normalised row peak): lets the kernel
-             * use the interval form of triangular banks; a bank without that structure is detected and ignored */
-            float *gain = NULL;
-            if (b->normalType != SpectralFilterBankNormal_None) {
-                const int width = b->fftLength / 2 + 1;
-                float *unit = (float *)calloc((size_t)b->num * width, sizeof(float));
-                float *fre = (float *)calloc((size_t)b->num + 2, sizeof(float));
-                int *bin = (int *)calloc((size_t)b->num + 2, sizeof(int));
-                gain = (float *)malloc(sizeof(float) * (size_t)b->num);
-                if (unit && fre && bin && gain &&
-                    !af_auditory_filterbank(b->num, b->fftLength, b->samplate, b->scaleType, b->styleType,
-                                            SpectralFilterBankNormal_None, b->lowFre, b->highFre, b->binPerOctave, unit, fre, bin)) {
-                    for (int m = 0; m < b->num; m++) {
-                        float pn = 0, pu = 0;
-                        for (int k = 0; k < width; k++) {
-                            if (b->bank[(size_t)m * width + k] > pn) pn = b->bank[(size_t)m * width + k];
-                            if (unit[(size_t)m * width + k] > pu) pu = unit[(size_t)m * width + k];
-                        }
-                        gain[m] = pu > 0 ? pn / pu : 0.0f;
-                    }
-                } else { free(gain); gain = NULL; }
-                free(unit); free(fre); free(bin);
-                if (!gain) { free(dct); return AF_ERR_NOMEM; }
-            }
-            rc = af_mfcc_plan_build(&b->mfccPlan, b->fftLength, b->num, ccNum, b->window, b->bank, &b->bands, dct, b->dataType, gain);
-            free(gain);
+            rc = af_mfcc_plan_build(&b->mfccPlan, b->fftLength, b->num, ccNum, b->window, b->bank, &b->bands, dct, b->dataType);
             free(dct);
             if (rc) return rc;
             b->mfccPlanCc = ccNum;

@@ -175,19 +175,18 @@ static int cqt_compute_ex(CQTObj c, const float *dData, int dataLength, int batc
         /* padded STFT semantics: drop the tail that does not fill a hop when more than one frame exists */
         const int frames = len / hop + 1;
         const int valid = frames > 1 ? len - len % hop : len;
-        const char *kq = getenv("AFB200_CQT_KERNEL");
         /* kernel set of this octave: the shared top-octave set, or -- VQT -- the octave's own */
         const size_t set = c->bank.vqt ? (size_t)o : 0;
         const unsigned char *bimg = c->dBimg ? c->dBimg + set * (size_t)(c->fftLength / 128) * 32768 : NULL;
         const float *bfrag = c->dBfrag ? c->dBfrag + set * (size_t)(c->fftLength / 8) * 96 * 4 : NULL;
         const float *kappa = c->dKappa2 + set * 2 * (size_t)c->binPerOctave * c->fftLength;
-        /* wgmma (default where the hop allows it) > mma.sync 3xTF32 > FP32 loop; AFB200_CQT_KERNEL = mma | fp32 forces the older ones */
-        if (c->dBimg && af_cqt_wgmma_supported(c->fftLength, hop, c->binPerOctave) && !kq) {
+        /* wgmma where the hop allows it, else mma.sync 3xTF32, else the FP32 loop */
+        if (c->dBimg && af_cqt_wgmma_supported(c->fftLength, hop, c->binPerOctave)) {
             if ((rc = af_launch_cqt_octave_wgmma(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bimg,
                                                 c->dScale + (size_t)k * c->binPerOctave, c->num, o * c->binPerOctave, dRe, dIm, st))) return rc;
             continue;
         }
-        if (c->dBfrag && af_cqt_tc_supported(c->fftLength, hop, c->binPerOctave) && !(kq && !strcmp(kq, "fp32"))) {
+        if (c->dBfrag && af_cqt_tc_supported(c->fftLength, hop, c->binPerOctave)) {
             if ((rc = af_launch_cqt_octave_tc(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bfrag,
                                               c->dScale + (size_t)k * c->binPerOctave, c->num, o * c->binPerOctave, dRe, dIm, st))) return rc;
             continue;

@@ -14,7 +14,6 @@
 // For N <= 4096 the columns kernel alone is the whole transform (N2 = 1).
 // Shared-memory legs use the same Stockham radix-4/2 autosort passes as stft_generic.cu.
 #include <math.h>
-#include <stdlib.h>
 #include "common.cuh"
 #include "fft32_gen.cuh"
 
@@ -623,7 +622,7 @@ void fill_params(const AfCwtArgs *a, CwtParams *p) {
     p->bankTable = a->bankTable; p->bankWidth = a->bankWidth;
     p->itemBase = 0;
     p->wType = a->wavelet.waveletType; p->g = a->wavelet.gamma; p->b = a->wavelet.beta; p->factor = (float)a->wavelet.factor;
-    const size_t budget = (size_t)(getenv("AFB200_CWT_LEG_KB") ? atoi(getenv("AFB200_CWT_LEG_KB")) : 72) * 1024;   // per-CTA leg buffers: small enough for 2-3 CTAs per SM so load / FFT / store phases of different CTAs overlap
+    const size_t budget = 72 * 1024;   // per-CTA leg buffers: small enough for 2-3 CTAs per SM so load / FFT / store phases of different CTAs overlap
     p->cols = p->N2 == 1 ? 1 : 8;
     while (p->cols > 1 && sizeof(float2) * 2 * (size_t)p->cols * (p->N1 + 1) > budget) p->cols >>= 1;
     p->rows = 16;
@@ -640,24 +639,17 @@ int set_smem(K kernel, size_t bytes, const char *name) {
 }  // namespace
 
 // fast path (N = 2^19): persistent fused inverse legs over a small ring of inter-leg slots
-static int cwt_fused_enabled(const AfCwtArgs *a) {
-    const char *e = getenv("AFB200_CWT_FUSED");
-    return a->log2n == 19 && !getenv("AFB200_CWT_GENERIC") && !(e && e[0] == '0');
-}
-static int cwt_group_items(void) {
-    const char *e = getenv("AFB200_CWT_GROUP");
-    const int g = e ? atoi(e) : 0;
-    return g > 0 && g <= 64 ? g : 2;                     // 3 slots x 2 items x 4 MB = 24 MB: half of the 50 MB L2 of an H100
-}
+static int cwt_fused_enabled(const AfCwtArgs *a) { return a->log2n == 19; }
+constexpr int kGroupItems = 2;                           // 3 slots x 2 items x 4 MB = 24 MB: half of the 50 MB L2 of an H100
 
 // workspace = forward spectrum (batch x N float2) + inter-leg buffer: batch x num x N float2 when N > 4096, or -- fused
-// fast path -- a ring of kRing x groupItems item slots plus the unit counters
+// fast path -- a ring of kRing x kGroupItems item slots plus the unit counters
 extern "C" size_t af_cwt_workspace_bytes(const AfCwtArgs *a) {
     const size_t N = (size_t)1 << a->log2n;
     size_t bytes = sizeof(float2) * N * (size_t)a->batch;
     if (cwt_fused_enabled(a)) {
         // the forward transform of the chunk uses one inter-leg slot per clip, the fused inverse the ring
-        size_t slots = (size_t)kRing * cwt_group_items();
+        size_t slots = (size_t)kRing * kGroupItems;
         if ((size_t)a->batch > slots) slots = (size_t)a->batch;
         return bytes + sizeof(float2) * N * slots + 65536;
     }
@@ -674,14 +666,13 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
     p.work = p.spec + (size_t)p.N * a->batch;
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    if (p.log2N1 == 10 && p.log2N2 == 9 && !getenv("AFB200_CWT_GENERIC")) {
-        // warp-level transforms (see k_cwt_cols_w / k_cwt_rows_w)
+    if (cwt_fused_enabled(a)) {
+        // warp-level transforms (see k_cwt_cols_w / k_cwt_rows_w): forward legs, then both inverse legs fused
         const size_t smC = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (1024 + p.N2 + 1024);
         const size_t smR = sizeof(c64) * (size_t)kWRows * kWRowPitch + sizeof(float2) * 512;
-        if ((rc = set_smem(k_cwt_cols_w<0>, smC, "smem k_cwt_cols_w<0>")) || (rc = set_smem(k_cwt_cols_w<1>, smC, "smem k_cwt_cols_w<1>")) ||
-            (rc = set_smem(k_cwt_rows_w<0>, smR, "smem k_cwt_rows_w<0>")) || (rc = set_smem(k_cwt_rows_w<1>, smR, "smem k_cwt_rows_w<1>"))) return rc;
+        if ((rc = set_smem(k_cwt_cols_w<0>, smC, "smem k_cwt_cols_w<0>")) || (rc = set_smem(k_cwt_rows_w<0>, smR, "smem k_cwt_rows_w<0>"))) return rc;
         const unsigned cb = (unsigned)(p.N2 / kWCols), rb = (unsigned)(p.N1 / kWRows), items = (unsigned)(a->batch * a->num);
-        if (a->support && a->supportReady && !getenv("AFB200_CWT_NOPRUNE")) {
+        if (a->support && a->supportReady) {
             if (!*a->supportReady) {                       // once per object: peak and [lo, hi) of every bank row
                 cudaError_t e = cudaMemsetAsync(a->support, 0x7f, sizeof(int) * (size_t)a->num, st);
                 if (e == cudaSuccess) e = cudaMemsetAsync(a->support + a->num, 0, sizeof(int) * 2 * (size_t)a->num, st);
@@ -703,66 +694,24 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
             AF_LAUNCH_CHECK("k_cwt_rows_w<0>");
         }
         if (a->forwardOnly) return AF_OK;
-        if (cwt_fused_enabled(a)) {
-            FusedParams f;
-            f.p = p;
-            f.items = (int)items; f.groupItems = cwt_group_items(); f.groups = (f.items + f.groupItems - 1) / f.groupItems;
-            f.cb = (int)cb; f.rb = (int)rb;
-            {
-                size_t slots = (size_t)kRing * f.groupItems;
-                if ((size_t)a->batch > slots) slots = (size_t)a->batch;
-                f.counters = reinterpret_cast<unsigned *>(p.work + (size_t)p.N * slots);
-            }
-            if ((size_t)(1 + 2 * f.groups) * sizeof(unsigned) > 65536) return af_fail(AF_ERR_UNSUPPORTED, "CWT: %d item groups exceed the counter block", f.groups);
-            cudaError_t e = cudaMemsetAsync(f.counters, 0, (size_t)(1 + 2 * f.groups) * sizeof(unsigned), st);
-            if (e != cudaSuccess) return af_cuda_check(e, "cudaMemsetAsync(cwt counters)");
-            const size_t smF = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (2048 + p.N2 + 512);
-            if ((rc = set_smem(k_cwt_fused_w, smF, "smem k_cwt_fused_w"))) return rc;
-            int sms = af_sm_count();
-            if (sms <= 0) sms = 132;
-            // Optional (AFB200_CWT_L2PERSIST=1): pin the ring in L2 with a persisting access-policy window on this stream.  The
-            // set-aside takes L2 away from the spectrum reads and the result stores, so the default is off: streaming result
-            // stores already keep the ring's lines in L2 for most of their life.
-            const char *pe = getenv("AFB200_CWT_L2PERSIST");
-            const bool persist = pe && pe[0] == '1';
-            const size_t ringBytes = sizeof(float2) * (size_t)p.N * kRing * f.groupItems;
-            if (persist) {
-                static int limitSet = 0;
-                int dev = 0, maxPersist = 0, maxWindow = 0;
-                cudaGetDevice(&dev);
-                cudaDeviceGetAttribute(&maxPersist, cudaDevAttrMaxPersistingL2CacheSize, dev);
-                cudaDeviceGetAttribute(&maxWindow, cudaDevAttrMaxAccessPolicyWindowSize, dev);
-                if (maxPersist > 0 && maxWindow > 0) {
-                    if (!limitSet) { cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)maxPersist); limitSet = 1; }
-                    cudaStreamAttrValue av;
-                    memset(&av, 0, sizeof(av));
-                    av.accessPolicyWindow.base_ptr = p.work;
-                    av.accessPolicyWindow.num_bytes = ringBytes < (size_t)maxWindow ? ringBytes : (size_t)maxWindow;
-                    av.accessPolicyWindow.hitRatio = ringBytes <= (size_t)maxPersist ? 1.0f : (float)((double)maxPersist / (double)ringBytes);
-                    av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-                    av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-                    cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &av);
-                    cudaGetLastError();
-                }
-            }
-            k_cwt_fused_w<<<(unsigned)(2 * sms), 256, smF, st>>>(f);
-            AF_LAUNCH_CHECK("k_cwt_fused_w");
-            if (persist) {
-                cudaStreamAttrValue av;
-                memset(&av, 0, sizeof(av));                          // num_bytes = 0: window off for whatever follows on this stream
-                cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &av);
-                cudaGetLastError();
-            }
-            return AF_OK;
+        FusedParams f;
+        f.p = p;
+        f.items = (int)items; f.groupItems = kGroupItems; f.groups = (f.items + f.groupItems - 1) / f.groupItems;
+        f.cb = (int)cb; f.rb = (int)rb;
+        {
+            size_t slots = (size_t)kRing * f.groupItems;
+            if ((size_t)a->batch > slots) slots = (size_t)a->batch;
+            f.counters = reinterpret_cast<unsigned *>(p.work + (size_t)p.N * slots);
         }
-        for (unsigned i0 = 0; i0 < items; i0 += items) {
-            CwtParams q = p;
-            q.itemBase = (int)i0;
-            k_cwt_cols_w<1><<<dim3(items, cb), kWCols * 32, smC, st>>>(q);
-            AF_LAUNCH_CHECK("k_cwt_cols_w<1>");
-            k_cwt_rows_w<1><<<dim3(items, rb), kWRows * 16, smR, st>>>(q);
-            AF_LAUNCH_CHECK("k_cwt_rows_w<1>");
-        }
+        if ((size_t)(1 + 2 * f.groups) * sizeof(unsigned) > 65536) return af_fail(AF_ERR_UNSUPPORTED, "CWT: %d item groups exceed the counter block", f.groups);
+        cudaError_t e = cudaMemsetAsync(f.counters, 0, (size_t)(1 + 2 * f.groups) * sizeof(unsigned), st);
+        if (e != cudaSuccess) return af_cuda_check(e, "cudaMemsetAsync(cwt counters)");
+        const size_t smF = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (2048 + p.N2 + 512);
+        if ((rc = set_smem(k_cwt_fused_w, smF, "smem k_cwt_fused_w"))) return rc;
+        int sms = af_sm_count();
+        if (sms <= 0) sms = 132;
+        k_cwt_fused_w<<<(unsigned)(2 * sms), 256, smF, st>>>(f);
+        AF_LAUNCH_CHECK("k_cwt_fused_w");
         return AF_OK;
     }
     const int threads = 512;

@@ -38,36 +38,18 @@ namespace {
 
 constexpr int kN = 2048;            // fftLength
 constexpr int kNC = 1024;           // packed complex points
-#ifndef AF_FRAME_WARPS
-#define AF_FRAME_WARPS 13
-#endif
-constexpr int kFrameWarps = AF_FRAME_WARPS;     // consumer warps = max frames per tile (<= 16: one mma M tile); 13 by default
-#ifndef AF_ABLATE
-#define AF_ABLATE 0     // diagnostic timing builds: 1 no bank loop, 2 no post-pass, 4 no FFTs, 8 no transposes, 16 no window/sample loads
-#endif
-#ifndef AF_EPI_WARPS
-#define AF_EPI_WARPS 2
-#endif
-#ifndef AF_CTAS_PER_SM
-#define AF_CTAS_PER_SM 1
-#endif
-constexpr int kEpiWarps = AF_EPI_WARPS;   // DCT epilogue warps; tile `it` is served by warp it % kEpiWarps
-constexpr int kCtasPerSm = AF_CTAS_PER_SM;   // independent CTAs per SM drift apart, so their phases (LSU-heavy load /
-                                             // transpose / bank vs FMA-heavy FFT) overlap instead of queueing on one pipe
+constexpr int kFrameWarps = 13;     // consumer warps = max frames per tile (<= 16: one mma M tile)
+constexpr int kEpiWarps = 2;        // DCT epilogue warps; tile `it` is served by warp it % kEpiWarps
 constexpr int kThreads = (kFrameWarps + 1 + kEpiWarps) * 32;   // + TMA producer warp + DCT epilogue warps
 constexpr int kMaxPeers = 15;      // extra destinations of the output tile (P2P stores to peer GPUs)
 constexpr int kLPitch = 132;        // log-mel tile row pitch (floats): 4g + t -> 32 distinct banks for mma A fragments
-constexpr int kLRows = kFrameWarps <= 8 ? 8 : 16;   // stored rows of the mma M=16 tile (rows beyond are zeros)
+constexpr int kLRows = 16;          // stored rows of the mma M=16 tile (rows >= kFrameWarps are zeros)
 constexpr int kStages = 2;
-#ifndef AF_LBUFS
-#define AF_LBUFS 3
-#endif
-constexpr int kLBufs = AF_LBUFS;    // log-mel tiles in flight between the frame warps and the DCT epilogue (2 leaves frame
+constexpr int kLBufs = 3;           // log-mel tiles in flight between the frame warps and the DCT epilogue (2 leaves frame
                                     // warps waiting for the epilogue)
 constexpr int kMaxNum = 128;        // filters (padded)
 constexpr int kScratchFloats = 1152;            // per warp: 33x32 float transpose plane, later Ps[0..1024] + zero pad
 constexpr int kPsPad = 1152;        // Ps[0..1024], zeros up to kPsPad (padded band reads)
-constexpr int kTailMax = 512;       // bins above the last filter's peak (interval mode)
 constexpr int kStageBytes = 16 * 64 * 4;   // result tile of one epilogue warp (<= 16 frames x 64 coefficients), source of the bulk stores
 
 struct Plan {                       // host-side descriptor of the device tables
@@ -81,10 +63,6 @@ struct Plan {                       // host-side descriptor of the device tables
     int melGroups;
     int melWFloats;
     int num, ccNum, ct, dataType;
-    // interval ("shared product") form of a triangular bank, see build_intervals()
-    int melMode;                    // 0: lane per filter over its whole support; 1: lane per interval
-    float *dMelAux;                 // [128 gains][kTailMax tail weights]
-    int tailStart, tailLen;
 };
 
 struct Params {
@@ -102,9 +80,7 @@ struct Params {
     int spanFloats;                 // floats per stage buffer
     int melGroups, melWFloats;
     int melGroupLen[4];
-    int melMode, num, tailStart, tailLen;
-    const float *melAux;
-    int ccNum, rectify, dataType;
+    int num, ccNum, rectify, dataType;
     int rawMel;                     // 1: stop after the bank: out[frame][num] = bank . |X|^2 (bftObj_bft real mode), no log / DCT
     int bulkStore;                  // 1: the result tile leaves as one TMA bulk store per destination (16-byte aligned rows)
     // fused all-gather: every finished tile is also stored at the same offset of up to kMaxPeers other buffers
@@ -115,7 +91,7 @@ struct Params {
 
 // shared-memory carve-up (bytes), all 16-byte aligned
 struct Smem {
-    int spanOff, scratchOff, windowOff, tw1Off, tw2Off, melWOff, melStartOff, melAuxOff, dctOff, lOff, stageOff, barOff, total;
+    int spanOff, scratchOff, windowOff, tw1Off, tw2Off, melWOff, melStartOff, dctOff, lOff, stageOff, barOff, total;
 };
 
 __host__ __device__ inline Smem carve(int spanFloats, int melWFloats, int ct) {
@@ -127,7 +103,6 @@ __host__ __device__ inline Smem carve(int spanFloats, int melWFloats, int ct) {
     s.tw2Off = o;      o += 32 * 8;
     s.melWOff = o;     o += ((melWFloats * 4 + 15) / 16) * 16;
     s.melStartOff = o; o += kMaxNum * 4;
-    s.melAuxOff = o;   o += (kMaxNum + kTailMax) * 4;
     s.dctOff = o;      o += kMaxNum * (ct <= 5 ? 40 : 72) * 4;
     s.lOff = o;        o += kLBufs * kLRows * kLPitch * 4;
     s.stageOff = o;    o += kEpiWarps * kStageBytes;
@@ -136,8 +111,8 @@ __host__ __device__ inline Smem carve(int spanFloats, int melWFloats, int ct) {
     return s;
 }
 
-template <int CT, int MODE>
-__global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
+template <int CT>
+__global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
     extern __shared__ __align__(128) unsigned char smem[];
     const Smem L = carve(p.spanFloats, p.melWFloats, CT);
     float *span = reinterpret_cast<float *>(smem + L.spanOff);
@@ -147,7 +122,6 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
     float2 *sTw2 = reinterpret_cast<float2 *>(smem + L.tw2Off);
     float *sMelW = reinterpret_cast<float *>(smem + L.melWOff);
     int *sMelStart = reinterpret_cast<int *>(smem + L.melStartOff);
-    float *sMelAux = reinterpret_cast<float *>(smem + L.melAuxOff);     // interval mode: [128 gains][tail weights]
     float *sDct = reinterpret_cast<float *>(smem + L.dctOff);
     float *sL = reinterpret_cast<float *>(smem + L.lOff);                 // [kLBufs][kLRows][kLPitch] log-mel tiles
     uint64_t *fullBar = reinterpret_cast<uint64_t *>(smem + L.barOff);
@@ -164,7 +138,6 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
     for (int i = threadIdx.x; i < 32; i += kThreads) sTw2[i] = p.tw2[i];
     for (int i = threadIdx.x; i < p.melWFloats; i += kThreads) sMelW[i] = p.melW[i];
     for (int i = threadIdx.x; i < kMaxNum; i += kThreads) sMelStart[i] = p.melStart[i];
-    for (int i = threadIdx.x; i < kMaxNum + kTailMax; i += kThreads) sMelAux[i] = MODE ? p.melAux[i] : 0.0f;
     for (int i = threadIdx.x; i < kMaxNum * kDctPitch; i += kThreads) sDct[i] = p.dct[i];
     for (int i = threadIdx.x; i < kLBufs * kLRows * kLPitch; i += kThreads) sL[i] = 0.0f;
     if (threadIdx.x == 0) {
@@ -226,8 +199,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
         : "r"(A0), "r"(A1), "r"(A2), "r"(A3), "r"(B0), "r"(B1))
 #pragma unroll 2
             for (int k0 = 0; k0 < kMaxNum; k0 += 8) {
-                const float af[4] = {A[g * kLPitch + k0 + t], kLRows > 8 ? A[(g + 8) * kLPitch + k0 + t] : 0.0f,
-                                     A[g * kLPitch + k0 + t + 4], kLRows > 8 ? A[(g + 8) * kLPitch + k0 + t + 4] : 0.0f};
+                const float af[4] = {A[g * kLPitch + k0 + t], A[(g + 8) * kLPitch + k0 + t],
+                                     A[g * kLPitch + k0 + t + 4], A[(g + 8) * kLPitch + k0 + t + 4]};
                 // TF32 split by truncation: hi = top 19 bits, lo = (x - hi) (exact), again cut to 19 bits
                 uint32_t ah[4], al[4], bh[CT][2], bl[CT][2];
 #pragma unroll
@@ -332,7 +305,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
             // ---- A: load 2048 samples (1024 packed pairs), apply 0.5*window ----
             const c64 *sp = reinterpret_cast<const c64 *>(span + (size_t)stage * p.spanFloats + warp * p.hop);
 #pragma unroll
-            for (int j = 0; j < 32; j++) z[j] = (AF_ABLATE & 16) ? c_pack(1.0f + j, lane) : v_mul(sp[lane + 32 * j], sWinC[lane + 32 * j]);
+            for (int j = 0; j < 32; j++) z[j] = v_mul(sp[lane + 32 * j], sWinC[lane + 32 * j]);
         }
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&emptyBar[stage]);     // span slot may be refilled
@@ -349,7 +322,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
         }
 
         // ---- B: 1024-point FFT as 32 x 32 ----
-        if (!(AF_ABLATE & 4)) af_fft32(z);                    // over n2; Y[n1=lane][ka] at AF_BR5(ka)
+        af_fft32(z);                                          // over n2; Y[n1=lane][ka] at AF_BR5(ka)
         {
             float yr[32], yi[32];
 #pragma unroll
@@ -360,7 +333,6 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
                 c_unpack(y, yr[ka], yi[ka]);
             }
             // 32 x 32 transpose, real plane then imaginary plane, through one 33-padded float buffer
-            if (!(AF_ABLATE & 8)) {
 #pragma unroll
             for (int ka = 0; ka < 32; ka++) scratch[ka * 33 + lane] = yr[ka];
             __syncwarp();
@@ -373,18 +345,14 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
 #pragma unroll
             for (int n1 = 0; n1 < 32; n1++) z[n1] = c_pack(yr[n1], scratch[lane * 33 + n1]);
             __syncwarp();
-            } else {
-#pragma unroll
-                for (int n1 = 0; n1 < 32; n1++) z[n1] = c_pack(yr[n1], yi[n1]);
-            }
         }
-        if (!(AF_ABLATE & 4)) af_fft32(z);                    // over n1; Z[lane + 32*kb] at AF_BR5(kb)
+        af_fft32(z);                                          // over n1; Z[lane + 32*kb] at AF_BR5(kb)
 
         // ---- C: real-FFT post-pass + power / magnitude -> Ps[0..1024] ----
         // (window pre-scaled by 1/2, so E' = Z[k] + conj Z[N-k] and O' = -i (Z[k] - conj Z[N-k]) need no halving;
         //  X[k] = E' + W O', conj X[N-k] = E' - W O' with W = W_2048^k = W_2048^lane * W_64^kb)
 #pragma unroll
-        for (int kb = 0; kb < ((AF_ABLATE & 2) ? 1 : 16); kb++) {
+        for (int kb = 0; kb < 16; kb++) {
             const c64 zk = z[AF_BR5(kb)];
             float pr, pi;
             c_unpack(z[AF_BR5(31 - kb)], pr, pi);
@@ -417,98 +385,40 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
 
         // ---- D: banded filter bank (lane = filter within group, bank-conflict-free starts) + rectify ----
         if (!p.rawMel) af_mbar_wait(&lEmpty[lbuf], ((uint32_t)(it / kLBufs) & 1u) ^ 1u);   // epilogue done with tile it-kLBufs
-        if (MODE) {
-            // Interval form of a triangular bank (two filters overlap on every bin and their weights there sum to the
-            // filters' gains: fall_m(k) = g_m (1 - r_{m+1}(k))).  Lane j owns interval j = the bins between the peaks
-            // of filters j-1 and j and accumulates A_j = sum r_j P and S_j = sum P ONCE; then
-            //     mel_m = g_m (A_m + (S_{m+1} - A_{m+1})),
-            // i.e. every bin is read and multiplied once instead of twice (half the shared-memory traffic of the
-            // filter-per-lane loop).  Padded slots carry r = 0 and are masked out of S by the (r > 0) test.
-            const float4 *wg4 = reinterpret_cast<const float4 *>(sMelW) + lane;
-            float A[4], U[4];
-#pragma unroll
-            for (int g = 0; g < 4; g++) {
-                A[g] = 0.0f; U[g] = 0.0f;
-                if (g >= p.melGroups) continue;
-                const int len4 = (AF_ABLATE & 1) ? 0 : p.melGroupLen[g] >> 2;
-                const float2 *ps2 = reinterpret_cast<const float2 *>(scratch + sMelStart[g * 32 + lane]);
-                float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f, a3 = 0.0f, s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
-                float4 w = wg4[0];
-                float2 p0 = ps2[0], p1 = ps2[1];
+        // weights: per group [len/4][32 lanes] float4 (LDS.128); P: two LDS.64 per 4 taps (starts are even and
+        // spread over distinct 8-byte bank pairs per half-warp by the host planner)
+        const float4 *wg4 = reinterpret_cast<const float4 *>(sMelW) + lane;
+        for (int g = 0; g < p.melGroups; g++) {
+            const int len4 = p.melGroupLen[g] >> 2;
+            const float2 *ps2 = reinterpret_cast<const float2 *>(scratch + sMelStart[g * 32 + lane]);
+            float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f, acc3 = 0.0f;
+            // software pipelined: the loads of stage i+1 are in flight while stage i is accumulated
+            // (the final prefetch over-reads one stage: the tables carry the padding).  A two-stage-deep
+            // pipeline needs 128 registers and a longer prologue per group.
+            float4 w = wg4[0];
+            float2 p0 = ps2[0], p1 = ps2[1];
 #pragma unroll 2
-                for (int i = 0; i < len4; i++) {
-                    const float4 wn = wg4[(i + 1) * 32];
-                    const float2 q0 = ps2[2 * i + 2], q1 = ps2[2 * i + 3];
-                    a0 = fmaf(p0.x, w.x, a0); a1 = fmaf(p0.y, w.y, a1); a2 = fmaf(p1.x, w.z, a2); a3 = fmaf(p1.y, w.w, a3);
-                    if (!(AF_ABLATE & 32)) {
-                        s0 = fmaf(p0.x, w.x > 0.0f ? 1.0f : 0.0f, s0); s1 = fmaf(p0.y, w.y > 0.0f ? 1.0f : 0.0f, s1);
-                        s2 = fmaf(p1.x, w.z > 0.0f ? 1.0f : 0.0f, s2); s3 = fmaf(p1.y, w.w > 0.0f ? 1.0f : 0.0f, s3);
-                    }
-                    w = wn; p0 = q0; p1 = q1;
-                }
-                A[g] = (a0 + a1) + (a2 + a3);
-                U[g] = ((s0 + s1) + (s2 + s3)) - A[g];
+            for (int i = 0; i < len4; i++) {
+                const float4 wn = wg4[(i + 1) * 32];
+                const float2 q0 = ps2[2 * i + 2], q1 = ps2[2 * i + 3];
+                acc0 = fmaf(p0.x, w.x, acc0);
+                acc1 = fmaf(p0.y, w.y, acc1);
+                acc2 = fmaf(p1.x, w.z, acc2);
+                acc3 = fmaf(p1.y, w.w, acc3);
+                w = wn; p0 = q0; p1 = q1;
+            }
+            float v = (acc0 + acc1) + (acc2 + acc3);
+            if (p.rawMel) {                                  // coalesced: one 128-byte row segment per group
+                if (g * 32 + lane < p.num) melRow[g * 32 + lane] = v;
                 wg4 += len4 * 32;
+                continue;
             }
-            // tail interval (above the last filter's peak): its falling weights directly, one bin per lane
-            float ut = 0.0f;
-            if (!(AF_ABLATE & 64)) for (int i = lane; i < p.tailLen; i += 32) ut = fmaf(scratch[p.tailStart + i], sMelAux[kMaxNum + i], ut);
-            if (!(AF_ABLATE & 64))
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) ut += __shfl_xor_sync(0xffffffffu, ut, o);
-#pragma unroll
-            for (int g = 0; g < 4; g++) {
-                if (g >= p.melGroups) { lrow[g * 32 + lane] = 0.0f; continue; }
-                float un = U[g];
-                if (!(AF_ABLATE & 64)) {
-                    un = __shfl_down_sync(0xffffffffu, U[g], 1);
-                    const float nextFirst = __shfl_sync(0xffffffffu, U[g < 3 ? g + 1 : 3], 0);
-                    if (lane == 31) un = nextFirst;
-                }
-                const int m = g * 32 + lane;
-                if (m + 1 == p.num) un = ut;
-                float v = m < p.num ? sMelAux[m] * (A[g] + un) : 0.0f;
-                if (p.rectify == CepstralRectify_CubicRoot) v = powf(v, 1.0f / 3.0f);
-                else v = __log2f(v < 1e-8f ? 1e-8f : v) * 0.30102999566398120f;
-                lrow[m] = m < p.num ? v : 0.0f;
-            }
-        } else
-        {
-            // weights: per group [len/4][32 lanes] float4 (LDS.128); P: two LDS.64 per 4 taps (starts are even and
-            // spread over distinct 8-byte bank pairs per half-warp by the host planner)
-            const float4 *wg4 = reinterpret_cast<const float4 *>(sMelW) + lane;
-            for (int g = 0; g < p.melGroups; g++) {
-                const int len4 = (AF_ABLATE & 1) ? 0 : p.melGroupLen[g] >> 2;
-                const float2 *ps2 = reinterpret_cast<const float2 *>(scratch + sMelStart[g * 32 + lane]);
-                float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f, acc3 = 0.0f;
-                // software pipelined: the loads of stage i+1 are in flight while stage i is accumulated
-                // (the final prefetch over-reads one stage: the tables carry the padding).  A two-stage-deep
-                // pipeline needs 128 registers and a longer prologue per group.
-                float4 w = wg4[0];
-                float2 p0 = ps2[0], p1 = ps2[1];
-#pragma unroll 2
-                for (int i = 0; i < len4; i++) {
-                    const float4 wn = wg4[(i + 1) * 32];
-                    const float2 q0 = ps2[2 * i + 2], q1 = ps2[2 * i + 3];
-                    acc0 = fmaf(p0.x, w.x, acc0);
-                    acc1 = fmaf(p0.y, w.y, acc1);
-                    acc2 = fmaf(p1.x, w.z, acc2);
-                    acc3 = fmaf(p1.y, w.w, acc3);
-                    w = wn; p0 = q0; p1 = q1;
-                }
-                float v = (acc0 + acc1) + (acc2 + acc3);
-                if (p.rawMel) {                                  // coalesced: one 128-byte row segment per group
-                    if (g * 32 + lane < p.num) melRow[g * 32 + lane] = v;
-                    wg4 += len4 * 32;
-                    continue;
-                }
-                if (p.rectify == CepstralRectify_CubicRoot) v = powf(v, 1.0f / 3.0f);
-                else v = __log2f(v < 1e-8f ? 1e-8f : v) * 0.30102999566398120f;   // log10 via MUFU.LG2
-                lrow[g * 32 + lane] = v;
-                wg4 += len4 * 32;
-            }
-            if (!p.rawMel) for (int g = p.melGroups; g < 4; g++) lrow[g * 32 + lane] = 0.0f;
+            if (p.rectify == CepstralRectify_CubicRoot) v = powf(v, 1.0f / 3.0f);
+            else v = __log2f(v < 1e-8f ? 1e-8f : v) * 0.30102999566398120f;   // log10 via MUFU.LG2
+            lrow[g * 32 + lane] = v;
+            wg4 += len4 * 32;
         }
+        if (!p.rawMel) for (int g = p.melGroups; g < 4; g++) lrow[g * 32 + lane] = 0.0f;
         __syncwarp();
         if (!p.rawMel && lane == 0) af_mbar_arrive(&lFull[lbuf]);           // row ready for the tensor-core DCT epilogue
 
@@ -518,7 +428,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) k_mfcc_fused(Params p) {
 void free_plan(Plan *pl) {
     if (!pl) return;
     af_dev_free(pl->dWindowHalf); af_dev_free(pl->dTw1); af_dev_free(pl->dTw2);
-    af_dev_free(pl->dMelW); af_dev_free(pl->dMelStart); af_dev_free(pl->dDct); af_dev_free(pl->dMelAux);
+    af_dev_free(pl->dMelW); af_dev_free(pl->dMelStart); af_dev_free(pl->dDct);
     free(pl);
 }
 
@@ -529,7 +439,8 @@ void free_plan(Plan *pl) {
 // where the group's length budget allows, spreads the 16 starts of a half-warp over different 8-byte bank
 // pairs.  The budget is the longest filter of the group (+1 for parity) rounded up to 4 taps, so short groups
 // of adjacent filters accept a 2-way conflict instead of padding; longest filters are placed first.
-static int plan_rows(const int *rowStart, const int *rowLen, int num, int *startShifted /* kMaxNum */, int *groupLen /* 4 */) {
+static int plan_mel(const AfBands *bands, int num, int *startShifted /* kMaxNum */, int *groupLen /* 4 */) {
+    const int *rowStart = bands->start, *rowLen = bands->len;
     int total = 0;
     for (int m = 0; m < kMaxNum; m++) startShifted[m] = 0;
     for (int g = 0; g < 4; g++) groupLen[g] = 0;
@@ -563,92 +474,6 @@ static int plan_rows(const int *rowStart, const int *rowLen, int num, int *start
     return total + 8 * 32;                                    // two stages of padding for the pipelined prefetch
 }
 
-static int plan_mel(const AfBands *bands, int num, int *startShifted, int *groupLen) {
-    return plan_rows(bands->start, bands->len, num, startShifted, groupLen);
-}
-
-// ---- interval form of a triangular bank ---------------------------------------------------------------------
-// Accepts a bank in which (i) every bin is covered by at most two filters, consecutive ones, and (ii) where filters
-// m-1 and m overlap, bank[m-1][k] / g_{m-1} + bank[m][k] / g_m = 1 (g = per-filter gain of the normalisation; the
-// Slaney and ETSI triangles of auditory_filterBank.c:373-500 have this form by construction).  Then bin k belongs to
-// exactly one interval j(k) (between the peaks of filters j-1 and j) with rising weight r[k] = bank[j][k] / g_j, and
-//     mel_m = g_m ( sum_{I_m} r P  +  sum_{I_{m+1}} (1 - r) P ).
-// Interval `num` (above the last peak) keeps the last filter's own falling weights (tail).  Verified numerically
-// against the actual table with tolerance kTriTol; any violation -> the generic filter-per-lane path is used.
-constexpr float kTriTol = 2e-6f;
-struct Intervals {
-    int start[kMaxNum + 1], len[kMaxNum + 1];
-    float r[kNC + 1];
-    int owner[kNC + 1];             // interval of each bin, -1 = none
-    float tailW[kTailMax];
-    int tailStart, tailLen;
-};
-
-static bool build_intervals(const float *bank, const AfBands *bands, int num, const float *gain, Intervals *iv) {
-    const int width = kNC + 1;
-    if (num < 2 || num > kMaxNum) return false;
-    int peak[kMaxNum];
-    for (int m = 0; m < num; m++) {
-        peak[m] = -1;
-        if (!(gain[m] > 0.0f)) return false;
-        if (bands->len[m] <= 0) continue;                    // a triangle narrower than the bin spacing: no bins, mel = 0
-        int best = bands->start[m];
-        for (int k = bands->start[m]; k < bands->start[m] + bands->len[m]; k++)
-            if (bank[(size_t)m * width + k] > bank[(size_t)m * width + best]) best = k;
-        peak[m] = best;
-    }
-    for (int k = 0; k < width; k++) { iv->r[k] = 0.0f; iv->owner[k] = -1; }
-    int lo = 0;                                              // filters are ordered: first candidate cover of bin k
-    int prevOwner = -1;
-    for (int k = 0; k < width; k++) {
-        int cover[3], nc = 0;
-        while (lo < num && bands->start[lo] + bands->len[lo] <= k) lo++;
-        for (int m = lo; m < num && bands->start[m] <= k && nc < 3; m++)
-            if (k < bands->start[m] + bands->len[m] && bank[(size_t)m * width + k] != 0.0f) cover[nc++] = m;
-        if (nc == 0) continue;
-        if (nc > 2 || (nc == 2 && cover[1] != cover[0] + 1)) return false;
-        int j; float r;
-        if (nc == 2) {
-            const int a = cover[0];
-            j = a + 1;
-            r = bank[(size_t)j * width + k] / gain[j];
-            if (fabsf(bank[(size_t)a * width + k] / gain[a] - (1.0f - r)) > kTriTol) return false;
-        } else {
-            // a bin under one filter only: the filter's centre bin (weight = gain), or the outer flank of the first /
-            // last filter (an inner flank would be shared with the neighbouring filter)
-            const int m = cover[0];
-            const float w = bank[(size_t)m * width + k] / gain[m];
-            if (fabsf(1.0f - w) <= kTriTol) { j = m; r = 1.0f; }
-            else if (m == 0 && k <= peak[0]) { j = 0; r = w; }
-            else if (m == num - 1 && k >= peak[m]) { j = num; r = 1.0f - w; }
-            else return false;
-        }
-        if (!(r > 0.0f) && j < num) r = 1e-30f;
-        if (j < prevOwner) return false;                     // intervals must be runs of consecutive bins
-        prevOwner = j;
-        iv->owner[k] = j;
-        iv->r[k] = r;
-    }
-    for (int j = 0; j <= num; j++) { iv->start[j] = 0; iv->len[j] = 0; }
-    for (int k = 0; k < width; k++) {
-        const int j = iv->owner[k];
-        if (j < 0) continue;
-        if (iv->len[j] == 0) iv->start[j] = k;
-        iv->len[j] = k - iv->start[j] + 1;
-    }
-    iv->tailStart = iv->start[num]; iv->tailLen = iv->len[num];
-    if (iv->tailLen > kTailMax) return false;
-    for (int i = 0; i < kTailMax; i++) iv->tailW[i] = 0.0f;
-    for (int i = 0; i < iv->tailLen; i++) {
-        const int k = iv->tailStart + i;
-        iv->tailW[i] = iv->owner[k] == num ? bank[(size_t)(num - 1) * width + k] / gain[num - 1] : 0.0f;
-    }
-    // empty intervals read (and ignore) the bins where they would sit, keeping the lanes' starts monotone
-    int last = 0;
-    for (int j = 0; j < num; j++) { if (iv->len[j] == 0) iv->start[j] = last; else last = iv->start[j] + iv->len[j]; }
-    return true;
-}
-
 extern "C" int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const AfBands *bands) {
     if (fftLength != kN || num < 1 || num > kMaxNum || ccNum < 1 || ccNum > 64 || !bands) return 0;
     int starts[kMaxNum], groupLen[4];
@@ -658,11 +483,11 @@ extern "C" int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const 
 }
 
 extern "C" void af_mfcc_plan_free(void *plan) { free_plan(static_cast<Plan *>(plan)); }
-extern "C" int af_mfcc_plan_mode(void *plan) { return plan ? static_cast<Plan *>(plan)->melMode : -1; }
+extern "C" int af_mfcc_plan_mode(void *plan) { return plan ? 0 : -1; }
 
 extern "C" int af_mfcc_plan_build(void **planOut, int fftLength, int num, int ccNum, const float *window,
                                   const float *bank, const AfBands *bands, const float *dct /* ccNum x num */,
-                                  int dataType, const float *gain /* num per-filter normalisation gains, or NULL */) {
+                                  int dataType) {
     *planOut = NULL;
     if (!af_mfcc_fused_supported(fftLength, num, ccNum, bands)) return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC plan: unsupported configuration");
     Plan *pl = static_cast<Plan *>(calloc(1, sizeof(Plan)));
@@ -694,67 +519,22 @@ extern "C" int af_mfcc_plan_build(void **planOut, int fftLength, int num, int cc
     const int width = kNC + 1;
     pl->melGroups = (num + 31) / 32;
     int starts[kMaxNum];
-    Intervals *iv = static_cast<Intervals *>(malloc(sizeof(Intervals)));
-    // The interval loop is opt-in (AFB200_MFCC_BANK_MODE=1): it halves the bank loop's shared-memory traffic, but the
-    // kernel is bound by the latency of queued MIO operations per warp, and the interval form adds a serial tail (warp
-    // reduction of the last interval + neighbour exchange by shuffles) that can outweigh the shorter loop.
-    const char *force = getenv("AFB200_MFCC_BANK_MODE");
-    float ones[kMaxNum];
-    for (int m = 0; m < kMaxNum; m++) ones[m] = 1.0f;
-    pl->melMode = 0;
-    if (iv && force && force[0] == '1' && build_intervals(bank, bands, num, gain ? gain : ones, iv)) {
-        int glen[4];
-        const int tot = plan_rows(iv->start, iv->len, num, starts, glen);
-        bool fits = tot * 4 <= 24 * 1024;
-        for (int g = 0; g < 4; g++) if (glen[g] + 8 > kPsPad - (kNC + 1)) fits = false;
-        if (fits) {
-            pl->melMode = 1;
-            pl->melWFloats = tot;
-            for (int g = 0; g < 4; g++) pl->melGroupLen[g] = glen[g];
-            pl->tailStart = iv->tailStart; pl->tailLen = iv->tailLen;
+    const int total = plan_mel(bands, num, starts, pl->melGroupLen);
+    pl->melWFloats = total;
+    float *mw = static_cast<float *>(calloc((size_t)(total > 0 ? total : 1), sizeof(float)));
+    int off = 0;
+    for (int g = 0; g < pl->melGroups; g++) {
+        for (int l = 0; l < 32; l++) {
+            const int m = g * 32 + l;
+            if (m >= num) continue;
+            const int delta = bands->start[m] - starts[m];
+            for (int i = 0; i < bands->len[m]; i++)
+                mw[off + ((i + delta) >> 2) * 128 + l * 4 + ((i + delta) & 3)] = bank[(size_t)m * width + bands->start[m] + i];
         }
+        off += pl->melGroupLen[g] * 32;
     }
-    if (pl->melMode == 1) {
-        const int total = pl->melWFloats;
-        float *mw = static_cast<float *>(calloc((size_t)total, sizeof(float)));
-        int off = 0;
-        for (int g = 0; g < pl->melGroups; g++) {
-            for (int l = 0; l < 32; l++) {
-                const int j = g * 32 + l;
-                if (j >= num) continue;
-                const int delta = iv->start[j] - starts[j];
-                for (int i = 0; i < iv->len[j]; i++) {
-                    const int k = iv->start[j] + i;
-                    if (iv->owner[k] == j) mw[off + ((i + delta) >> 2) * 128 + l * 4 + ((i + delta) & 3)] = iv->r[k];
-                }
-            }
-            off += pl->melGroupLen[g] * 32;
-        }
-        float aux[kMaxNum + kTailMax];
-        for (int m = 0; m < kMaxNum; m++) aux[m] = m < num ? (gain ? gain[m] : 1.0f) : 0.0f;
-        for (int i = 0; i < kTailMax; i++) aux[kMaxNum + i] = iv->tailW[i];
-        if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelW), mw, sizeof(float) * (size_t)total);
-        if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelAux), aux, sizeof(aux));
-        free(mw);
-    } else {
-        const int total = plan_mel(bands, num, starts, pl->melGroupLen);
-        pl->melWFloats = total;
-        float *mw = static_cast<float *>(calloc((size_t)(total > 0 ? total : 1), sizeof(float)));
-        int off = 0;
-        for (int g = 0; g < pl->melGroups; g++) {
-            for (int l = 0; l < 32; l++) {
-                const int m = g * 32 + l;
-                if (m >= num) continue;
-                const int delta = bands->start[m] - starts[m];
-                for (int i = 0; i < bands->len[m]; i++)
-                    mw[off + ((i + delta) >> 2) * 128 + l * 4 + ((i + delta) & 3)] = bank[(size_t)m * width + bands->start[m] + i];
-            }
-            off += pl->melGroupLen[g] * 32;
-        }
-        if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelW), mw, sizeof(float) * (size_t)(total > 0 ? total : 1));
-        free(mw);
-    }
-    free(iv);
+    if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelW), mw, sizeof(float) * (size_t)(total > 0 ? total : 1));
+    free(mw);
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelStart), starts, sizeof(int) * kMaxNum);
 
     // DCT table as the mma B operand: D^T[m][c] with row pitch 40 (72 for cc > 40): pitch % 32 == 8 makes the
@@ -785,24 +565,21 @@ static int launch_fused(void *plan, const float *data, int dataLength, int batch
     p.melW = pl->dMelW; p.melStart = pl->dMelStart; p.dct = pl->dDct;
     p.dataStride = dataLength; p.batch = batch; p.timeLength = timeLength; p.hop = slideLength;
     p.melGroups = pl->melGroups; p.melWFloats = pl->melWFloats;
-    p.melMode = pl->melMode; p.num = pl->num; p.tailStart = pl->tailStart; p.tailLen = pl->tailLen; p.melAux = pl->dMelAux;
+    p.num = pl->num;
     for (int g = 0; g < 4; g++) p.melGroupLen[g] = pl->melGroupLen[g];
     p.ccNum = pl->ccNum; p.rectify = rectifyType; p.dataType = pl->dataType;
     p.rawMel = rawMel;
-    if (rawMel && pl->melMode) return af_fail(AF_ERR_UNSUPPORTED, "fused filter-bank output needs the filter-per-lane plan");
     if (nPeer < 0 || nPeer > kMaxPeers || (nPeer > 0 && !peerOut)) return af_fail(AF_ERR_ARG, "fused MFCC: nPeer=%d outside [0, %d]", nPeer, kMaxPeers);
     p.nPeer = nPeer;
     for (int d = 0; d < nPeer; d++) p.peerOut[d] = peerOut[d];
     {   // one bulk store per destination needs 16-byte aligned tiles: ccNum % 4 == 0 and aligned bases
         int bulk = !rawMel && pl->ccNum % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
         for (int d = 0; d < nPeer; d++) if (reinterpret_cast<uintptr_t>(peerOut[d]) & 15) bulk = 0;
-        const char *sv = getenv("AFB200_MFCC_STORE");
-        if (sv && !strcmp(sv, "plain")) bulk = 0;
         p.bulkStore = bulk;
     }
 
     // frames per tile: as many as fit the shared-memory budget (<= kFrameWarps)
-    const int budget = kCtasPerSm == 1 ? 227 * 1024 : (233472 - kCtasPerSm * 1024) / kCtasPerSm;
+    const int budget = 227 * 1024;
     int F = kFrameWarps;
     for (; F >= 1; F--) {
         int spanFloats = (F - 1) * slideLength + kN;
@@ -818,21 +595,19 @@ static int launch_fused(void *plan, const float *data, int dataLength, int batch
 
     int sms = af_sm_count();
     if (sms <= 0) sms = 132;
-    long long grid = p.totalTiles < (long long)sms * kCtasPerSm ? p.totalTiles : (long long)sms * kCtasPerSm;
+    long long grid = p.totalTiles < (long long)sms ? p.totalTiles : (long long)sms;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaSuccess;
-#define AF_MFCC_LAUNCH2(CT_, MODE_)                                                                               \
-    e = cudaFuncSetAttribute(k_mfcc_fused<CT_, MODE_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smemBytes);  \
+#define AF_MFCC_LAUNCH(CT_)                                                                                       \
+    e = cudaFuncSetAttribute(k_mfcc_fused<CT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smemBytes);         \
     if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_mfcc_fused)");                          \
-    k_mfcc_fused<CT_, MODE_><<<(unsigned)grid, kThreads, smemBytes, st>>>(p)
-#define AF_MFCC_LAUNCH(CT_) if (pl->melMode) { AF_MFCC_LAUNCH2(CT_, 1); } else { AF_MFCC_LAUNCH2(CT_, 0); }
+    k_mfcc_fused<CT_><<<(unsigned)grid, kThreads, smemBytes, st>>>(p)
     switch (pl->ct) {
     case 2: AF_MFCC_LAUNCH(2); break;
     case 3: AF_MFCC_LAUNCH(3); break;
     case 5: AF_MFCC_LAUNCH(5); break;
     default: AF_MFCC_LAUNCH(8); break;
     }
-#undef AF_MFCC_LAUNCH2
 #undef AF_MFCC_LAUNCH
     AF_LAUNCH_CHECK("k_mfcc_fused");
     return AF_OK;
@@ -848,30 +623,4 @@ extern "C" int af_launch_mfcc_fused(void *plan, const float *data, int dataLengt
 extern "C" int af_launch_mel_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
                                    int slideLength, float *out, void *stream) {
     return launch_fused(plan, data, dataLength, batch, timeLength, slideLength, 0, out, 0, NULL, 1, stream);
-}
-
-// Diagnostic / test hook (host only, no device needed): the interval form the planner derives from a bank.
-// Returns 1 when the bank has the triangular two-overlap structure (then owner/r/tail/starts/groupLen are filled), else 0.
-extern "C" int afb200_mfccIntervalPlan(const float *bank, int num, const float *gain, int *owner /* 1025 */,
-                                       float *r /* 1025 */, int *ivStart /* num+1 */, int *ivLen /* num+1 */,
-                                       float *tailW /* 512 */, int *groupLen /* 4 */, int *startShifted /* 128 */) {
-    if (!bank || num < 2 || num > kMaxNum) return 0;
-    AfBands bands;
-    if (af_bands_build(bank, num, kNC + 1, &bands)) return 0;
-    Intervals *iv = static_cast<Intervals *>(malloc(sizeof(Intervals)));
-    float ones[kMaxNum];
-    for (int m = 0; m < kMaxNum; m++) ones[m] = 1.0f;
-    int ok = iv && build_intervals(bank, &bands, num, gain ? gain : ones, iv) ? 1 : 0;
-    if (ok) {
-        for (int k = 0; k <= kNC; k++) { if (owner) owner[k] = iv->owner[k]; if (r) r[k] = iv->r[k]; }
-        for (int j = 0; j <= num; j++) { if (ivStart) ivStart[j] = iv->start[j]; if (ivLen) ivLen[j] = iv->len[j]; }
-        if (tailW) for (int i = 0; i < kTailMax; i++) tailW[i] = iv->tailW[i];
-        int st[kMaxNum], gl[4];
-        plan_rows(iv->start, iv->len, num, st, gl);
-        if (groupLen) for (int g = 0; g < 4; g++) groupLen[g] = gl[g];
-        if (startShifted) for (int m = 0; m < kMaxNum; m++) startShifted[m] = st[m];
-    }
-    free(iv);
-    af_bands_free(&bands);
-    return ok;
 }

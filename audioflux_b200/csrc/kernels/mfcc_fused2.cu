@@ -36,27 +36,9 @@ namespace {
 constexpr int kN = 2048;
 constexpr int kBins = 1025;
 constexpr int kPairs = 513;         // bin pairs of the power-spectrum tile
-#ifndef AF2_FRAME_WARPS
-#define AF2_FRAME_WARPS 13
-#endif
-#ifndef AF2_BANK_WARPS
-#define AF2_BANK_WARPS 4
-#endif
-#ifndef AF2_DCT_WARPS
-#define AF2_DCT_WARPS 2
-#endif
-#ifndef AF2_ABLATE
-#define AF2_ABLATE 0                // diagnostic timing builds: 1 no bank, 2 no DCT, 4 no FFTs, 8 no transposes, 16 no loads
-#endif
-#ifndef AF2_WAIT
-#define AF2_WAIT 0                  // which mbarrier waits carry a suspend-time hint: 1 frame warps (power tile), 2 bank warps, 4 DCT warps, 8 frame warps (samples), 16 producer (tile protocol)
-#endif
-#ifndef AF2_WAIT_NS
-#define AF2_WAIT_NS 1000
-#endif
-constexpr int kFW = AF2_FRAME_WARPS;            // frame warps = max frames per tile (<= 16: one mma M tile)
-constexpr int kBW = AF2_BANK_WARPS;             // filter-bank warps (one interval per lane)
-constexpr int kDW = AF2_DCT_WARPS;              // DCT (tensor-core) + store warps, one tile behind the bank warps
+constexpr int kFW = 13;             // frame warps = max frames per tile (<= 16: one mma M tile)
+constexpr int kBW = 4;              // filter-bank warps (one interval per lane)
+constexpr int kDW = 2;              // DCT (tensor-core) + store warps, one tile behind the bank warps
 constexpr int kEW = kBW;                        // (planner: helper lanes that walk intervals)
 constexpr int kThreads = (kFW + 1 + kBW + kDW) * 32;  // + producer / special-column warp: 20 warps at <= 96 registers
 constexpr int kMaxPeers = 15;
@@ -120,26 +102,6 @@ __device__ __forceinline__ void bulk_store(void *dstGmem, const void *srcSmem, u
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// wait of one warp class: plain try_wait loop, or (AF2_WAIT bit set) try_wait with a suspend-time hint -- the warp sleeps in
-// hardware until the phase completes instead of polling through issue slots the compute warps need
-template <int BIT>
-__device__ __forceinline__ void wait_cls(uint64_t *bar, uint32_t parity) {
-    if (AF2_WAIT & BIT) {
-        uint32_t spins = 0, ok = 0;
-        while (true) {
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-                "selp.u32 %0, 1, 0, p;\n\t}"
-                : "=r"(ok) : "r"(af_smem_u32(bar)), "r"(parity), "r"((uint32_t)AF2_WAIT_NS) : "memory");
-            if (ok) break;
-            if (++spins > (1u << 24)) __trap();
-        }
-    } else {
-        af_mbar_wait(bar, parity);
-    }
-}
 
 __device__ __forceinline__ float rectify_value(float v, int rectify) {
     if (rectify == CepstralRectify_CubicRoot) return powf(v, 1.0f / 3.0f);
@@ -232,7 +194,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             const int f0 = (int)(tile % (unsigned)p.tilesPerClip) * F;
             const int nf = min(F, p.timeLength - f0);
             const int sb = it & 1;
-            wait_cls<16>(&specFull[sb], (uint32_t)(it >> 1) & 1u);
+            af_mbar_wait(&specFull[sb], (uint32_t)(it >> 1) & 1u);
             // a[n2] = R_n2[0], b[n2] = R_n2[32] (both real).  kind 0: X[64 k2] = DFT32(a)[k2], k2 = 0..16;
             // kind 1: X[32 + 64 k2] = DFT32(b[n2] W_64^n2)[k2], k2 = 0..15
             c64 u[32];
@@ -246,7 +208,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 if (n2 >= 16 && kind) u[n2] = c_mul_mi(u[n2]);                        // W_64^16 = -i
             }
             af_fft32_fma(u);
-            wait_cls<16>(pEmpty, ((uint32_t)it & 1u) ^ 1u);                   // bank done with the previous tile
+            af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);                   // bank done with the previous tile
             if (f < nf) {
                 float *dst = sP + 2 * f + (kind ? 32 * pitch : 0);                    // bin 64 k2 + 32 kind -> pair 32 k2 + 16 kind
 #pragma unroll
@@ -274,48 +236,46 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         int it = 0;
         for (unsigned tile = blockIdx.x; tile < p.totalTiles; tile += gridDim.x, ++it) {
             const int lbuf = it & 1;
-            wait_cls<2>(pFull, (uint32_t)it & 1u);
-            if (!p.rawMel) wait_cls<2>(&lEmpty[lbuf], ((uint32_t)(it >> 1) & 1u) ^ 1u);    // DCT done with tile it - 2
+            af_mbar_wait(pFull, (uint32_t)it & 1u);
+            if (!p.rawMel) af_mbar_wait(&lEmpty[lbuf], ((uint32_t)(it >> 1) & 1u) ^ 1u);    // DCT done with tile it - 2
             // ---- phase 1: ONE PIECE (<= Lmax bin pairs of one interval) PER LANE AND PASS, all frames of the tile in
             // registers: one LDS.128 of weights (rise of filter i, fall of filter i-1) and, per frame, one LDS.64 of the
             // power pair + two complex-pair FMAs -- kFW independent accumulator chains per lane.  Pass 0 walks the low rows of the
             // power tile, pass 1 the rest; once every helper warp is through a pass the rows it read are dead and take
             // the pieces' partial sums S[piece][frame] = (rise part, fall part), piece index = row index.
             c64 *sS = reinterpret_cast<c64 *>(sP);
-            if (!(AF2_ABLATE & 1)) {
-                for (int ps = 0; ps < p.nPass; ps++) {
-                    const unsigned piece = sAssign[(ps * kBW + e) * 32 + lane];
-                    const bool have = piece != 0xffffu;
-                    const unsigned d0 = sDesc[have ? piece : 0];
-                    const int len = have ? (int)((d0 >> 16) & 15u) : 0;
-                    const float4 *wt = sTab + (d0 & 0xffffu);
-                    const c64 *q = reinterpret_cast<const c64 *>(sP) + (size_t)(d0 >> 20) * pitch;
-                    c64 aR[kFW], aF[kFW];
+            for (int ps = 0; ps < p.nPass; ps++) {
+                const unsigned piece = sAssign[(ps * kBW + e) * 32 + lane];
+                const bool have = piece != 0xffffu;
+                const unsigned d0 = sDesc[have ? piece : 0];
+                const int len = have ? (int)((d0 >> 16) & 15u) : 0;
+                const float4 *wt = sTab + (d0 & 0xffffu);
+                const c64 *q = reinterpret_cast<const c64 *>(sP) + (size_t)(d0 >> 20) * pitch;
+                c64 aR[kFW], aF[kFW];
 #pragma unroll
-                    for (int f = 0; f < kFW; f++) { aR[f] = 0ull; aF[f] = 0ull; }
-                    const int maxLen = p.passLen[ps];
-                    for (int j = 0; j < maxLen; j++) {
-                        if (j < len) {
-                            const float4 w = wt[j];
-                            const c64 wr = c_pack(w.x, w.y), wf = c_pack(w.z, w.w);
-#pragma unroll
-                            for (int f = 0; f < kFW; f++) {
-                                const c64 v = q[f];
-                                aR[f] = v_fma(v, wr, aR[f]);
-                                aF[f] = v_fma(v, wf, aF[f]);
-                            }
-                            q += pitch;
-                        }
-                    }
-                    named_bar_sync(3, kBW * 32);                   // every helper warp has read this pass's rows
-                    if (have) {
+                for (int f = 0; f < kFW; f++) { aR[f] = 0ull; aF[f] = 0ull; }
+                const int maxLen = p.passLen[ps];
+                for (int j = 0; j < maxLen; j++) {
+                    if (j < len) {
+                        const float4 w = wt[j];
+                        const c64 wr = c_pack(w.x, w.y), wf = c_pack(w.z, w.w);
 #pragma unroll
                         for (int f = 0; f < kFW; f++) {
-                            float r0, r1, f0_, f1_;
-                            c_unpack(aR[f], r0, r1);
-                            c_unpack(aF[f], f0_, f1_);
-                            sS[(size_t)piece * pitch + f] = c_pack(r0 + r1, f0_ + f1_);
+                            const c64 v = q[f];
+                            aR[f] = v_fma(v, wr, aR[f]);
+                            aF[f] = v_fma(v, wf, aF[f]);
                         }
+                        q += pitch;
+                    }
+                }
+                named_bar_sync(3, kBW * 32);                   // every helper warp has read this pass's rows
+                if (have) {
+#pragma unroll
+                    for (int f = 0; f < kFW; f++) {
+                        float r0, r1, f0_, f1_;
+                        c_unpack(aR[f], r0, r1);
+                        c_unpack(aF[f], f0_, f1_);
+                        sS[(size_t)piece * pitch + f] = c_pack(r0 + r1, f0_ + f1_);
                     }
                 }
             }
@@ -330,39 +290,31 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             named_bar_sync(1, kBW * 32);                           // every partial sum of the tile is in shared memory
             // ---- phase 2: mel_m = sum of the rise parts of interval m + the fall parts of interval m + 1 (pieces in
             // ascending order), rectified (cepstra) or staged as the result row (filter bank) ----
-            // (kBW * 32 >= num: one band per helper lane; with fewer helper warps a lane takes kBands bands)
-            constexpr int kBands = (kMaxNum + kBW * 32 - 1) / (kBW * 32);
-            float v[kBands][kFW];
+            static_assert(kBW * 32 >= kMaxNum, "one band per helper lane");
+            const int m = e * 32 + lane;
+            float v[kFW];
 #pragma unroll
-            for (int b = 0; b < kBands; b++) {
-                const int m = (b * kBW + e) * 32 + lane;
+            for (int f = 0; f < kFW; f++) v[f] = 0.0f;
+            if (m < p.num) {
+                const int a0 = sPrefix[m], a1 = sPrefix[m + 1], a2 = sPrefix[m + 2];
+                for (int s = a0; s < a1; s++) {
+                    const c64 *row = sS + (size_t)s * pitch;
 #pragma unroll
-                for (int f = 0; f < kFW; f++) v[b][f] = 0.0f;
-                if (!(AF2_ABLATE & 1) && m < p.num) {
-                    const int a0 = sPrefix[m], a1 = sPrefix[m + 1], a2 = sPrefix[m + 2];
-                    for (int s = a0; s < a1; s++) {
-                        const c64 *row = sS + (size_t)s * pitch;
+                    for (int f = 0; f < kFW; f++) v[f] += c_re(row[f]);
+                }
+                for (int s = a1; s < a2; s++) {
+                    const c64 *row = sS + (size_t)s * pitch;
 #pragma unroll
-                        for (int f = 0; f < kFW; f++) v[b][f] += c_re(row[f]);
-                    }
-                    for (int s = a1; s < a2; s++) {
-                        const c64 *row = sS + (size_t)s * pitch;
-#pragma unroll
-                        for (int f = 0; f < kFW; f++) v[b][f] += c_im(row[f]);
-                    }
+                    for (int f = 0; f < kFW; f++) v[f] += c_im(row[f]);
                 }
             }
             __syncwarp();
             if (lane == 0) af_mbar_arrive(pEmpty);                 // frame warps may overwrite the power tile (and the sums in it)
+            if (m < p.num) {
 #pragma unroll
-            for (int b = 0; b < kBands; b++) {
-                const int m = (b * kBW + e) * 32 + lane;
-                if (!(AF2_ABLATE & 1) && m < p.num) {
-#pragma unroll
-                    for (int f = 0; f < kFW; f++) {
-                        if (p.rawMel) { if (f < nf) stage[f * stagePitch + m] = v[b][f]; }
-                        else L[f * kLPitch + m] = rectify_value(v[b][f], p.rectify);
-                    }
+                for (int f = 0; f < kFW; f++) {
+                    if (p.rawMel) { if (f < nf) stage[f * stagePitch + m] = v[f]; }
+                    else L[f * kLPitch + m] = rectify_value(v[f], p.rectify);
                 }
             }
             if (!p.rawMel) {
@@ -401,7 +353,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             const int nf = min(F, p.timeLength - f0);
             const int lbuf = it & 1;
             const float *L = sL + (size_t)lbuf * 16 * kLPitch;
-            wait_cls<4>(&lFull[lbuf], (uint32_t)(it >> 1) & 1u);
+            af_mbar_wait(&lFull[lbuf], (uint32_t)(it >> 1) & 1u);
             // out[16 x 8 CT] = L[16 x 128] . D^T[128 x 8 CT]: mma.sync m16n8k8 TF32, 3xTF32 split (hi by truncation,
             // lo = x - hi exact), separate accumulators for hi*hi and the cross terms
             float acc[kNB][4], acx[kNB][4];
@@ -415,7 +367,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         : "+f"(ACC[0]), "+f"(ACC[1]), "+f"(ACC[2]), "+f"(ACC[3])                                              \
         : "r"(A0), "r"(A1), "r"(A2), "r"(A3), "r"(B0), "r"(B1))
 #pragma unroll 2
-            for (int k0 = 0; k0 < ((AF2_ABLATE & 2) ? 8 : kMaxNum); k0 += 8) {
+            for (int k0 = 0; k0 < kMaxNum; k0 += 8) {
                 const float af[4] = {L[g * kLPitch + k0 + t], L[(g + 8) * kLPitch + k0 + t],
                                      L[g * kLPitch + k0 + t + 4], L[(g + 8) * kLPitch + k0 + t + 4]};
                 uint32_t ah[4], al[4];
@@ -508,7 +460,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         const bool active = warp < nf;
         const int sb = it & 1;
 
-        wait_cls<8>(&fullBar[stage], stagePhase);
+        af_mbar_wait(&fullBar[stage], stagePhase);
 
         c64 z[32];
         if (active) {
@@ -516,7 +468,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             const float *sp = span + (size_t)stage * p.spanFloats + warp * p.hop + lane;
 #pragma unroll
             for (int m = 0; m < 32; m++)
-                z[m] = (AF2_ABLATE & 16) ? c_pack(1.0f + m, lane) : v_mul(c_pack(sp[64 * m], sp[64 * m + 32]), sWinC[m * 32 + lane]);
+                z[m] = v_mul(c_pack(sp[64 * m], sp[64 * m + 32]), sWinC[m * 32 + lane]);
         }
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&emptyBar[stage]);           // span slot may be refilled
@@ -524,13 +476,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         if (!active) {
             // keep the tile protocols in step (one arrival per warp per tile and barrier)
             if (lane == 0) af_mbar_arrive(&specFull[sb]);
-            wait_cls<1>(pEmpty, ((uint32_t)it & 1u) ^ 1u);
+            af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);
             if (lane == 0) af_mbar_arrive(pFull);
             continue;
         }
 
         // ---- B: 64-point real DFT of the lane's column: packed complex 32-point DFT + in-lane post-pass ----
-        if (!(AF2_ABLATE & 4)) af_fft32_fma(z);                    // Z[k] at AF_BR5(k)
+        af_fft32_fma(z);                                           // Z[k] at AF_BR5(k)
         // R[k] = (Z[k] + conj Z[32-k]) - i W_64^k (Z[k] - conj Z[32-k]) at AF_BR5(k), (R[0], R[32]) in z[0]
         af_rfft64_post_fma(z);
         sSpec[((size_t)sb * 32 + lane) * kSpecPitch + warp] = z[0];
@@ -545,28 +497,22 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 const c64 y = c_mul_fma(z[AF_BR5(k1)], sTwC[(k1 - 1) * 32 + lane]);
                 c_unpack(y, yr[k1], yi[k1]);
             }
-            if (!(AF2_ABLATE & 8)) {
 #pragma unroll
-                for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yr[k1];
-                __syncwarp();
+            for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yr[k1];
+            __syncwarp();
 #pragma unroll
-                for (int n2 = 0; n2 < 32; n2++) yr[n2] = scratch[lane * 33 + n2];
-                __syncwarp();
+            for (int n2 = 0; n2 < 32; n2++) yr[n2] = scratch[lane * 33 + n2];
+            __syncwarp();
 #pragma unroll
-                for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yi[k1];
-                __syncwarp();
+            for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yi[k1];
+            __syncwarp();
 #pragma unroll
-                for (int n2 = 0; n2 < 32; n2++) z[n2] = c_pack(yr[n2], scratch[lane * 33 + n2]);
-                __syncwarp();
-            } else {
-                yr[0] = yi[0] = 0.0f;
-#pragma unroll
-                for (int n2 = 0; n2 < 32; n2++) z[n2] = c_pack(yr[n2], yi[n2]);
-            }
+            for (int n2 = 0; n2 < 32; n2++) z[n2] = c_pack(yr[n2], scratch[lane * 33 + n2]);
+            __syncwarp();
         }
         // ---- D: 32-point DFT over n2 in lane k1: bins k1 + 64 k2 and, mirrored, 64 (32 - k2) - k1 ----
-        if (!(AF2_ABLATE & 4)) af_fft32_fma(z);
-        wait_cls<1>(pEmpty, ((uint32_t)it & 1u) ^ 1u);      // bank done with the previous tile's spectra
+        af_fft32_fma(z);
+        af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);      // bank done with the previous tile's spectra
         if (lane) {
             if (p.dataType == SpectralData_Mag) {                  // (uniform branch: no sqrt sequence in the power path)
 #pragma unroll
@@ -827,8 +773,6 @@ static int launch_fused2(void *plan, const float *data, int dataLength, int batc
     const int rowFloats = rawMel ? pl->num : pl->ccNum;
     int bulk = rowFloats % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
     for (int d = 0; d < nPeer; d++) if (reinterpret_cast<uintptr_t>(peerOut[d]) & 15) bulk = 0;
-    const char *sv = getenv("AFB200_MFCC_STORE");
-    if (sv && !strcmp(sv, "plain")) bulk = 0;
     pp->bulkStore = bulk;
 
     // shared-memory carve-up: as many frames per tile as fit (<= kFW), two TMA stages when they fit, else one

@@ -75,8 +75,7 @@ int afb200_peerFree(void *devPtr);
 int afb200_ipcGetHandle(void *devPtr, void *handle64);
 int afb200_ipcOpenHandle(const void *handle64, void **devPtr);
 int afb200_ipcCloseHandle(void *devPtr);
-/* diagnostics: bank loop of the fused MFCC plan built by the last bftObj_mfccBatch call
- * (1 interval / shared-product form of a triangular bank, 0 filter-per-lane, -1 no fused plan) */
+/* diagnostics, after a bftObj_mfccBatch call: 0: the v1 fused kernel serves this object, -1: it does not */
 int bftObj_mfccPlanMode(BFTObj bftObj);
 int bftObj_getFilterBankArr(BFTObj bftObj, float *bank /* num x (fftLength/2+1) host */);
 /* in: rows x num; out: rows x ccNum */
@@ -117,10 +116,6 @@ int afb200_auditoryFilterBank(int num, int fftLength, int samplate, int scaleTyp
                               int normType, float lowFre, float highFre, int binPerOctave,
                               float *bank, float *freBandArr /* num */, int *binBandArr /* num */);
 int afb200_decimatorTaps(float *left32, float *right31);
-/* planner of the fused MFCC kernel's bank loop (host only): 1 when `bank` (num x 1025) has the triangular
- * two-overlap structure and the interval form applies; fills the per-bin interval owner / rising weight etc. */
-int afb200_mfccIntervalPlan(const float *bank, int num, const float *gain, int *owner, float *r, int *ivStart,
-                            int *ivLen, float *tailW, int *groupLen, int *startShifted);
 /* planner of the second-generation fused kernel (kernels/mfcc_fused2.cu, host only): every bin of `bank` (num x 1025)
  * is given to one interval i in [0, num] on which filter i "rises" and filter i-1 "falls" (the bank's own weights);
  * returns the number of float4 table entries (rise[2q], rise[2q+1], fall[2q], fall[2q+1]) or -1 when some bin is

@@ -233,28 +233,31 @@ def test_mfcc_fused_vs_oracle(torch_cuda, hop, cc, norm, dt, rect, L):
                                                          (S.MEL, ST.SLANEY, N.NONE, 40, 16000, D.POWER),
                                                          (S.ERB, ST.ETSI, N.BAND_WIDTH, 77, 22050, D.MAG)])
 def test_mfcc_fused_bank_loop_modes(torch_cuda, product_lib, monkeypatch, scale, style, norm, num, sr, dt):
-    """The fused kernel has two bank loops: the interval ("shared product") form for triangular banks and the
-    filter-per-lane loop for any banded bank.  Both against the oracle, and against each other."""
+    """The two fused kernels' bank loops: the default selection (v2's interval form for these banks) and the v1
+    filter-per-lane loop (AFB200_MFCC_KERNEL=v1, on a fresh object).  Both against the oracle, and against each other."""
     torch = torch_cuda
     x = np.stack([tones(31, 20480, sr), noise(32, 20480)])
     xd = torch.from_numpy(x).cuda()
     cc = min(20, num)
     outs = {}
-    for mode in ("1", "0"):
-        monkeypatch.setenv("AFB200_MFCC_BANK_MODE", mode)
+    for kernel in ("default", "v1"):
+        if kernel == "v1":
+            monkeypatch.setenv("AFB200_MFCC_KERNEL", "v1")
         b = af.BFT(num, 11, sr, slide_length=512, scale_type=scale, style_type=style, normal_type=norm, data_type=dt)
-        outs[mode] = b.mfcc_batch(xd, cc).cpu().numpy()
-        # every bank above has the structure; -1 = this shape is outside the fused kernel (composed path)
-        assert product_lib.bftObj_mfccPlanMode(b._obj) in (int(mode), -1)
+        outs[kernel] = b.mfcc_batch(xd, cc).cpu().numpy()
+    # -1 = this shape is outside the v1 kernel (composed path); the Slaney mel-128 banks must really run v1
+    assert product_lib.bftObj_mfccPlanMode(b._obj) in (0, -1)
+    if scale == S.MEL and style == ST.SLANEY and num == 128:
+        assert product_lib.bftObj_mfccPlanMode(b._obj) == 0
     lo, hi, _, _ = O.bft_revise_range(num, 2048, sr, None, None, af.enum_value(scale), 12)
     bank, _, _ = O.auditory_filterbank(num, 2048, sr, af.enum_value(scale), af.enum_value(style), af.enum_value(norm),
                                        float(lo), float(hi), 12)
     for i in range(2):
         mel = O.bft(x[i], num, 11, sr, 512, scale=af.enum_value(scale), data_type=af.enum_value(dt), bank=bank)
         want = O.xxcc(mel, cc)
-        assert rel_max(outs["1"][i], want) < TOL
-        assert rel_max(outs["0"][i], want) < TOL
-    assert rel_max(outs["1"], outs["0"]) < 2e-5
+        assert rel_max(outs["default"][i], want) < TOL
+        assert rel_max(outs["v1"][i], want) < TOL
+    assert rel_max(outs["default"], outs["v1"]) < 2e-5
 
 
 def test_mfcc_fused_non_triangular_bank_uses_filter_loop(torch_cuda, product_lib):

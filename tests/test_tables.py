@@ -174,80 +174,6 @@ def test_gammatone_banks_against_reference_build(product_lib, ref_lib, scale, lo
             np.testing.assert_allclose(b.get_fre_band_arr(), q.get_fre_band_arr(), rtol=1e-6)
 
 
-# ---- planner of the fused MFCC kernel's bank loop: interval ("shared product") form of triangular banks ----
-def _interval_plan(lib, bank, gain=None):
-    num = bank.shape[0]
-    owner = np.zeros(1025, np.int32)
-    r = np.zeros(1025, np.float32)
-    st = np.zeros(num + 1, np.int32)
-    ln = np.zeros(num + 1, np.int32)
-    tail = np.zeros(512, np.float32)
-    gl = np.zeros(4, np.int32)
-    ss = np.zeros(128, np.int32)
-    bank = np.ascontiguousarray(bank, np.float32)
-    g = None if gain is None else np.ascontiguousarray(gain, np.float32)
-    ok = lib.afb200_mfccIntervalPlan(bank.ctypes.data, num, None if g is None else g.ctypes.data, owner.ctypes.data,
-                                     r.ctypes.data, st.ctypes.data, ln.ctypes.data, tail.ctypes.data, gl.ctypes.data,
-                                     ss.ctypes.data)
-    return ok, owner, r, st, ln, tail, gl, ss
-
-
-def _interval_mel(bank, gain, P, plan):
-    """mel_m = g_m (A_m + S_{m+1} - A_{m+1}) exactly as the kernel evaluates it (float64 here)."""
-    _, owner, r, st, ln, tail, _, _ = plan
-    num = bank.shape[0]
-    g = np.ones(num) if gain is None else gain.astype(np.float64)
-    A = np.zeros(num + 1)
-    S = np.zeros(num + 1)
-    m = (owner >= 0) & (owner < num)
-    np.add.at(A, owner[m], r[m].astype(np.float64) * P[m])
-    np.add.at(S, owner[m], np.where(r[m] > 0, P[m], 0.0))
-    U = S - A
-    U[num] = sum(float(tail[i]) * P[st[num] + i] for i in range(ln[num]))
-    return g * (A[:num] + U[1:num + 1])
-
-
-@pytest.mark.parametrize("scale,style,norm,num,sr", [(2, 0, 0, 128, 48000), (2, 0, 1, 128, 48000), (2, 0, 2, 128, 48000),
-                                                      (3, 1, 1, 64, 48000), (4, 0, 0, 128, 48000), (3, 0, 0, 128, 32000),
-                                                      (2, 1, 0, 128, 48000), (2, 0, 0, 40, 16000), (2, 5, 0, 128, 48000),
-                                                      (3, 0, 1, 100, 44100), (4, 1, 2, 77, 22050)])
-def test_mfcc_interval_plan_reproduces_the_bank(product_lib, scale, style, norm, num, sr):
-    lo, hi, _, _ = O.bft_revise_range(num, 2048, sr, None, None, scale, 12)
-    bank, _, _ = O.auditory_filterbank(num, 2048, sr, scale, style, norm, float(lo), float(hi), 12)
-    gain = None
-    if norm:
-        unit, _, _ = O.auditory_filterbank(num, 2048, sr, scale, style, 0, float(lo), float(hi), 12)
-        pu = unit.max(1)
-        gain = np.where(pu > 0, bank.max(1) / np.where(pu > 0, pu, 1), 1).astype(np.float32)
-    plan = _interval_plan(product_lib, bank, gain)
-    assert plan[0] == 1
-    owner, r = plan[1], plan[2]
-    assert (np.diff(owner[owner >= 0]) >= 0).all()                 # intervals are runs of consecutive bins
-    assert ((r > 0) == (owner >= 0))[owner < num].all()            # every owned bin counts in S_j
-    B = bank.astype(np.float64)
-    rng = np.random.default_rng(0)
-    for _ in range(3):
-        P = rng.random(1025) ** 8 * 100
-        want = B @ P
-        assert np.abs(_interval_mel(bank, gain, P, plan) - want).max() <= 5e-7 * np.abs(want).max()
-    eye = np.eye(1025)
-    got = np.stack([_interval_mel(bank, gain, eye[k], plan) for k in range(1025)], axis=1)   # = the bank itself
-    assert np.abs(got - B).max() <= 3e-7 * max(np.abs(B).max(), 1e-30)
-
-
-def test_mfcc_interval_plan_rejects_other_banks(product_lib):
-    rect, _, _ = O.auditory_filterbank(128, 2048, 48000, 2, 4, 0, 0.0, 24000.0, 12)    # overlapping boxes sum to 2
-    assert _interval_plan(product_lib, rect)[0] == 0
-    rnd = np.random.default_rng(1).random((16, 1025)).astype(np.float32)               # dense
-    assert _interval_plan(product_lib, rnd)[0] == 0
-    tri, _, _ = O.auditory_filterbank(128, 2048, 48000, 2, 0, 0, 0.0, 24000.0, 12)
-    assert _interval_plan(product_lib, tri)[0] == 1
-    bad = tri.copy()
-    bad[40, np.nonzero(tri[40])[0][0]] *= 1.01                      # one weight off by 1 %: structure check must fail
-    assert _interval_plan(product_lib, bad)[0] == 0
-    assert _interval_plan(product_lib, tri, np.full(128, 2.0, np.float32))[0] == 0    # wrong gains
-
-
 # ---- planner of the second-generation fused kernel (kernels/mfcc_fused2.cu): per-tile interval form with the bank's own weights ----
 def _bank_plan2(lib, bank):
     num = bank.shape[0]

@@ -220,6 +220,23 @@ SPECTRAL_API = {
     "spectralObj_spectralBatch": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]),
 }
 
+# non-stationary Gabor transform (src/nsgt_algorithm.h:34-57, include/afb200_nsgt.h) and the additive batched entry point
+# (include/afb200_ext.h)
+NSGT_API = {
+    "nsgtObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, c_int_p, c_float_p, c_float_p, c_int_p, c_int_p,
+                              c_int_p, c_int_p, c_int_p, c_int_p]),
+    "nsgtObj_getMaxTimeLength": (C.c_int, [vp]),
+    "nsgtObj_getTotalTimeLength": (C.c_int, [vp]),
+    "nsgtObj_getTimeLengthArr": (vp, [vp]),
+    "nsgtObj_getFreBandArr": (vp, [vp]),
+    "nsgtObj_getBinBandArr": (vp, [vp]),
+    "nsgtObj_setMinLength": (None, [vp, C.c_int]),
+    "nsgtObj_nsgt": (None, [vp, vp, vp, vp]),
+    "nsgtObj_getCellData": (None, [vp, P(vp), P(vp)]),
+    "nsgtObj_free": (None, [vp]),
+    "nsgtObj_nsgtBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -227,10 +244,13 @@ REFERENCE_BUILDERS = {
     "auditory_filterBank": (None, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_float, C.c_float, C.c_int, vp, vp, vp]),
     "chroma_cqtFilterBank": (None, [C.c_int, C.c_int, C.c_int, c_float_p, vp]),
+    # src/filterbank/nsgt_filterBank.h (nsgt_filterBank.c:48-239)
+    "nsgt_filterBank": (None, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                               C.c_float, C.c_float, C.c_int, P(vp), vp, vp, vp, vp, c_int_p, c_int_p]),
 }
 
 
-def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, REFERENCE_BUILDERS)) -> dict:
+def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -65,6 +65,7 @@ int af_sm_count(void);
 /* ---------------- setup-time tables (host/af_window.c, af_filterbank.c, ...) ---------------- */
 int af_window_symmetric(int windowType, int length, const float *value, double *out);
 int af_window_fft(int windowType, int length, float *out);
+int af_window_create(int windowType, int length, int periodic, float *out);
 
 typedef struct {
     float low, high;      /* after the range rules of bftObj_new / cwtObj_new */
@@ -292,6 +293,37 @@ typedef struct {
     float par[4 * AFB200_SPECTRAL_MAX_REQ];
 } AfSpectralArgs;
 int af_launch_spectral(const AfSpectralArgs *a, void *stream);
+
+/* NSGT band transforms (kernels/nsgt.cu).  Bands with L <= AF_NSGT_BLUESTEIN_MAX run as Bluestein FFTs of size
+ * M = 2^ceil(log2(2L-1)) (k_nsgt_bluestein, one CTA per (group of bands, clip)); longer bands, up to AF_NSGT_MAX_LEN,
+ * as a direct DFT (k_nsgt_direct, one CTA per (band, clip)). */
+#define AF_NSGT_BLUESTEIN_MAX 4096
+#define AF_NSGT_MAX_LEN 16384
+#define AF_NSGT_GROUP_BUDGET 8192     /* sum of M over the bands of one Bluestein group */
+#define AF_NSGT_FINE 64               /* direct path: twiddle e^{2 pi i idx/L} = coarse[idx / 64] * fine[idx % 64] */
+typedef struct {
+    int L, log2M;
+    int off;        /* first spectrum bin of the window (clamped at 0) */
+    int winOff;     /* window offset in the concatenated windows */
+    int cellOff;    /* first cell of the band */
+    int tabOff;     /* float2 offset in `tab`: Bluestein chirp c_m = e^{i pi m^2/L} (L), direct: fine (64) then coarse */
+    int filtOff;    /* float2 offset in `filt`: FFT_M of the chirp filter, divided by L*M (Bluestein only) */
+    int band;
+} AfNsgtBand;
+typedef struct {
+    int fftLength, num, maxLen, totalLen, batch;
+    const float *specRe, *specIm;  /* device, batch x (fftLength/2+1) */
+    const float *win;              /* device, totalLen */
+    const int *map;                /* device, num x maxLen: cell index of every matrix column, -1 = none */
+    const AfNsgtBand *bands;       /* device, num: Bluestein bands group after group, then the direct bands */
+    const int *groupStart;         /* device, nGroups+1 offsets into `bands` */
+    const float *tab, *filt;       /* device, interleaved complex */
+    int nGroups, maxM;             /* Bluestein: groups, largest M */
+    int nDirect, maxDirectL;       /* direct: bands[groupStart[nGroups] ..] */
+    float *outRe, *outIm;          /* device, batch x num x maxLen */
+    float *cellRe, *cellIm;        /* device, batch x totalLen, or NULL */
+} AfNsgtArgs;
+int af_launch_nsgt(const AfNsgtArgs *a, void *stream);
 
 void af_count_launch(int n);
 

@@ -106,4 +106,22 @@ int af_window_fft(int type, int n, float *out) {
     return AF_OK;
 }
 
+/* window_createXxx(length, flag) of src/dsp/flux_window.c:64-78 and its siblings: flag 0 the symmetric window, flag 1
+ * ("periodic") the symmetric window of length+1 with the last sample dropped, for EVERY type (unlike af_window_fft,
+ * which keeps Bartlett / Triang / Bohman symmetric as window_calFFTWindow does); length 1 is {1}; Rect is ones. */
+int af_window_create(int type, int n, int periodic, float *out) {
+    if (n <= 0 || !out) return AF_ERR_ARG;
+    if (type <= Window_Rect || type > Window_Tukey || n == 1) {
+        for (int i = 0; i < n; i++) out[i] = 1.0f;
+        return AF_OK;
+    }
+    const int L = periodic ? n + 1 : n;
+    double *w = (double *)malloc(sizeof(double) * (size_t)L);
+    if (!w) return AF_ERR_NOMEM;
+    af_window_symmetric(type, L, NULL, w);
+    for (int i = 0; i < n; i++) out[i] = (float)w[i];
+    free(w);
+    return AF_OK;
+}
+
 int afb200_window(int windowType, int length, float *out) { return af_window_fft(windowType, length, out); }

@@ -55,6 +55,12 @@ class SpectralFilterBankNormalType(Enum):
     BAND_WIDTH = 2
 
 
+class NSGTFilterBankType(Enum):
+    """src/nsgt_algorithm.h:14-18"""
+    EFFICIENT = 0
+    STANDARD = 1
+
+
 class CepstralRectifyType(Enum):
     LOG = 0
     CUBIC_ROOT = 1

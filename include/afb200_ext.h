@@ -21,6 +21,7 @@
 #include "afb200_spectrogram.h"
 #include "afb200_pwt.h"
 #include "afb200_spectral.h"
+#include "afb200_nsgt.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -162,6 +163,12 @@ enum {
  * temporal features start afresh (frame 0 of clip b never looks at clip b-1). */
 int spectralObj_spectralBatch(SpectralObj spectralObj, const float *spec, const float *phase, int timeLength, int batch,
                               int nReq, const int *req, const float *par, float *out, int memKind, void *stream);
+
+/* NSGT of a batch: data batch x 2^radix2Exp -> matrix planes batch x num x maxTimeLength, and (when cellReal / cellImag
+ * are not NULL) the cells batch x totalTimeLength.  Columns the reference's time grids map to no cell are 0.
+ * Each clip's result is bit-identical to nsgtObj_nsgt on that clip, whatever the batch. */
+int nsgtObj_nsgtBatch(NSGTObj nsgtObj, const float *data, int batch, float *mReal, float *mImag,
+                      float *cellReal, float *cellImag, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

@@ -34,32 +34,51 @@ int af_devbuf_reserve(AfDevBuf *b, size_t bytes);
 void af_devbuf_free(AfDevBuf *b);
 int af_dev_upload(void **dptr, const void *host, size_t bytes);   /* cudaMalloc + H2D */
 void af_dev_free(void *dptr);
-int af_stream_create(void **stream);
-void af_stream_destroy(void *stream);
 int af_stream_sync(void *stream);
-int af_event_create(void **ev);
-void af_event_destroy(void *ev);
-int af_event_record(void *ev, void *stream);
-int af_stream_wait_event(void *stream, void *ev);
 int af_memcpy_h2d(void *dst, const void *src, size_t bytes, void *stream);
-int af_memcpy_d2h(void *dst, const void *src, size_t bytes, void *stream);
 int af_memset_d(void *dst, int v, size_t bytes, void *stream);
 size_t af_dev_free_bytes(void);
 
-/* Host-pointer batches: items flow through two device slots on three streams -- copy-in of chunk k+1, the transform
- * of chunk k and copy-out of chunk k-1 overlap (H2D and D2H are opposite PCIe directions).  With page-locked caller
- * buffers a call runs at the speed of the larger transfer and needs two chunks of device memory instead of the
- * batch; pageable buffers work too (the driver stages them synchronously). */
+/* Every batched entry point runs through af_run_batch, which holds the memKind rule:
+ * - AFB200_MEM_DEVICE: the chunk function runs once on the caller's pointers and stream, without synchronising.
+ * - AFB200_MEM_HOST: items flow through two device slots on three streams -- copy-in of chunk k+1, the transform of
+ *   chunk k and copy-out of chunk k-1 overlap (H2D and D2H are opposite PCIe directions) -- and the call returns
+ *   synchronised, with no copy into or out of caller memory still in flight, whether it succeeded or not.  With
+ *   page-locked caller buffers a call runs at the speed of the larger transfer and needs at most two chunks of device
+ *   memory instead of the batch; pageable buffers work too (the driver stages them synchronously).
+ * A chunk is about `chunkBytes` of the larger side (in + in-out planes, or out + in-out planes), a multiple of 16
+ * items when it holds at least 16, and at least one item.  Items must be independent of one another. */
+enum { AF_IN = 1, AF_OUT = 2, AF_INOUT = 3 };
+#define AF_PIPE_MAX_PLANES 6
+#define AF_PIPE_CHUNK_BYTES ((size_t)64 << 20)
+typedef struct {
+    const void *ptr;      /* caller's pointer (host or device, as memKind says); NULL: the plane is not used in this call */
+    size_t per;           /* floats per item */
+    int dir;              /* AF_IN, AF_OUT or AF_INOUT: in-out planes are copied in before the chunk and back after it */
+    int layers;           /* > 1: `layers` planes of batch x per floats one after the other (device chunk: layers x nb x per) */
+} AfPlane;
 typedef struct {
     int ready;
-    void *inStream, *outStream, *evIn[2], *evDone[2], *evOut[2];
-    AfDevBuf in[2], out0[2], out1[2];
+    void *stream, *inStream, *outStream, *evIn[2], *evDone[2], *evOut[2];
+    AfDevBuf slot[2][AF_PIPE_MAX_PLANES];
 } AfPipe;
-/* transform of `nb` items already on the device: dIn -> dOut0 (and dOut1 when the entry point has two planes) */
-typedef int (*AfChunkFn)(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *stream);
-int af_pipe_run(AfPipe *pipe, AfChunkFn fn, void *obj, const float *hIn, size_t inFloatsPerItem, int batch,
-                float *hOut0, float *hOut1, size_t outFloatsPerItem, void *computeStream);
+/* transform of `nb` items on the device: d[i] is plane i (NULL when it is not used), ctx the entry point's arguments */
+typedef int (*AfChunkFn)(void *ctx, int nb, float *const *d, void *stream);
+int af_run_batch(AfPipe *pipe, int memKind, void *stream, AfChunkFn fn, void *ctx, const AfPlane *planes, int nPlanes,
+                 int batch, size_t chunkBytes);
 void af_pipe_free(AfPipe *pipe);
+
+/* streaming bookkeeping shared by STFT, CQT and SpectrogramObj (stft_algorithm.c:474-599, cqt_algorithm.c:346-456):
+ * the samples that did not complete a hop are carried to the next call */
+typedef struct {
+    float *buf;           /* fftLength + slideLength floats */
+    int length;           /* may be negative when slideLength > fftLength: samples of the next call to skip */
+    float *cur; size_t curCap;   /* tail ++ new samples */
+} AfTail;
+/* 1: *cur / *curLength hold the carried samples followed by `data`; 0: not a whole frame yet (or out of memory) */
+int af_tail_assemble(AfTail *t, int fftLength, int slideLength, const float *data, int dataLength,
+                     const float **cur, int *curLength);
+void af_tail_free(AfTail *t);
 int af_sm_count(void);
 
 /* ---------------- setup-time tables (host/af_window.c, af_filterbank.c, ...) ---------------- */
@@ -119,6 +138,7 @@ void af_cwt_scales(int num, int dataLength, int samplate, float lowFre, float hi
                    int binPerOctave, float cf, float *freBandArr, int *binBandArr, float *scaleArr);
 
 void af_dct2_matrix(int num, int ccNum, float *out /* ccNum x num, ortho scaled */);
+int af_dct2_upload_transposed(float **dDctT, int n);   /* device [n][n]: the transpose of af_dct2_matrix(n, n) */
 void af_fft_twiddles(int n, float *cosArr, float *sinArr /* n/2 each: cos, -sin (2 pi i/n) */);
 
 /* ---------------- kernel launchers (kernels directory), all asynchronous on `stream` ---------------- */
@@ -247,12 +267,13 @@ typedef struct {
     float lowFre, highFre;
     int windowType, dataType, scaleType, styleType, normalType;
 } AfBftSpec;
-/* streaming bookkeeping of an STFT object (af_stft.c): tail of the earlier calls ++ data -> *cur / *curLength; 0 = no frame yet */
-int af_stft_continue_assemble(STFTObj s, const float *data, int dataLength, const float **cur, int *curLength);
 int af_filterbank_clipped(void);   /* non-zero weights the last af_auditory_filterbank call (this thread) dropped above the Nyquist bin */
 int af_bft_create(const AfBftSpec *spec, BFTObj *out);      /* 0, -1 (memory), -2 (unsupported bank) */
-int af_bft_phase(BFTObj b, const float *data, int dataLength, int batch, int lowIndex, int count, float *phase,
-                 int memKind, void *stream);
+int af_bft_device(BFTObj b);      /* lazy device set-up of the object's tables */
+/* device clips -> spect [batch x T x num] (real mode) and, when dPhase is given, the phase of the STFT bins
+ * lowIndex .. lowIndex+count-1 [batch x T x count] (spectrogramObj_spectrogramBatch) */
+int af_bft_spectrogram(BFTObj b, const float *dData, int dataLength, int batch, float *dSpect, int lowIndex, int count,
+                       float *dPhase, void *stream);
 int af_launch_phase(const float *re, const float *im, int rows, int width, int lo, int count, float *out, void *stream);
 
 /* synchrosqueezing (kernels/squeeze.cu): row index of the instantaneous frequency, row scatter */
@@ -276,6 +297,12 @@ int af_launch_reassign(const AfReassignArgs *a, const float *r1, const float *i1
 
 /* cepstral deconvolution of rows x num constant-Q magnitudes (kernels/deconv.cu): mode 0 cqhc, 1 deconv */
 int af_launch_cq_deconv(const float *in, int rows, int num, int mode, int hcNum, int bpo, float *out0, float *out1, void *stream);
+/* the same rows through af_run_batch (cqtObj_cqhcBatch / cqtObj_deconvBatch / spectrogramObj_deconvBatch, af_cqt.c) */
+int af_deconv_batch(AfPipe *pipe, const float *in, int rows, int num, int mode, int hcNum, int bpo, float *out0, float *out1,
+                    int memKind, void *stream);
+/* af_launch_xxcc through af_run_batch, rows as items (xxccObj_xxccBatch / cqtObj_cqccBatch, af_xxcc.c) */
+int af_xxcc_batch(AfPipe *pipe, const float *in, int rows, int num, int ccNum, int rectifyType, const float *dctT,
+                  float *out, int memKind, void *stream);
 
 /* energy / rms / zero-crossing rate of the windowed frames of ONE clip (src/temporal_algorithm.c:93-146); device arrays [T] */
 int af_launch_temporal(const float *data, int fftLength, int slideLength, int timeLength, const float *window,

@@ -26,28 +26,22 @@ struct OpaqueBFT {
     AfBands bands;
     /* device (lazy) */
     int devReady;
-    void *stream;
     float *dWindow, *dBank, *dPacked;
     int *dStart, *dLen, *dOff;
     AfBankDev bankDev;
-    AfDevBuf dIn, dSpecRe, dSpecIm, dOutRe, dOutIm;
+    AfDevBuf dSpecRe, dSpecIm, dMel;     /* spectrum planes; mel planes of the general MFCC path */
     /* fused MFCC plan cache */
     void *mfccPlan;
     int mfccPlanCc;
     void *melPlan;                       /* same fused kernel stopped after the bank (real-mode bftObj_bft at n = 2048) */
     void *mfccPlan2, *melPlan2;          /* second-generation fused kernel (kernels/mfcc_fused2.cu), preferred when the bank qualifies */
     int mfccPlan2Cc, v2State;            /* v2State: 0 unknown, 1 usable, -1 not (bank structure / AFB200_MFCC_KERNEL=v1) */
-    float *dDctT; int dctReady;          /* general path: transposed DCT [num][num] */
-    AfPipe pipe;                         /* host-pointer batches: chunked copy-in / transform / copy-out */
-    int pipeLength, pipeCc, pipeRectify; /* arguments of the call the pipe is currently serving */
+    float *dDctT;                        /* general path: transposed DCT [num][num] */
+    AfPipe pipe;
     int isTemporal;                      /* bft_algorithm.c:376, 532-534: energy / rms / zcr of the frames of the last bftObj_bft call */
     float *tempHost; int tempLength;     /* host: [energy | rms | zcr], tempLength frames each */
-    AfDevBuf dTemp;
     ReassignObj reassign;                /* isReassign = 1 (bft_algorithm.c:332-341): the bank is applied to the reassigned spectrum */
 };
-
-static int bft_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st);
-static int mfcc_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st);
 
 int bftObj_new(BFTObj *out, int num, int radix2Exp, int *samplate, float *lowFre, float *highFre,
                int *binPerOctave, WindowType *windowType, int *slideLength,
@@ -164,11 +158,10 @@ static int bft_v2_usable(BFTObj b, int ccNum) {
     return b->v2State > 0 && ccNum >= 1 && ccNum <= 64;
 }
 
-static int bft_device(BFTObj b) {
+int af_bft_device(BFTObj b) {
     int rc = af_device_ready();
     if (rc) return rc;
     if (b->devReady) return AF_OK;
-    if ((rc = af_stream_create(&b->stream))) return rc;
     const int width = b->fftLength / 2 + 1, num = b->num;
     if ((rc = af_dev_upload((void **)&b->dWindow, b->window, sizeof(float) * (size_t)b->fftLength))) return rc;
     /* banded representation when the support is sparse, dense matrix otherwise */
@@ -287,43 +280,49 @@ static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, 
     return AF_OK;
 }
 
+/* one argument block for every chunk function of this file */
+typedef struct { BFTObj b; int dataLength, ccNum, rectifyType; } BftCall;
+
+static int bft_chunk(void *p, int nb, float *const *d, void *st) {
+    const BftCall *a = (const BftCall *)p;
+    return bft_compute(a->b, d[0], a->dataLength, nb, d[1], d[2], st);
+}
+
 int bftObj_bftBatch(BFTObj b, const float *data, int dataLength, int batch, float *mReal3, float *mImag3,
                     int memKind, void *stream) {
     if (!b || !data || !mReal3 || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "bftObj_bftBatch: bad argument");
     af_clear_error();
-    int rc = bft_device(b);
+    int rc = af_bft_device(b);
     if (rc) return rc;
     const int T = bftObj_calTimeLength(b, dataLength);
     if (T <= 0) return AF_OK;
-    void *st = stream ? stream : b->stream;
-    const int needIm = !b->resultType && mImag3;
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;                      /* NULL = the CUDA default stream */
-        if ((rc = bft_compute(b, data, dataLength, batch, mReal3, needIm ? mImag3 : NULL, st))) return rc;
-        return AF_OK;                       /* asynchronous on the caller's stream */
-    }
-    b->pipeLength = dataLength;
-    return af_pipe_run(&b->pipe, bft_chunk, b, data, (size_t)dataLength, batch, mReal3, needIm ? mImag3 : NULL,
-                       (size_t)T * b->num, st);
+    BftCall a = {b, dataLength, 0, 0};
+    const size_t outPer = (size_t)T * b->num;
+    const AfPlane pl[3] = {{data, (size_t)dataLength, AF_IN, 0}, {mReal3, outPer, AF_OUT, 0},
+                           {!b->resultType ? mImag3 : NULL, outPer, AF_OUT, 0}};
+    return af_run_batch(&b->pipe, memKind, stream, bft_chunk, &a, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
 }
 
-/* temporal descriptors of the clip's frames (isTemporal): one more small kernel on the object's stream */
+static int temporal_chunk(void *p, int nb, float *const *d, void *st) {
+    const BftCall *a = (const BftCall *)p;
+    const int T = bftObj_calTimeLength(a->b, a->dataLength);
+    (void)nb;                                         /* one clip */
+    return af_launch_temporal(d[0], a->b->fftLength, a->b->slideLength, T, a->b->dWindow, d[1], d[1] + T, d[1] + 2 * (size_t)T, st);
+}
+
+/* temporal descriptors of the clip's frames (isTemporal): one more small kernel */
 static int bft_temporal(BFTObj b, const float *dataArr, int dataLength) {
     const int T = bftObj_calTimeLength(b, dataLength);
     if (T <= 0) return AF_OK;
-    int rc;
     if (T != b->tempLength) {
         free(b->tempHost);
         b->tempHost = (float *)calloc((size_t)3 * T, sizeof(float));
         if (!b->tempHost) { b->tempLength = 0; return AF_ERR_NOMEM; }
         b->tempLength = T;
     }
-    if ((rc = af_devbuf_reserve(&b->dIn, sizeof(float) * (size_t)dataLength)) || (rc = af_devbuf_reserve(&b->dTemp, sizeof(float) * 3 * (size_t)T))) return rc;
-    float *d = (float *)b->dTemp.ptr;
-    if ((rc = af_memcpy_h2d(b->dIn.ptr, dataArr, sizeof(float) * (size_t)dataLength, b->stream))) return rc;
-    if ((rc = af_launch_temporal((const float *)b->dIn.ptr, b->fftLength, b->slideLength, T, b->dWindow, d, d + T, d + 2 * (size_t)T, b->stream))) return rc;
-    if ((rc = af_memcpy_d2h(b->tempHost, d, sizeof(float) * 3 * (size_t)T, b->stream))) return rc;
-    return af_stream_sync(b->stream);
+    BftCall a = {b, dataLength, 0, 0};
+    const AfPlane pl[2] = {{dataArr, (size_t)dataLength, AF_IN, 0}, {b->tempHost, 3 * (size_t)T, AF_OUT, 0}};
+    return af_run_batch(&b->pipe, AFB200_MEM_HOST, NULL, temporal_chunk, &a, pl, 2, 1, AF_PIPE_CHUNK_BYTES);
 }
 
 void bftObj_bft(BFTObj b, float *dataArr, int dataLength, float *mRealArr3, float *mImageArr3) {
@@ -332,24 +331,14 @@ void bftObj_bft(BFTObj b, float *dataArr, int dataLength, float *mRealArr3, floa
     if (b->isTemporal) bft_temporal(b, dataArr, dataLength);
 }
 
-/* phase of the STFT bins lowIndex..highIndex as spectrogramObj_spectrogram reports it for the Linear scale
- * (src/spectrogram_algorithm.c:1040-1056): atan2f(im, re < 1e-16 ? 1e-16 : re).  phase: batch x T x count. */
-int af_bft_phase(BFTObj b, const float *data, int dataLength, int batch, int lowIndex, int count, float *phase,
-                 int memKind, void *stream) {
-    if (!b || !data || !phase || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "spectrogram phase: bad argument");
-    int rc = bft_device(b);
-    if (rc) return rc;
+/* real-mode bank of the clips, then -- with dPhase -- the phase of the STFT bins lowIndex..lowIndex+count-1 as
+ * spectrogramObj_spectrogram reports it for the Linear scale (src/spectrogram_algorithm.c:1040-1056):
+ * atan2f(im, re < 1e-16 ? 1e-16 : re).  phase: batch x T x count. */
+int af_bft_spectrogram(BFTObj b, const float *dData, int dataLength, int batch, float *dSpect, int lowIndex, int count,
+                       float *dPhase, void *st) {
+    int rc = bft_compute(b, dData, dataLength, batch, dSpect, NULL, st);
+    if (rc || !dPhase) return rc;
     const int T = bftObj_calTimeLength(b, dataLength), width = b->fftLength / 2 + 1;
-    if (T <= 0) return AF_OK;
-    void *st = memKind == AFB200_MEM_DEVICE ? stream : (stream ? stream : b->stream);
-    const float *dData = data;
-    float *dPhase = phase;
-    const size_t inB = sizeof(float) * (size_t)batch * dataLength, outB = sizeof(float) * (size_t)batch * T * count;
-    if (memKind != AFB200_MEM_DEVICE) {
-        if ((rc = af_devbuf_reserve(&b->dIn, inB)) || (rc = af_devbuf_reserve(&b->dOutRe, outB))) return rc;
-        if ((rc = af_memcpy_h2d(b->dIn.ptr, data, inB, st))) return rc;
-        dData = (const float *)b->dIn.ptr; dPhase = (float *)b->dOutRe.ptr;
-    }
     const size_t perClip = sizeof(float) * (size_t)T * width;
     size_t budget = af_dev_free_bytes() / 4;
     if (budget < perClip) budget = perClip;
@@ -369,9 +358,7 @@ int af_bft_phase(BFTObj b, const float *data, int dataLength, int batch, int low
         if ((rc = af_launch_phase((const float *)b->dSpecRe.ptr, (const float *)b->dSpecIm.ptr, nb * T, width, lowIndex, count,
                                   dPhase + (size_t)c0 * T * count, st))) return rc;
     }
-    if (memKind == AFB200_MEM_DEVICE) return AF_OK;
-    if ((rc = af_memcpy_d2h(phase, b->dOutRe.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    return AF_OK;
 }
 
 /* ---- fused / composed MFCC: bft(real mode) -> rectify -> ortho DCT-II -> first ccNum ---- */
@@ -410,35 +397,19 @@ static int mfcc_compute(BFTObj b, const float *dData, int dataLength, int batch,
     }
     if (nPeer > 0) return af_fail(AF_ERR_UNSUPPORTED, "bftObj_mfccBatchScatter: only the fused fftLength=2048 path can store to peers");
     /* general composition (any fftLength / bank / alignment), still entirely on the device */
-    if (!b->dctReady) {
-        const int n = b->num;
-        float *d = (float *)malloc(sizeof(float) * (size_t)n * n), *t = (float *)malloc(sizeof(float) * (size_t)n * n);
-        if (!d || !t) { free(d); free(t); return AF_ERR_NOMEM; }
-        af_dct2_matrix(n, n, d);
-        for (int k = 0; k < n; k++) for (int j = 0; j < n; j++) t[(size_t)j * n + k] = d[(size_t)k * n + j];
-        rc = af_dev_upload((void **)&b->dDctT, t, sizeof(float) * (size_t)n * n);
-        free(d); free(t);
-        if (rc) return rc;
-        b->dctReady = 1;
-    }
+    if (!b->dDctT && (rc = af_dct2_upload_transposed(&b->dDctT, b->num))) return rc;
     const int savedType = b->resultType;
     b->resultType = 1;
-    const size_t melB = sizeof(float) * (size_t)batch * T * b->num;
-    rc = af_devbuf_reserve(&b->dOutIm, melB);          /* reuse as mel scratch */
-    if (!rc) rc = bft_compute(b, dData, dataLength, batch, (float *)b->dOutIm.ptr, NULL, st);
+    rc = af_devbuf_reserve(&b->dMel, sizeof(float) * (size_t)batch * T * b->num);
+    if (!rc) rc = bft_compute(b, dData, dataLength, batch, (float *)b->dMel.ptr, NULL, st);
     b->resultType = savedType;
     if (rc) return rc;
-    return af_launch_xxcc((const float *)b->dOutIm.ptr, batch * T, b->num, ccNum, rectifyType, b->dDctT, dOut, st);
+    return af_launch_xxcc((const float *)b->dMel.ptr, batch * T, b->num, ccNum, rectifyType, b->dDctT, dOut, st);
 }
 
-static int mfcc_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st) {
-    BFTObj b = (BFTObj)obj;
-    (void)dOut1;
-    return mfcc_compute(b, dIn, b->pipeLength, nb, b->pipeCc, b->pipeRectify, dOut0, 0, NULL, st);
-}
-static int bft_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st) {
-    BFTObj b = (BFTObj)obj;
-    return bft_compute(b, dIn, b->pipeLength, nb, dOut0, dOut1, st);
+static int mfcc_chunk(void *p, int nb, float *const *d, void *st) {
+    const BftCall *a = (const BftCall *)p;
+    return mfcc_compute(a->b, d[0], a->dataLength, nb, a->ccNum, a->rectifyType, d[1], 0, NULL, st);
 }
 
 int bftObj_mfccBatch(BFTObj b, const float *data, int dataLength, int batch, int ccNum, int rectifyType,
@@ -446,18 +417,13 @@ int bftObj_mfccBatch(BFTObj b, const float *data, int dataLength, int batch, int
     if (!b || !data || !out || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "bftObj_mfccBatch: bad argument");
     if (ccNum < 1 || ccNum > b->num) return af_fail(AF_ERR_ARG, "bftObj_mfccBatch: ccNum=%d outside [1, %d]", ccNum, b->num);
     af_clear_error();
-    int rc = bft_device(b);
+    int rc = af_bft_device(b);
     if (rc) return rc;
     const int T = bftObj_calTimeLength(b, dataLength);
     if (T <= 0) return AF_OK;
-    void *st = stream ? stream : b->stream;
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;                      /* NULL = the CUDA default stream */
-        if ((rc = mfcc_compute(b, data, dataLength, batch, ccNum, rectifyType, out, 0, NULL, st))) return rc;
-        return AF_OK;                       /* asynchronous on the caller's stream */
-    }
-    b->pipeLength = dataLength; b->pipeCc = ccNum; b->pipeRectify = rectifyType;
-    return af_pipe_run(&b->pipe, mfcc_chunk, b, data, (size_t)dataLength, batch, out, NULL, (size_t)T * ccNum, st);
+    BftCall a = {b, dataLength, ccNum, rectifyType};
+    const AfPlane pl[2] = {{data, (size_t)dataLength, AF_IN, 0}, {out, (size_t)T * ccNum, AF_OUT, 0}};
+    return af_run_batch(&b->pipe, memKind, stream, mfcc_chunk, &a, pl, 2, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 /* MFCC + all-gather in one kernel: device pointers only.  `out` is this GPU's destination, peerOut[0..nPeer) are
@@ -469,7 +435,7 @@ int bftObj_mfccBatchScatter(BFTObj b, const float *data, int dataLength, int bat
         return af_fail(AF_ERR_ARG, "bftObj_mfccBatchScatter: bad argument");
     if (ccNum < 1 || ccNum > b->num) return af_fail(AF_ERR_ARG, "bftObj_mfccBatchScatter: ccNum=%d outside [1, %d]", ccNum, b->num);
     af_clear_error();
-    int rc = bft_device(b);
+    int rc = af_bft_device(b);
     if (rc) return rc;
     if (bftObj_calTimeLength(b, dataLength) <= 0) return AF_OK;
     return mfcc_compute(b, data, dataLength, batch, ccNum, rectifyType, out, nPeer, (float *const *)peerOut, stream);
@@ -480,12 +446,10 @@ void bftObj_free(BFTObj b) {
     af_mfcc_plan_free(b->mfccPlan); af_mfcc_plan_free(b->melPlan);
     af_mfcc2_plan_free(b->mfccPlan2); af_mfcc2_plan_free(b->melPlan2);
     reassignObj_free(b->reassign);
-    free(b->tempHost); af_devbuf_free(&b->dTemp);
-    af_devbuf_free(&b->dIn); af_devbuf_free(&b->dSpecRe); af_devbuf_free(&b->dSpecIm);
-    af_devbuf_free(&b->dOutRe); af_devbuf_free(&b->dOutIm);
+    free(b->tempHost);
+    af_devbuf_free(&b->dSpecRe); af_devbuf_free(&b->dSpecIm); af_devbuf_free(&b->dMel);
     af_dev_free(b->dWindow); af_dev_free(b->dBank); af_dev_free(b->dPacked);
     af_dev_free(b->dStart); af_dev_free(b->dLen); af_dev_free(b->dOff); af_dev_free(b->dDctT);
-    af_stream_destroy(b->stream);
     af_pipe_free(&b->pipe);
     af_bands_free(&b->bands);
     free(b->window); free(b->bank); free(b->freBandArr); free(b->binBandArr);

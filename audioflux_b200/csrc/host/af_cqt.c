@@ -15,23 +15,19 @@ struct OpaqueCQT {
     float left32[32], right31[32];
     /* device (lazy) */
     int devReady;
-    void *stream;
     float *dBfrag;                               /* tensor-core octave kernel: pre-split kernel fragments */
     unsigned char *dBimg;                        /* wgmma octave kernel: pre-swizzled shared-memory images of the kernels */
     float *dKappa2, *dLeft, *dRight, *dScale;    /* dScale: octaveNum x bpo, rebuilt when isScale flips */
     int scaleDirty;
-    AfDevBuf dIn, dSigA, dSigB, dOutRe, dOutIm;
+    AfDevBuf dSigA, dSigB;                       /* decimated signal, octave after octave */
     /* post-processing of the last transform (chroma / cqcc) */
     int timeLength;                /* frames of the last cqtObj_cqt call (cqt_algorithm.c:463-478) */
     int chromaNum;
     float *dChromaBank, *dDctT;
-    AfDevBuf dPostA, dPostB, dPostOut;
-    AfPipe pipe;                   /* host-pointer batches: chunked copy-in / transform / copy-out */
-    int pipeLength;
+    AfPipe pipe;
     /* streaming (isContinue, cqt_algorithm.c:346-456): full-rate samples that did not complete a hop wait for the next call */
     int isContinue;
-    float *tail; int tailLength;   /* host; tailLength < 0: samples of the next call to skip (slide > fftLength) */
-    float *cur; size_t curCap;
+    AfTail tail;
 };
 
 int cqtObj_newWith(CQTObj *out, int num, int *samplate, float *minFre, int *binPerOctave, float *factor,
@@ -87,7 +83,7 @@ static int cqt_time_length(const struct OpaqueCQT *c, int dataLength, int isCont
 }
 int cqtObj_calTimeLength(CQTObj c, int dataLength) {
     if (!c) return 0;
-    if (c->isContinue) return dataLength + c->tailLength <= 0 ? 0 : cqt_time_length(c, dataLength + c->tailLength, 1);
+    if (c->isContinue) return dataLength + c->tail.length <= 0 ? 0 : cqt_time_length(c, dataLength + c->tail.length, 1);
     return cqt_time_length(c, dataLength, 0);
 }
 int cqtObj_getFFTLength(CQTObj c) { return c ? c->fftLength : 0; }
@@ -105,7 +101,6 @@ static int cqt_device(CQTObj c) {
     int rc = af_device_ready();
     if (rc) return rc;
     if (!c->devReady) {
-        if ((rc = af_stream_create(&c->stream))) return rc;
         /* kernel sets: one (the top octave's, shared) or -- VQT -- one per octave, set o at offset o * bpo rows */
         const int sets = c->bank.vqt ? c->octaveNum : 1;
         const size_t setFloats = 2 * (size_t)c->binPerOctave * c->fftLength;
@@ -198,67 +193,29 @@ static int cqt_compute_ex(CQTObj c, const float *dData, int dataLength, int batc
     return AF_OK;
 }
 
+typedef struct { CQTObj c; int dataLength, T, padLeft; } CqtCall;
+
+static int cqt_chunk(void *p, int nb, float *const *d, void *st) {
+    const CqtCall *a = (const CqtCall *)p;
+    return cqt_compute_ex(a->c, d[0], a->dataLength, nb, a->T, a->padLeft, d[1], d[2], st);
+}
+
+static int cqt_run(CQTObj c, const float *data, int dataLength, int batch, int T, int padLeft, float *re, float *im,
+                   int memKind, void *stream) {
+    CqtCall a = {c, dataLength, T, padLeft};
+    const size_t outPer = (size_t)T * c->num;
+    const AfPlane pl[3] = {{data, (size_t)dataLength, AF_IN, 0}, {re, outPer, AF_OUT, 0}, {im, outPer, AF_OUT, 0}};
+    return af_run_batch(&c->pipe, memKind, stream, cqt_chunk, &a, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
+}
+
 /* batched / device entry points are stateless: centre padding, every clip on its own */
-static int cqt_compute(CQTObj c, const float *dData, int dataLength, int batch, float *dRe, float *dIm, void *st) {
-    return cqt_compute_ex(c, dData, dataLength, batch, cqt_time_length(c, dataLength, 0), c->fftLength / 2, dRe, dIm, st);
-}
-
-static int cqt_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st) {
-    CQTObj c = (CQTObj)obj;
-    return cqt_compute(c, dIn, c->pipeLength, nb, dOut0, dOut1, st);
-}
-
 int cqtObj_cqtBatch(CQTObj c, const float *data, int dataLength, int batch, float *mReal3, float *mImag3,
                     int memKind, void *stream) {
     if (!c || !data || !mReal3 || !mImag3 || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "cqtObj_cqtBatch: bad argument");
     af_clear_error();
     int rc = cqt_device(c);
     if (rc) return rc;
-    const int T = cqt_time_length(c, dataLength, 0);
-    void *st = stream ? stream : c->stream;
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;
-        return cqt_compute(c, data, dataLength, batch, mReal3, mImag3, st);
-    }
-    c->pipeLength = dataLength;
-    return af_pipe_run(&c->pipe, cqt_chunk, c, data, (size_t)dataLength, batch, mReal3, mImag3, (size_t)T * c->num, st);
-}
-
-/* streaming bookkeeping of _cqtObj_dealData (cqt_algorithm.c:346-456): 1 = *cur / *curLength hold tail + new samples */
-static int cqt_continue_assemble(CQTObj c, const float *data, int dataLength, const float **cur, int *curLength) {
-    const int n = c->fftLength, hop = c->slideLength;
-    if (!c->tail) {
-        c->tail = (float *)calloc((size_t)n + (size_t)hop + 1, sizeof(float));
-        if (!c->tail) return 0;
-    }
-    const int total = c->tailLength + dataLength;
-    if (total < n) {
-        if (c->tailLength >= 0) memcpy(c->tail + c->tailLength, data, sizeof(float) * (size_t)dataLength);
-        else if (dataLength + c->tailLength > 0) memcpy(c->tail, data - c->tailLength, sizeof(float) * (size_t)(dataLength + c->tailLength));
-        c->tailLength = total;
-        c->timeLength = 0;
-        return 0;
-    }
-    const int tailLen = (total - n) % hop + (n - hop);
-    if ((size_t)total + (size_t)n > c->curCap) {
-        free(c->cur);
-        c->curCap = (size_t)total + (size_t)n;
-        c->cur = (float *)malloc(sizeof(float) * c->curCap);
-        if (!c->cur) { c->curCap = 0; return 0; }
-    }
-    int len;
-    if (c->tailLength < 0) {
-        len = dataLength + c->tailLength;
-        memcpy(c->cur, data - c->tailLength, sizeof(float) * (size_t)len);
-    } else {
-        if (c->tailLength > 0) memcpy(c->cur, c->tail, sizeof(float) * (size_t)c->tailLength);
-        memcpy(c->cur + c->tailLength, data, sizeof(float) * (size_t)dataLength);
-        len = c->tailLength + dataLength;
-    }
-    if (tailLen > 0) memcpy(c->tail, c->cur + (len - tailLen), sizeof(float) * (size_t)tailLen);
-    c->tailLength = tailLen;
-    *cur = c->cur; *curLength = len;
-    return 1;
+    return cqt_run(c, data, dataLength, batch, cqt_time_length(c, dataLength, 0), c->fftLength / 2, mReal3, mImag3, memKind, stream);
 }
 
 void cqtObj_cqt(CQTObj c, float *dataArr, int dataLength, float *mRealArr3, float *mImageArr3) {
@@ -272,22 +229,22 @@ void cqtObj_cqt(CQTObj c, float *dataArr, int dataLength, float *mRealArr3, floa
     const float *x = NULL;
     int len = 0;
     if (!mRealArr3 || !mImageArr3) return;
-    if (!cqt_continue_assemble(c, dataArr, dataLength, &x, &len)) return;
+    if (!af_tail_assemble(&c->tail, c->fftLength, c->slideLength, dataArr, dataLength, &x, &len)) { c->timeLength = 0; return; }
     af_clear_error();
     if (cqt_device(c)) return;
-    const int T = cqt_time_length(c, len, 1);
-    c->timeLength = T;
-    if (T <= 0) return;
-    const size_t inB = sizeof(float) * (size_t)len, outB = sizeof(float) * (size_t)T * c->num;
-    void *st = c->stream;
-    if (af_devbuf_reserve(&c->dIn, inB) || af_devbuf_reserve(&c->dOutRe, outB) || af_devbuf_reserve(&c->dOutIm, outB)) return;
-    if (af_memcpy_h2d(c->dIn.ptr, x, inB, st)) return;
-    if (cqt_compute_ex(c, (const float *)c->dIn.ptr, len, 1, T, 0, (float *)c->dOutRe.ptr, (float *)c->dOutIm.ptr, st)) return;
-    if (af_memcpy_d2h(mRealArr3, c->dOutRe.ptr, outB, st) || af_memcpy_d2h(mImageArr3, c->dOutIm.ptr, outB, st)) return;
-    af_stream_sync(st);
+    c->timeLength = cqt_time_length(c, len, 1);
+    if (c->timeLength <= 0) return;
+    cqt_run(c, x, len, 1, c->timeLength, 0, mRealArr3, mImageArr3, AFB200_MEM_HOST, NULL);
 }
 
 /* ---- chroma: rows x num CQT planes -> rows x chromaNum (cqt_algorithm.c:484-600) ---- */
+typedef struct { CQTObj c; int chromaNum, isMag, normType; } ChromaCall;
+
+static int chroma_chunk(void *p, int nb, float *const *d, void *st) {
+    const ChromaCall *a = (const ChromaCall *)p;
+    return af_launch_chroma(d[0], d[1], nb, a->c->num, a->chromaNum, a->isMag, a->normType, a->c->dChromaBank, d[2], st);
+}
+
 int cqtObj_chromaBatch(CQTObj c, const float *mReal, const float *mImag, int rows, int chromaNum, int dataType,
                        int normType, float *out, int memKind, void *stream) {
     if (!c || !mReal || !mImag || !out || rows < 0) return af_fail(AF_ERR_ARG, "cqtObj_chromaBatch: bad argument");
@@ -307,17 +264,9 @@ int cqtObj_chromaBatch(CQTObj c, const float *mReal, const float *mImag, int row
         if (rc) return rc;
         c->chromaNum = chromaNum;
     }
-    const int isMag = dataType == SpectralData_Mag;
-    if (memKind == AFB200_MEM_DEVICE)
-        return af_launch_chroma(mReal, mImag, rows, c->num, chromaNum, isMag, normType, c->dChromaBank, out, stream);
-    void *st = stream ? stream : c->stream;
-    const size_t inB = sizeof(float) * (size_t)rows * c->num, outB = sizeof(float) * (size_t)rows * chromaNum;
-    if ((rc = af_devbuf_reserve(&c->dPostA, inB)) || (rc = af_devbuf_reserve(&c->dPostB, inB)) || (rc = af_devbuf_reserve(&c->dPostOut, outB))) return rc;
-    if ((rc = af_memcpy_h2d(c->dPostA.ptr, mReal, inB, st)) || (rc = af_memcpy_h2d(c->dPostB.ptr, mImag, inB, st))) return rc;
-    if ((rc = af_launch_chroma((const float *)c->dPostA.ptr, (const float *)c->dPostB.ptr, rows, c->num, chromaNum, isMag,
-                               normType, c->dChromaBank, (float *)c->dPostOut.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(out, c->dPostOut.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    ChromaCall a = {c, chromaNum, dataType == SpectralData_Mag, normType};
+    const AfPlane pl[3] = {{mReal, (size_t)c->num, AF_IN, 0}, {mImag, (size_t)c->num, AF_IN, 0}, {out, (size_t)chromaNum, AF_OUT, 0}};
+    return af_run_batch(&c->pipe, memKind, stream, chroma_chunk, &a, pl, 3, rows, AF_PIPE_CHUNK_BYTES);
 }
 
 void cqtObj_chroma(CQTObj c, int *chromaNum, SpectralDataType *dataType, ChromaDataNormalType *normType,
@@ -340,24 +289,8 @@ int cqtObj_cqccBatch(CQTObj c, const float *in, int rows, int ccNum, int rectify
     af_clear_error();
     int rc = cqt_device(c);
     if (rc) return rc;
-    if (!c->dDctT) {
-        const int n = c->num;
-        float *d = (float *)malloc(sizeof(float) * (size_t)n * n), *t = (float *)malloc(sizeof(float) * (size_t)n * n);
-        if (!d || !t) { free(d); free(t); return AF_ERR_NOMEM; }
-        af_dct2_matrix(n, n, d);
-        for (int k = 0; k < n; k++) for (int j = 0; j < n; j++) t[(size_t)j * n + k] = d[(size_t)k * n + j];
-        rc = af_dev_upload((void **)&c->dDctT, t, sizeof(float) * (size_t)n * n);
-        free(d); free(t);
-        if (rc) return rc;
-    }
-    if (memKind == AFB200_MEM_DEVICE) return af_launch_xxcc(in, rows, c->num, ccNum, rectifyType, c->dDctT, out, stream);
-    void *st = stream ? stream : c->stream;
-    const size_t inB = sizeof(float) * (size_t)rows * c->num, outB = sizeof(float) * (size_t)rows * ccNum;
-    if ((rc = af_devbuf_reserve(&c->dPostA, inB)) || (rc = af_devbuf_reserve(&c->dPostOut, outB))) return rc;
-    if ((rc = af_memcpy_h2d(c->dPostA.ptr, in, inB, st))) return rc;
-    if ((rc = af_launch_xxcc((const float *)c->dPostA.ptr, rows, c->num, ccNum, rectifyType, c->dDctT, (float *)c->dPostOut.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(out, c->dPostOut.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    if (!c->dDctT && (rc = af_dct2_upload_transposed(&c->dDctT, c->num))) return rc;
+    return af_xxcc_batch(&c->pipe, in, rows, c->num, ccNum, rectifyType, c->dDctT, out, memKind, stream);
 }
 
 void cqtObj_cqcc(CQTObj c, float *mDataArr1, int ccNum, CepstralRectifyType *rectifyType, float *mDataArr2) {
@@ -369,22 +302,27 @@ void cqtObj_cqcc(CQTObj c, float *mDataArr1, int ccNum, CepstralRectifyType *rec
 
 /* ---- cqhc / deconv: rows x num magnitudes (or powers) -> harmonic-index picks of the timbre sequence / timbre + pitch
  * (cqt_algorithm.c:662-781).  mode 0: out0 [rows x hcNum]; mode 1: out0 = timbre, out1 = pitch [rows x num] ---- */
+typedef struct { int num, mode, hcNum, bpo; } DeconvCall;
+
+static int deconv_chunk(void *p, int nb, float *const *d, void *st) {
+    const DeconvCall *a = (const DeconvCall *)p;
+    return af_launch_cq_deconv(d[0], nb, a->num, a->mode, a->hcNum, a->bpo, d[1], d[2], st);
+}
+
+int af_deconv_batch(AfPipe *pipe, const float *in, int rows, int num, int mode, int hcNum, int bpo, float *out0, float *out1,
+                    int memKind, void *stream) {
+    if (rows <= 0) return AF_OK;
+    DeconvCall a = {num, mode, hcNum, bpo};
+    const size_t outPer = (size_t)(mode ? num : hcNum);
+    const AfPlane pl[3] = {{in, (size_t)num, AF_IN, 0}, {out0, outPer, AF_OUT, 0}, {mode ? out1 : NULL, outPer, AF_OUT, 0}};
+    return af_run_batch(pipe, memKind, stream, deconv_chunk, &a, pl, 3, rows, AF_PIPE_CHUNK_BYTES);
+}
+
 static int cqt_deconv_batch(CQTObj c, const float *in, int rows, int mode, int hcNum, float *out0, float *out1, int memKind, void *stream) {
     af_clear_error();
     int rc = cqt_device(c);
     if (rc) return rc;
-    if (rows <= 0) return AF_OK;
-    if (memKind == AFB200_MEM_DEVICE) return af_launch_cq_deconv(in, rows, c->num, mode, hcNum, c->binPerOctave, out0, out1, stream);
-    void *st = stream ? stream : c->stream;
-    const size_t inB = sizeof(float) * (size_t)rows * c->num, outB = sizeof(float) * (size_t)rows * (mode ? c->num : hcNum);
-    if ((rc = af_devbuf_reserve(&c->dPostA, inB)) || (rc = af_devbuf_reserve(&c->dPostOut, outB)) ||
-        (mode && (rc = af_devbuf_reserve(&c->dPostB, outB)))) return rc;
-    if ((rc = af_memcpy_h2d(c->dPostA.ptr, in, inB, st))) return rc;
-    if ((rc = af_launch_cq_deconv((const float *)c->dPostA.ptr, rows, c->num, mode, hcNum, c->binPerOctave, (float *)c->dPostOut.ptr,
-                                  mode ? (float *)c->dPostB.ptr : NULL, st))) return rc;
-    if ((rc = af_memcpy_d2h(out0, c->dPostOut.ptr, outB, st))) return rc;
-    if (mode && (rc = af_memcpy_d2h(out1, c->dPostB.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    return af_deconv_batch(&c->pipe, in, rows, c->num, mode, hcNum, c->binPerOctave, out0, out1, memKind, stream);
 }
 
 int cqtObj_cqhcBatch(CQTObj c, const float *in, int rows, int hcNum, float *out, int memKind, void *stream) {
@@ -407,15 +345,13 @@ void cqtObj_deconv(CQTObj c, float *mDataArr1, float *mDataArr2, float *mDataArr
 
 void cqtObj_free(CQTObj c) {
     if (!c) return;
-    af_devbuf_free(&c->dIn); af_devbuf_free(&c->dSigA); af_devbuf_free(&c->dSigB);
-    af_devbuf_free(&c->dOutRe); af_devbuf_free(&c->dOutIm);
-    af_devbuf_free(&c->dPostA); af_devbuf_free(&c->dPostB); af_devbuf_free(&c->dPostOut);
+    af_devbuf_free(&c->dSigA); af_devbuf_free(&c->dSigB);
     af_pipe_free(&c->pipe);
     af_dev_free(c->dChromaBank); af_dev_free(c->dDctT);
     af_dev_free(c->dBfrag); af_dev_free(c->dBimg);
     af_dev_free(c->dKappa2); af_dev_free(c->dLeft); af_dev_free(c->dRight); af_dev_free(c->dScale);
-    af_stream_destroy(c->stream);
     af_cqt_bank_free(&c->bank);
-    free(c->kappa2); free(c->tail); free(c->cur);
+    free(c->kappa2);
+    af_tail_free(&c->tail);
     free(c);
 }

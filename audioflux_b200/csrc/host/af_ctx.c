@@ -92,7 +92,7 @@ int af_dev_upload(void **dptr, const void *host, size_t bytes) {
 
 void af_dev_free(void *p) { if (p) cudaFree(p); }
 
-int af_stream_create(void **s) {
+static int af_stream_create(void **s) {
     if (*s) return AF_OK;                                  /* already created by an earlier, partially failed initialisation */
     cudaStream_t st;
     int e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
@@ -100,13 +100,10 @@ int af_stream_create(void **s) {
     *s = (void *)st;
     return AF_OK;
 }
-void af_stream_destroy(void *s) { if (s) cudaStreamDestroy((cudaStream_t)s); }
+static void af_stream_destroy(void *s) { if (s) cudaStreamDestroy((cudaStream_t)s); }
 int af_stream_sync(void *s) { return af_cuda_check(cudaStreamSynchronize((cudaStream_t)s), "cudaStreamSynchronize"); }
 int af_memcpy_h2d(void *d, const void *h, size_t n, void *s) {
     return af_cuda_check(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, (cudaStream_t)s), "cudaMemcpyAsync H2D");
-}
-int af_memcpy_d2h(void *h, const void *d, size_t n, void *s) {
-    return af_cuda_check(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, (cudaStream_t)s), "cudaMemcpyAsync D2H");
 }
 int af_memset_d(void *d, int v, size_t n, void *s) {
     return af_cuda_check(cudaMemsetAsync(d, v, n, (cudaStream_t)s), "cudaMemsetAsync");
@@ -124,61 +121,100 @@ int af_sm_count(void) {
 }
 
 /* ---- events: ordering between the copy / compute / read-back streams of the host-pointer pipelines ---- */
-int af_event_create(void **ev) {
+static int af_event_create(void **ev) {
     cudaEvent_t e;
     int rc = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     if (rc != cudaSuccess) { *ev = NULL; return af_cuda_check(rc, "cudaEventCreate"); }
     *ev = (void *)e;
     return AF_OK;
 }
-void af_event_destroy(void *ev) { if (ev) cudaEventDestroy((cudaEvent_t)ev); }
-int af_event_record(void *ev, void *stream) { return af_cuda_check(cudaEventRecord((cudaEvent_t)ev, (cudaStream_t)stream), "cudaEventRecord"); }
-int af_stream_wait_event(void *stream, void *ev) { return af_cuda_check(cudaStreamWaitEvent((cudaStream_t)stream, (cudaEvent_t)ev, 0), "cudaStreamWaitEvent"); }
+static void af_event_destroy(void *ev) { if (ev) cudaEventDestroy((cudaEvent_t)ev); }
+static int af_event_record(void *ev, void *stream) { return af_cuda_check(cudaEventRecord((cudaEvent_t)ev, (cudaStream_t)stream), "cudaEventRecord"); }
+static int af_stream_wait_event(void *stream, void *ev) { return af_cuda_check(cudaStreamWaitEvent((cudaStream_t)stream, (cudaEvent_t)ev, 0), "cudaStreamWaitEvent"); }
 
-int af_pipe_run(AfPipe *pp, AfChunkFn fn, void *obj, const float *hIn, size_t inPer, int batch,
-                float *hOut0, float *hOut1, size_t outPer, void *st) {
+static size_t plane_floats(const AfPlane *p) { return p->per * (size_t)(p->layers > 1 ? p->layers : 1); }
+
+/* items c0 .. c0+nb-1 of a plane between caller memory and a slot (device layout layers x nb x per) */
+static int plane_copy(const AfPlane *p, float *dev, int c0, int nb, int batch, int toDevice, void *st) {
+    const size_t w = sizeof(float) * p->per * nb, hostPitch = sizeof(float) * p->per * batch;
+    char *host = (char *)p->ptr + sizeof(float) * p->per * c0;
+    int e;
+    if (p->layers > 1)
+        e = toDevice ? cudaMemcpy2DAsync(dev, w, host, hostPitch, w, p->layers, cudaMemcpyHostToDevice, (cudaStream_t)st)
+                     : cudaMemcpy2DAsync(host, hostPitch, dev, w, w, p->layers, cudaMemcpyDeviceToHost, (cudaStream_t)st);
+    else
+        e = toDevice ? cudaMemcpyAsync(dev, host, w, cudaMemcpyHostToDevice, (cudaStream_t)st)
+                     : cudaMemcpyAsync(host, dev, w, cudaMemcpyDeviceToHost, (cudaStream_t)st);
+    return af_cuda_check(e, toDevice ? "cudaMemcpyAsync H2D" : "cudaMemcpyAsync D2H");
+}
+
+static int pipe_chunks(AfPipe *pp, AfChunkFn fn, void *ctx, const AfPlane *pl, int np, int batch, int chunk, void *st) {
+    int rc, inout = 0;
+    for (int i = 0; i < np; i++) inout |= pl[i].ptr && pl[i].dir == AF_INOUT;
+    for (int s = 0; s < (chunk < batch ? 2 : 1); s++)              /* the second slot only when a second chunk exists */
+        for (int i = 0; i < np; i++)
+            if (pl[i].ptr && (rc = af_devbuf_reserve(&pp->slot[s][i], sizeof(float) * plane_floats(&pl[i]) * chunk))) return rc;
+    int k = 0;
+    for (int c0 = 0; c0 < batch; c0 += chunk, k++) {
+        const int nb = batch - c0 < chunk ? batch - c0 : chunk, s = k & 1;
+        float *d[AF_PIPE_MAX_PLANES];
+        for (int i = 0; i < np; i++) d[i] = pl[i].ptr ? (float *)pp->slot[s][i].ptr : NULL;
+        if (k >= 2) {                                   /* slot reuse: its previous transform and read-back are over */
+            if ((rc = af_stream_wait_event(pp->inStream, pp->evDone[s])) || (rc = af_stream_wait_event(st, pp->evOut[s]))) return rc;
+            if (inout && (rc = af_stream_wait_event(pp->inStream, pp->evOut[s]))) return rc;
+        }
+        for (int i = 0; i < np; i++)
+            if (pl[i].ptr && (pl[i].dir & AF_IN) && (rc = plane_copy(&pl[i], d[i], c0, nb, batch, 1, pp->inStream))) return rc;
+        if ((rc = af_event_record(pp->evIn[s], pp->inStream)) || (rc = af_stream_wait_event(st, pp->evIn[s]))) return rc;
+        if ((rc = fn(ctx, nb, d, st))) return rc;
+        if ((rc = af_event_record(pp->evDone[s], st)) || (rc = af_stream_wait_event(pp->outStream, pp->evDone[s]))) return rc;
+        for (int i = 0; i < np; i++)
+            if (pl[i].ptr && (pl[i].dir & AF_OUT) && (rc = plane_copy(&pl[i], d[i], c0, nb, batch, 0, pp->outStream))) return rc;
+        if ((rc = af_event_record(pp->evOut[s], pp->outStream))) return rc;
+    }
+    return AF_OK;
+}
+
+int af_run_batch(AfPipe *pp, int memKind, void *stream, AfChunkFn fn, void *ctx, const AfPlane *pl, int np, int batch,
+                 size_t chunkBytes) {
+    if (np > AF_PIPE_MAX_PLANES) return af_fail(AF_ERR_ARG, "af_run_batch: %d planes", np);
+    if (memKind == AFB200_MEM_DEVICE) {                /* asynchronous on the caller's stream (NULL = the default stream) */
+        float *d[AF_PIPE_MAX_PLANES];
+        for (int i = 0; i < np; i++) d[i] = (float *)pl[i].ptr;
+        return fn(ctx, batch, d, stream);
+    }
     int rc;
     if (!pp->ready) {
-        if ((rc = af_stream_create(&pp->inStream)) || (rc = af_stream_create(&pp->outStream))) return rc;
+        if ((rc = af_stream_create(&pp->stream)) || (rc = af_stream_create(&pp->inStream)) || (rc = af_stream_create(&pp->outStream))) return rc;
         for (int s = 0; s < 2; s++)
             if ((rc = af_event_create(&pp->evIn[s])) || (rc = af_event_create(&pp->evDone[s])) || (rc = af_event_create(&pp->evOut[s]))) return rc;
         pp->ready = 1;
     }
-    /* chunk: about 64 MB of the larger side, a multiple of 16 items when possible, at least 1 */
-    const size_t big = inPer > outPer * (hOut1 ? 2 : 1) ? inPer : outPer * (hOut1 ? 2 : 1);
-    long long per = ((long long)64 << 20) / (long long)(big * sizeof(float) > 0 ? big * sizeof(float) : 1);
+    size_t inB = 0, outB = 0;
+    for (int i = 0; i < np; i++) {
+        if (!pl[i].ptr) continue;
+        if (pl[i].dir & AF_IN) inB += sizeof(float) * plane_floats(&pl[i]);
+        if (pl[i].dir & AF_OUT) outB += sizeof(float) * plane_floats(&pl[i]);
+    }
+    const size_t big = inB > outB ? inB : outB;
+    long long per = (long long)(chunkBytes / (big > 0 ? big : 1));
     if (per >= 16) per -= per % 16;
     if (per < 1) per = 1;
     if (per > batch) per = batch;
-    const int chunk = (int)per;
-    for (int s = 0; s < 2; s++) {
-        if ((rc = af_devbuf_reserve(&pp->in[s], sizeof(float) * inPer * chunk)) ||
-            (rc = af_devbuf_reserve(&pp->out0[s], sizeof(float) * outPer * chunk))) return rc;
-        if (hOut1 && (rc = af_devbuf_reserve(&pp->out1[s], sizeof(float) * outPer * chunk))) return rc;
-    }
-    int k = 0;
-    for (int c0 = 0; c0 < batch; c0 += chunk, k++) {
-        const int nb = batch - c0 < chunk ? batch - c0 : chunk, s = k & 1;
-        if (k >= 2) {                                   /* slot reuse: its previous transform and read-back are over */
-            if ((rc = af_stream_wait_event(pp->inStream, pp->evDone[s])) || (rc = af_stream_wait_event(st, pp->evOut[s]))) return rc;
-        }
-        if ((rc = af_memcpy_h2d(pp->in[s].ptr, hIn + (size_t)c0 * inPer, sizeof(float) * inPer * nb, pp->inStream))) return rc;
-        if ((rc = af_event_record(pp->evIn[s], pp->inStream)) || (rc = af_stream_wait_event(st, pp->evIn[s]))) return rc;
-        if ((rc = fn(obj, (const float *)pp->in[s].ptr, nb, (float *)pp->out0[s].ptr, hOut1 ? (float *)pp->out1[s].ptr : NULL, st))) return rc;
-        if ((rc = af_event_record(pp->evDone[s], st)) || (rc = af_stream_wait_event(pp->outStream, pp->evDone[s]))) return rc;
-        if ((rc = af_memcpy_d2h(hOut0 + (size_t)c0 * outPer, pp->out0[s].ptr, sizeof(float) * outPer * nb, pp->outStream))) return rc;
-        if (hOut1 && (rc = af_memcpy_d2h(hOut1 + (size_t)c0 * outPer, pp->out1[s].ptr, sizeof(float) * outPer * nb, pp->outStream))) return rc;
-        if ((rc = af_event_record(pp->evOut[s], pp->outStream))) return rc;
-    }
-    if ((rc = af_stream_sync(pp->inStream)) || (rc = af_stream_sync(st))) return rc;
-    return af_stream_sync(pp->outStream);
+    void *st = stream ? stream : pp->stream;
+    rc = batch > 0 ? pipe_chunks(pp, fn, ctx, pl, np, batch, (int)per, st) : AF_OK;
+    /* wait for all three streams whatever happened: no copy touches caller memory after the call returns */
+    const int e1 = cudaStreamSynchronize((cudaStream_t)pp->inStream), e2 = cudaStreamSynchronize((cudaStream_t)st),
+              e3 = cudaStreamSynchronize((cudaStream_t)pp->outStream);
+    if (rc) return rc;
+    return af_cuda_check(e1 ? e1 : e2 ? e2 : e3, "cudaStreamSynchronize");
 }
 
 void af_pipe_free(AfPipe *pp) {
-    af_stream_destroy(pp->inStream); af_stream_destroy(pp->outStream);
+    af_stream_destroy(pp->stream); af_stream_destroy(pp->inStream); af_stream_destroy(pp->outStream);
     for (int s = 0; s < 2; s++) {
         af_event_destroy(pp->evIn[s]); af_event_destroy(pp->evDone[s]); af_event_destroy(pp->evOut[s]);
-        af_devbuf_free(&pp->in[s]); af_devbuf_free(&pp->out0[s]); af_devbuf_free(&pp->out1[s]);
+        for (int i = 0; i < AF_PIPE_MAX_PLANES; i++) af_devbuf_free(&pp->slot[s][i]);
     }
     memset(pp, 0, sizeof(*pp));
 }

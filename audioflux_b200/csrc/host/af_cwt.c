@@ -17,15 +17,15 @@ struct OpaqueCWT {
     int *binBandArr;
     /* device (lazy) */
     int devReady;
-    void *stream;
     float *dScale;
-    AfDevBuf dIn, dWork, dOutRe, dOutIm;
+    AfDevBuf dWork;
     float *bankHost, *dBank;       /* PWT: auditory bank num x (fftLength/2+1) instead of a wavelet family */
     int bankWidth;
     int detEnabled;                /* cwtObj_enableDet */
     int haveSpec;                  /* dWork starts with the spectrum of the last single-clip call */
     AfDevBuf dSupport;             /* fast path: per bank row the bins above 2^-28 of its peak (filled by the launcher) */
     int supportReady;
+    AfPipe pipe;
 };
 
 int cwtObj_new(CWTObj *out, int num, int radix2Exp, int *samplate, float *lowFre, float *highFre,
@@ -87,7 +87,6 @@ static int cwt_device(CWTObj c) {
     int rc = af_device_ready();
     if (rc) return rc;
     if (c->devReady) return AF_OK;
-    if ((rc = af_stream_create(&c->stream))) return rc;
     if ((rc = af_dev_upload((void **)&c->dScale, c->scaleArr, sizeof(float) * (size_t)c->num))) return rc;
     if (c->bankHost && (rc = af_dev_upload((void **)&c->dBank, c->bankHost, sizeof(float) * (size_t)c->num * c->bankWidth))) return rc;
     if ((rc = af_devbuf_reserve(&c->dSupport, sizeof(int) * 3 * (size_t)c->num))) return rc;
@@ -133,46 +132,30 @@ static int cwt_compute(CWTObj c, const float *dData, int batch, int det, float *
     return AF_OK;
 }
 
+typedef struct { CWTObj c; int det; } CwtCall;
+
+static int cwt_chunk(void *p, int nb, float *const *d, void *st) {
+    const CwtCall *a = (const CwtCall *)p;
+    return cwt_compute(a->c, d[0], nb, a->det, d[1], d[2], st);
+}
+
 static int cwt_batch(CWTObj c, const float *data, int batch, int det, float *mReal4, float *mImag4, int memKind,
                      void *stream, const char *who) {
     if (!c || !mReal4 || !mImag4 || batch <= 0) return af_fail(AF_ERR_ARG, "%s: bad argument", who);
     af_clear_error();
     int rc = cwt_device(c);
     if (rc) return rc;
-    void *st = stream ? stream : c->stream;
-    if (!data) {                        /* cwtObj_cwtDet(obj, NULL, ...): the spectrum of the last single-clip call */
-        if (batch != 1 || !c->haveSpec) return af_fail(AF_ERR_ARG, "%s: no data and no spectrum of a previous single-clip call", who);
-        if (memKind == AFB200_MEM_DEVICE) return cwt_compute(c, NULL, 1, det, mReal4, mImag4, stream);
-        const size_t outB = sizeof(float) * (size_t)c->num * c->dataLength;
-        if ((rc = af_devbuf_reserve(&c->dOutRe, outB)) || (rc = af_devbuf_reserve(&c->dOutIm, outB))) return rc;
-        if ((rc = cwt_compute(c, NULL, 1, det, (float *)c->dOutRe.ptr, (float *)c->dOutIm.ptr, st))) return rc;
-        if ((rc = af_memcpy_d2h(mReal4, c->dOutRe.ptr, outB, st)) || (rc = af_memcpy_d2h(mImag4, c->dOutIm.ptr, outB, st))) return rc;
-        return af_stream_sync(st);
-    }
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;
-        return cwt_compute(c, data, batch, det, mReal4, mImag4, st);
-    }
-    /* host pointers: chunks of clips whose planes fit a bounded staging buffer (<= 512 MB per plane, at least one clip):
-     * one copy in, one launch sequence over chunk x num items, two copies out per chunk.  Long transforms (2^19 points:
-     * 176 MB per plane and clip) go two clips at a time, the short windows of CWT.ccwt (2^12 points) hundreds at a time
-     * instead of one latency-bound round trip per window. */
-    const size_t inB = sizeof(float) * (size_t)c->dataLength, outB = sizeof(float) * (size_t)c->num * c->dataLength;
-    size_t chunk = ((size_t)512 << 20) / outB;
-    if (chunk < 1) chunk = 1;
-    if (chunk > (size_t)batch) chunk = (size_t)batch;
-    if ((rc = af_devbuf_reserve(&c->dIn, chunk * inB)) || (rc = af_devbuf_reserve(&c->dOutRe, chunk * outB)) ||
-        (rc = af_devbuf_reserve(&c->dOutIm, chunk * outB))) return rc;
-    for (int b = 0; b < batch; b += (int)chunk) {
-        const size_t nb = (size_t)(batch - b) < chunk ? (size_t)(batch - b) : chunk;
-        if ((rc = af_memcpy_h2d(c->dIn.ptr, data + (size_t)b * c->dataLength, nb * inB, st))) return rc;
-        if ((rc = cwt_compute(c, (const float *)c->dIn.ptr, (int)nb, det, (float *)c->dOutRe.ptr, (float *)c->dOutIm.ptr, st))) return rc;
-        if ((rc = af_memcpy_d2h(mReal4 + (size_t)b * c->num * c->dataLength, c->dOutRe.ptr, nb * outB, st)) ||
-            (rc = af_memcpy_d2h(mImag4 + (size_t)b * c->num * c->dataLength, c->dOutIm.ptr, nb * outB, st))) return rc;
-        if ((rc = af_stream_sync(st))) return rc;
-    }
+    /* cwtObj_cwtDet(obj, NULL, ...): no input plane, the spectrum of the last single-clip call */
+    if (!data && (batch != 1 || !c->haveSpec)) return af_fail(AF_ERR_ARG, "%s: no data and no spectrum of a previous single-clip call", who);
+    CwtCall a = {c, det};
+    const size_t outPer = (size_t)c->num * c->dataLength;
+    const AfPlane pl[3] = {{data, (size_t)c->dataLength, AF_IN, 0}, {mReal4, outPer, AF_OUT, 0}, {mImag4, outPer, AF_OUT, 0}};
+    /* host pointers: at most 512 MB per output plane in a chunk.  Long transforms (2^19 points: 176 MB per plane and
+     * clip) go two clips at a time, the short windows of CWT.ccwt (2^12 points) hundreds at a time instead of one
+     * latency-bound round trip per window. */
+    rc = af_run_batch(&c->pipe, memKind, stream, cwt_chunk, &a, pl, 3, batch, (size_t)1024 << 20);
     if (batch > 1) c->haveSpec = 0;      /* cwtObj_cwtDet(NULL) continues a SINGLE-clip call only */
-    return AF_OK;
+    return rc;
 }
 
 int cwtObj_cwtBatch(CWTObj c, const float *data, int batch, float *mReal4, float *mImag4, int memKind, void *stream) {
@@ -214,11 +197,11 @@ int cwtObj_getFilterBankArr(CWTObj c, float *bank) {
 
 void cwtObj_free(CWTObj c) {
     if (!c) return;
-    af_devbuf_free(&c->dIn); af_devbuf_free(&c->dWork); af_devbuf_free(&c->dOutRe); af_devbuf_free(&c->dOutIm);
+    af_devbuf_free(&c->dWork);
     af_dev_free(c->dScale); af_dev_free(c->dBank);
     af_devbuf_free(&c->dSupport);
+    af_pipe_free(&c->pipe);
     free(c->bankHost);
-    af_stream_destroy(c->stream);
     free(c->freBandArr); free(c->binBandArr); free(c->scaleArr);
     free(c);
 }
@@ -314,10 +297,10 @@ int pwtObj_getFilterBankArr(PWTObj p, float *bank) { return p ? cwtObj_getFilter
 void pwtObj_free(PWTObj p) {
     if (!p) return;
     CWTObj c = &p->c;
-    af_devbuf_free(&c->dIn); af_devbuf_free(&c->dWork); af_devbuf_free(&c->dOutRe); af_devbuf_free(&c->dOutIm);
+    af_devbuf_free(&c->dWork);
     af_dev_free(c->dScale); af_dev_free(c->dBank);
     af_devbuf_free(&c->dSupport);
-    af_stream_destroy(c->stream);
+    af_pipe_free(&c->pipe);
     free(c->bankHost); free(c->freBandArr); free(c->binBandArr); free(c->scaleArr);
     free(p);
 }

@@ -352,6 +352,16 @@ void af_dct2_matrix(int num, int ccNum, float *out) {
     }
 }
 
+int af_dct2_upload_transposed(float **dDctT, int n) {
+    float *d = (float *)malloc(sizeof(float) * (size_t)n * n), *t = (float *)malloc(sizeof(float) * (size_t)n * n);
+    if (!d || !t) { free(d); free(t); return AF_ERR_NOMEM; }
+    af_dct2_matrix(n, n, d);
+    for (int k = 0; k < n; k++) for (int j = 0; j < n; j++) t[(size_t)j * n + k] = d[(size_t)k * n + j];
+    int rc = af_dev_upload((void **)dDctT, t, sizeof(float) * (size_t)n * n);
+    free(d); free(t);
+    return rc;
+}
+
 void af_fft_twiddles(int n, float *c, float *s) {
     for (int i = 0; i < n / 2; i++) { c[i] = (float)cos(2.0 * M_PI * i / n); s[i] = (float)-sin(2.0 * M_PI * i / n); }
 }

@@ -28,9 +28,8 @@ struct OpaqueNSGT {
     float *cellRe, *cellIm;                        /* totalLen: cells of the last nsgtObj_nsgt call */
 
     int dirty;                                     /* tables changed since the last upload */
-    void *stream;
     void *dWin, *dMap, *dBands, *dGroup, *dTab, *dFilt;
-    AfDevBuf spec, in, out0, out1, cell0, cell1;
+    AfDevBuf spec;                                 /* half spectra of the clips */
     AfPipe pipe;
 };
 
@@ -398,7 +397,6 @@ static void nsgt_device_tables_free(NSGTObj s) {
 static int nsgt_device(NSGTObj s) {
     int rc = af_device_ready();
     if (rc) return rc;
-    if (!s->stream && (rc = af_stream_create(&s->stream))) return rc;
     if (!s->dirty) return AF_OK;
     nsgt_device_tables_free(s);
     if ((rc = af_dev_upload(&s->dWin, s->win, sizeof(float) * (size_t)s->totalLen)) ||
@@ -434,8 +432,8 @@ static int nsgt_run(NSGTObj s, const float *dIn, int nb, float *re, float *im, f
     return af_launch_nsgt(&a, st);
 }
 
-static int nsgt_chunk(void *obj, const float *dIn, int nb, float *dRe, float *dIm, void *st) {
-    return nsgt_run((NSGTObj)obj, dIn, nb, dRe, dIm, NULL, NULL, st);
+static int nsgt_chunk(void *p, int nb, float *const *d, void *st) {
+    return nsgt_run((NSGTObj)p, d[0], nb, d[1], d[2], d[3], d[4], st);
 }
 
 int nsgtObj_nsgtBatch(NSGTObj s, const float *data, int batch, float *mReal, float *mImag, float *cellReal,
@@ -446,35 +444,10 @@ int nsgtObj_nsgtBatch(NSGTObj s, const float *data, int batch, float *mReal, flo
     int rc = nsgt_device(s);
     if (rc) return rc;
     if (batch == 0) return AF_OK;
-    if (memKind == AFB200_MEM_DEVICE) return nsgt_run(s, data, batch, mReal, mImag, cellReal, cellImag, stream);
-
-    void *st = stream ? stream : s->stream;
-    const size_t N = (size_t)s->fftLength, outPer = (size_t)s->num * s->maxLen, cellPer = (size_t)s->totalLen;
-    if (!cellReal) return af_pipe_run(&s->pipe, nsgt_chunk, s, data, N, batch, mReal, mImag, outPer, st);
-    /* with the cells: chunks of about 64 MB of output, one after the other */
-    long long per = ((long long)64 << 20) / (long long)(sizeof(float) * 2 * (outPer + cellPer));
-    if (per < 1) per = 1;
-    if (per > batch) per = batch;
-    const int chunk = (int)per;
-    if ((rc = af_devbuf_reserve(&s->in, sizeof(float) * N * chunk)) ||
-        (rc = af_devbuf_reserve(&s->out0, sizeof(float) * outPer * chunk)) ||
-        (rc = af_devbuf_reserve(&s->out1, sizeof(float) * outPer * chunk)) ||
-        (rc = af_devbuf_reserve(&s->cell0, sizeof(float) * cellPer * chunk)) ||
-        (rc = af_devbuf_reserve(&s->cell1, sizeof(float) * cellPer * chunk)))
-        return rc;
-    for (int c0 = 0; c0 < batch; c0 += chunk) {
-        const int nb = batch - c0 < chunk ? batch - c0 : chunk;
-        if ((rc = af_memcpy_h2d(s->in.ptr, data + (size_t)c0 * N, sizeof(float) * N * nb, st)) ||
-            (rc = nsgt_run(s, (const float *)s->in.ptr, nb, (float *)s->out0.ptr, (float *)s->out1.ptr,
-                           (float *)s->cell0.ptr, (float *)s->cell1.ptr, st)) ||
-            (rc = af_memcpy_d2h(mReal + (size_t)c0 * outPer, s->out0.ptr, sizeof(float) * outPer * nb, st)) ||
-            (rc = af_memcpy_d2h(mImag + (size_t)c0 * outPer, s->out1.ptr, sizeof(float) * outPer * nb, st)) ||
-            (rc = af_memcpy_d2h(cellReal + (size_t)c0 * cellPer, s->cell0.ptr, sizeof(float) * cellPer * nb, st)) ||
-            (rc = af_memcpy_d2h(cellImag + (size_t)c0 * cellPer, s->cell1.ptr, sizeof(float) * cellPer * nb, st)) ||
-            (rc = af_stream_sync(st)))
-            return rc;
-    }
-    return AF_OK;
+    const size_t outPer = (size_t)s->num * s->maxLen, cellPer = (size_t)s->totalLen;
+    const AfPlane pl[5] = {{data, (size_t)s->fftLength, AF_IN, 0}, {mReal, outPer, AF_OUT, 0}, {mImag, outPer, AF_OUT, 0},
+                           {cellReal, cellPer, AF_OUT, 0}, {cellImag, cellPer, AF_OUT, 0}};
+    return af_run_batch(&s->pipe, memKind, stream, nsgt_chunk, s, pl, 5, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 void nsgtObj_nsgt(NSGTObj s, float *dataArr, float *mRealArr3, float *mImageArr3) {
@@ -485,10 +458,8 @@ void nsgtObj_nsgt(NSGTObj s, float *dataArr, float *mRealArr3, float *mImageArr3
 void nsgtObj_free(NSGTObj s) {
     if (!s) return;
     nsgt_device_tables_free(s);
-    af_devbuf_free(&s->spec); af_devbuf_free(&s->in); af_devbuf_free(&s->out0); af_devbuf_free(&s->out1);
-    af_devbuf_free(&s->cell0); af_devbuf_free(&s->cell1);
+    af_devbuf_free(&s->spec);
     af_pipe_free(&s->pipe);
-    af_stream_destroy(s->stream);
     free(s->lenArr); free(s->binBandArr); free(s->offArr); free(s->cellOff); free(s->map); free(s->groupStart);
     free(s->freBandArr); free(s->win); free(s->tab); free(s->filt); free(s->bands);
     free(s->cellRe); free(s->cellIm);

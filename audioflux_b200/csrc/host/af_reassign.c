@@ -19,8 +19,8 @@ struct OpaqueReassign {
     ReassignType reType;
     float thresh;
     int resultType, order;
-    void *stream;
-    AfDevBuf dIn, dS[6], dIdx[2], dMax, dAcc[2], dOut[2];
+    AfDevBuf dS[6], dIdx[2], dMax, dAcc[2];   /* the three STFTs (S_h only when the caller does not take it), cell planes */
+    AfPipe pipe;
 };
 
 int reassignObj_new(ReassignObj *out, int radix2Exp, int *samplate, WindowType *windowType, int *slideLength,
@@ -82,10 +82,10 @@ static int reassign_device(ReassignObj r, const float *dData, int dataLength, in
     const int needT = r->reType == Reassign_All || r->reType == Reassign_Time;
     /* S_h goes straight into the caller's second pair of planes when there is one (Reassign_None: into the first) */
     float *s1r = none ? dRe4 : dRe5, *s1i = none ? dIm4 : dIm5;
-    if (!s1r || !s1i) {
-        if ((rc = af_devbuf_reserve(&r->dS[0], plane)) || (rc = af_devbuf_reserve(&r->dS[1], plane))) return rc;
-        s1r = (float *)r->dS[0].ptr; s1i = (float *)r->dS[1].ptr;
-    }
+    if (!s1r && (rc = af_devbuf_reserve(&r->dS[0], plane))) return rc;
+    if (!s1i && (rc = af_devbuf_reserve(&r->dS[1], plane))) return rc;
+    if (!s1r) s1r = (float *)r->dS[0].ptr;
+    if (!s1i) s1i = (float *)r->dS[1].ptr;
     if ((rc = stftObj_stftBatch(r->stft[0], dData, dataLength, batch, s1r, s1i, AFB200_MEM_DEVICE, st))) return rc;
     if (none) return AF_OK;
     for (int k = 2; k < 6; k++) {
@@ -107,30 +107,30 @@ static int reassign_device(ReassignObj r, const float *dData, int dataLength, in
                               dRe4, dIm4, st);
 }
 
+typedef struct { ReassignObj r; int dataLength; } ReassignCall;
+
+static int reassign_chunk(void *p, int nb, float *const *d, void *st) {
+    const ReassignCall *a = (const ReassignCall *)p;
+    return reassign_device(a->r, d[0], a->dataLength, nb, d[1], d[2], d[3], d[4], st);
+}
+
 int reassignObj_reassignBatch(ReassignObj r, const float *data, int dataLength, int batch, float *re4, float *im4,
                               float *re5, float *im5, int memKind, void *stream) {
     if (!r || !data || !re4 || !im4 || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "reassignObj_reassignBatch: bad argument");
     af_clear_error();
     int rc = af_device_ready();
     if (rc) return rc;
-    if (memKind == AFB200_MEM_DEVICE) return reassign_device(r, data, dataLength, batch, re4, im4, re5, im5, stream);
-    if (!r->stream && (rc = af_stream_create(&r->stream))) return rc;
-    void *st = stream ? stream : r->stream;
-    const int T = reassignObj_calTimeLength(r, dataLength), W = r->fftLength / 2 + 1;
+    const int T = reassignObj_calTimeLength(r, dataLength);
     if (T <= 0) return AF_OK;
-    const size_t plane = sizeof(float) * (size_t)batch * T * W, inB = sizeof(float) * (size_t)batch * dataLength;
-    if ((rc = af_devbuf_reserve(&r->dIn, inB)) || (rc = af_devbuf_reserve(&r->dOut[0], plane)) || (rc = af_devbuf_reserve(&r->dOut[1], plane)) ||
-        (rc = af_devbuf_reserve(&r->dS[0], plane)) || (rc = af_devbuf_reserve(&r->dS[1], plane))) return rc;
-    if ((rc = af_memcpy_h2d(r->dIn.ptr, data, inB, st))) return rc;
+    /* Reassign_None: S_h itself into the first pair; else the reassigned planes are added into it (im4 only when
+     * resultType = 0 asks for it) and S_h goes to the second pair */
     const int none = r->reType == Reassign_None;
-    if (!none && ((rc = af_memcpy_h2d(r->dOut[0].ptr, re4, plane, st)) || (rc = af_memcpy_h2d(r->dOut[1].ptr, im4, plane, st)))) return rc;
-    if ((rc = reassign_device(r, (const float *)r->dIn.ptr, dataLength, batch, (float *)r->dOut[0].ptr, (float *)r->dOut[1].ptr,
-                              none ? NULL : (float *)r->dS[0].ptr, none ? NULL : (float *)r->dS[1].ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(re4, r->dOut[0].ptr, plane, st))) return rc;
-    if ((none || r->resultType == 0) && (rc = af_memcpy_d2h(im4, r->dOut[1].ptr, plane, st))) return rc;
-    if (!none && re5 && (rc = af_memcpy_d2h(re5, r->dS[0].ptr, plane, st))) return rc;
-    if (!none && im5 && (rc = af_memcpy_d2h(im5, r->dS[1].ptr, plane, st))) return rc;
-    return af_stream_sync(st);
+    ReassignCall a = {r, dataLength};
+    const size_t plane = (size_t)T * (r->fftLength / 2 + 1);
+    const AfPlane pl[5] = {{data, (size_t)dataLength, AF_IN, 0}, {re4, plane, none ? AF_OUT : AF_INOUT, 0},
+                           {im4, plane, none ? AF_OUT : r->resultType == 0 ? AF_INOUT : AF_IN, 0},
+                           {none ? NULL : re5, plane, AF_OUT, 0}, {none ? NULL : im5, plane, AF_OUT, 0}};
+    return af_run_batch(&r->pipe, memKind, stream, reassign_chunk, &a, pl, 5, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 void reassignObj_reassign(ReassignObj r, float *dataArr, int dataLength, float *mRealArr4, float *mImageArr4,
@@ -142,9 +142,9 @@ void reassignObj_reassign(ReassignObj r, float *dataArr, int dataLength, float *
 void reassignObj_free(ReassignObj r) {
     if (!r) return;
     for (int k = 0; k < 3; k++) stftObj_free(r->stft[k]);
-    af_devbuf_free(&r->dIn); af_devbuf_free(&r->dMax);
+    af_devbuf_free(&r->dMax);
     for (int k = 0; k < 6; k++) af_devbuf_free(&r->dS[k]);
-    for (int k = 0; k < 2; k++) { af_devbuf_free(&r->dIdx[k]); af_devbuf_free(&r->dAcc[k]); af_devbuf_free(&r->dOut[k]); }
-    af_stream_destroy(r->stream);
+    for (int k = 0; k < 2; k++) { af_devbuf_free(&r->dIdx[k]); af_devbuf_free(&r->dAcc[k]); }
+    af_pipe_free(&r->pipe);
     free(r);
 }

@@ -13,10 +13,9 @@ struct OpaqueSpectral {
     int contig, start, nb;      /* contig: bins start .. start+nb-1, else the owned list idx */
     int *idx;
     int idxDirty;
-    void *stream;
     float *dFre;
     int *dIdx;
-    AfDevBuf dIn, dPh, dOut;
+    AfPipe pipe;
 };
 
 static int needs_fre(int f) {
@@ -76,13 +75,18 @@ void spectralObj_setEdgeArr(SpectralObj s, int *indexArr, int indexLength) {
 static int spectral_device(SpectralObj s, int wantFre) {
     int rc = af_device_ready();
     if (rc) return rc;
-    if (!s->stream && (rc = af_stream_create(&s->stream))) return rc;
     if (wantFre && !s->dFre && (rc = af_dev_upload((void **)&s->dFre, s->fre, sizeof(float) * (size_t)s->num))) return rc;
     if (!s->contig && (s->idxDirty || !s->dIdx)) {
         if ((rc = af_dev_upload((void **)&s->dIdx, s->idx, sizeof(int) * (size_t)s->nb))) return rc;
         s->idxDirty = 0;
     }
     return AF_OK;
+}
+
+static int spectral_chunk(void *p, int nb, float *const *d, void *st) {
+    AfSpectralArgs a = *(const AfSpectralArgs *)p;
+    a.spec = d[0]; a.phase = d[1]; a.out = d[2]; a.batch = nb;
+    return af_launch_spectral(&a, st);
 }
 
 int spectralObj_spectralBatch(SpectralObj s, const float *spec, const float *phase, int timeLength, int batch,
@@ -123,25 +127,11 @@ int spectralObj_spectralBatch(SpectralObj s, const float *spec, const float *pha
         a.meanFre = m / (float)s->nb;
     }
     if (batch == 0) return AF_OK;
-
-    if (memKind == AFB200_MEM_DEVICE) {
-        a.spec = spec; a.phase = wantPh ? phase : NULL; a.out = out;
-        return af_launch_spectral(&a, stream);     /* asynchronous on the caller's stream */
-    }
-    void *st = stream ? stream : s->stream;
-    const size_t inB = sizeof(float) * (size_t)batch * timeLength * s->num;
-    const size_t outB = sizeof(float) * (size_t)planes * batch * timeLength;
-    if ((rc = af_devbuf_reserve(&s->dIn, inB)) || (rc = af_devbuf_reserve(&s->dOut, outB))) return rc;
-    if (wantPh && (rc = af_devbuf_reserve(&s->dPh, inB))) return rc;
-    if ((rc = af_memcpy_h2d(s->dIn.ptr, spec, inB, st))) return rc;
-    if (wantPh && (rc = af_memcpy_h2d(s->dPh.ptr, phase, inB, st))) return rc;
-    if (readOut && (rc = af_memcpy_h2d(s->dOut.ptr, out, outB, st))) return rc;
-    a.spec = (const float *)s->dIn.ptr;
-    a.phase = wantPh ? (const float *)s->dPh.ptr : NULL;
-    a.out = (float *)s->dOut.ptr;
-    if ((rc = af_launch_spectral(&a, st))) return rc;
-    if ((rc = af_memcpy_d2h(out, s->dOut.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    /* clips as items; `out` holds `planes` planes of batch x T, so it moves as one layered plane */
+    const size_t in = (size_t)timeLength * s->num;
+    const AfPlane pl[3] = {{spec, in, AF_IN, 0}, {wantPh ? phase : NULL, in, AF_IN, 0},
+                           {out, (size_t)timeLength, readOut ? AF_INOUT : AF_OUT, planes}};
+    return af_run_batch(&s->pipe, memKind, stream, spectral_chunk, &a, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 /* ---- the reference's per-feature entry points: one clip of timeLength frames, host pointers ---- */
@@ -209,9 +199,8 @@ void spectralObj_var(SpectralObj s, float *m, float *v, float *f) {
 
 void spectralObj_free(SpectralObj s) {
     if (!s) return;
-    af_devbuf_free(&s->dIn); af_devbuf_free(&s->dPh); af_devbuf_free(&s->dOut);
+    af_pipe_free(&s->pipe);
     af_dev_free(s->dFre); af_dev_free(s->dIdx);
-    af_stream_destroy(s->stream);
     free(s->fre); free(s->idx);
     free(s);
 }

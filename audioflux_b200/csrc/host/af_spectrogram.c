@@ -14,15 +14,15 @@
 struct OpaqueSpectrogram {
     BFTObj core;
     XXCCObj cc;
-    int num, fftLength, samplate, lowIndex, highIndex, timeLength;
+    int num, fftLength, slideLength, samplate, lowIndex, highIndex, timeLength;
     SpectralFilterBankScaleType scaleType;
     SpectralFilterBankStyleType styleType;
     float *freBandArr;      /* Linear: own arrays (grid of __vlinspace); else borrowed from the core */
     int *binBandArr;
     int ownBands;
-    void *cuStream;         /* deconv with host pointers: staging buffers and the stream they are filled on */
-    AfDevBuf dPostA, dPostB, dPostOut;
-    STFTObj stream;         /* isContinue = 1: an STFT object that only keeps the tail between calls (stft_algorithm.c:474-599) */
+    int isContinue;         /* the samples that did not complete a frame wait in `tail` for the next call */
+    AfTail tail;
+    AfPipe pipe;
 };
 
 int spectrogramObj_new(SpectrogramObj *out, int num, int *samplate, float *lowFre, float *highFre, int *binPerOctave,
@@ -85,14 +85,10 @@ int spectrogramObj_new(SpectrogramObj *out, int num, int *samplate, float *lowFr
     if (rc) { free(s); return rc; }
     bftObj_setResultType(s->core, 1);
     if (xxccObj_new(&s->cc, num)) { spectrogramObj_free(s); return -1; }
-    if (streaming) {
-        /* the reference hands isContinue to its STFT object (spectrogram_algorithm.c:655-664): samples that did not
-         * complete a frame wait for the next call.  Same bookkeeping here, in front of the fused / general kernels. */
-        WindowType wt = (WindowType)spec.windowType;
-        int one = 1;
-        if (stftObj_new(&s->stream, r, &wt, &spec.slideLength, &one)) { spectrogramObj_free(s); return -1; }
-    }
-    s->num = num; s->fftLength = n; s->samplate = sr; s->lowIndex = spec.lowIndex; s->highIndex = spec.highIndex;
+    /* the reference hands isContinue to its STFT object (spectrogram_algorithm.c:655-664): samples that did not
+     * complete a frame wait for the next call.  Same bookkeeping here, in front of the fused / general kernels. */
+    s->isContinue = streaming;
+    s->num = num; s->fftLength = n; s->slideLength = spec.slideLength; s->samplate = sr; s->lowIndex = spec.lowIndex; s->highIndex = spec.highIndex;
     s->scaleType = scale; s->styleType = (SpectralFilterBankStyleType)spec.styleType;
     if (scale == SpectralFilterBankScale_Linear) {
         /* :1909-1941: slices of linspace(0, sr/2, n/2+1) and arange(n/2+1) starting at lowIndex */
@@ -154,22 +150,34 @@ void spectrogramObj_enableDebug(SpectrogramObj s, int flag) { (void)s; (void)fla
 void spectrogramObj_setDataNormValue(SpectrogramObj s, float v) { if (s) bftObj_setDataNormValue(s->core, v); }
 int spectrogramObj_calTimeLength(SpectrogramObj s, int dataLength) {
     if (!s) return 0;
-    return s->stream ? stftObj_calTimeLength(s->stream, dataLength) : bftObj_calTimeLength(s->core, dataLength);   /* :848-853 */
+    return bftObj_calTimeLength(s->core, dataLength + (s->isContinue ? s->tail.length : 0));   /* :848-853 */
 }
 float *spectrogramObj_getFreBandArr(SpectrogramObj s) { return s ? s->freBandArr : NULL; }
 int *spectrogramObj_getBinBandArr(SpectrogramObj s) { return s ? s->binBandArr : NULL; }
 int spectrogramObj_getBandNum(SpectrogramObj s) { return s ? s->num : 0; }
 int spectrogramObj_getBinBandLength(SpectrogramObj s) { return s ? s->num : 0; }
 
+typedef struct { SpectrogramObj s; int dataLength; } SpectrogramCall;
+
+static int spectrogram_chunk(void *p, int nb, float *const *d, void *st) {
+    const SpectrogramCall *a = (const SpectrogramCall *)p;
+    return af_bft_spectrogram(a->s->core, d[0], a->dataLength, nb, d[1], a->s->lowIndex, a->s->num, d[2], st);
+}
+
 /* batch x dataLength -> spect: batch x T x bandNum (and phase, Linear scale only, may be NULL) */
 int spectrogramObj_spectrogramBatch(SpectrogramObj s, const float *data, int dataLength, int batch, float *spect,
                                     float *phase, int memKind, void *stream) {
     if (!s || !data || !spect || dataLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "spectrogramObj_spectrogramBatch: bad argument");
-    int rc = bftObj_bftBatch(s->core, data, dataLength, batch, spect, NULL, memKind, stream);
+    af_clear_error();
+    int rc = af_bft_device(s->core);
     if (rc) return rc;
-    if (phase && s->scaleType == SpectralFilterBankScale_Linear)
-        rc = af_bft_phase(s->core, data, dataLength, batch, s->lowIndex, s->num, phase, memKind, stream);
-    return rc;
+    const int T = bftObj_calTimeLength(s->core, dataLength);
+    if (T <= 0) return AF_OK;
+    SpectrogramCall a = {s, dataLength};
+    const size_t outPer = (size_t)T * s->num;
+    const AfPlane pl[3] = {{data, (size_t)dataLength, AF_IN, 0}, {spect, outPer, AF_OUT, 0},
+                           {s->scaleType == SpectralFilterBankScale_Linear ? phase : NULL, outPer, AF_OUT, 0}};
+    return af_run_batch(&s->pipe, memKind, stream, spectrogram_chunk, &a, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 /* the fused path of the headline metric behind this front door: batch x dataLength -> batch x T x ccNum */
@@ -182,9 +190,9 @@ int spectrogramObj_mfccBatch(SpectrogramObj s, const float *data, int dataLength
 void spectrogramObj_spectrogram(SpectrogramObj s, float *dataArr, int dataLength, float *mSpectArr, float *mPhaseArr) {
     if (!s || !dataArr || dataLength <= 0 || !mSpectArr) return;      /* :966-978: nothing to do without data */
     const float *x = dataArr;
-    if (s->stream) {                                                  /* streaming: tail of the earlier calls ++ dataArr */
+    if (s->isContinue) {                                              /* streaming: tail of the earlier calls ++ dataArr */
         s->timeLength = 0;
-        if (!af_stft_continue_assemble(s->stream, dataArr, dataLength, &x, &dataLength)) return;
+        if (!af_tail_assemble(&s->tail, s->fftLength, s->slideLength, dataArr, dataLength, &x, &dataLength)) return;
     }
     s->timeLength = bftObj_calTimeLength(s->core, dataLength);
     spectrogramObj_spectrogramBatch(s, x, dataLength, 1, mSpectArr, mPhaseArr, AFB200_MEM_HOST, NULL);
@@ -223,17 +231,7 @@ int spectrogramObj_deconvBatch(SpectrogramObj s, const float *in, int rows, floa
     af_clear_error();
     int rc = af_device_ready();
     if (rc) return rc;
-    if (rows == 0) return AF_OK;
-    if (memKind == AFB200_MEM_DEVICE) return af_launch_cq_deconv(in, rows, s->num, 1, 0, 12, timbre, pitch, stream);
-    if (!s->cuStream && (rc = af_stream_create(&s->cuStream))) return rc;
-    void *st = stream ? stream : s->cuStream;
-    const size_t bytes = sizeof(float) * (size_t)rows * s->num;
-    if ((rc = af_devbuf_reserve(&s->dPostA, bytes)) || (rc = af_devbuf_reserve(&s->dPostOut, bytes)) ||
-        (rc = af_devbuf_reserve(&s->dPostB, bytes))) return rc;
-    if ((rc = af_memcpy_h2d(s->dPostA.ptr, in, bytes, st))) return rc;
-    if ((rc = af_launch_cq_deconv((const float *)s->dPostA.ptr, rows, s->num, 1, 0, 12, (float *)s->dPostOut.ptr, (float *)s->dPostB.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(timbre, s->dPostOut.ptr, bytes, st)) || (rc = af_memcpy_d2h(pitch, s->dPostB.ptr, bytes, st))) return rc;
-    return af_stream_sync(st);
+    return af_deconv_batch(&s->pipe, in, rows, s->num, 1, 0, 12, timbre, pitch, memKind, stream);
 }
 
 /* mDataArr1: timeLength x num of the LAST spectrogram call -> mDataArr2 (timbre / tone), mDataArr3 (pitch) */
@@ -244,11 +242,10 @@ void spectrogramObj_deconv(SpectrogramObj s, float *mDataArr1, float *mDataArr2,
 
 void spectrogramObj_free(SpectrogramObj s) {
     if (!s) return;
-    af_devbuf_free(&s->dPostA); af_devbuf_free(&s->dPostB); af_devbuf_free(&s->dPostOut);
-    af_stream_destroy(s->cuStream);
+    af_pipe_free(&s->pipe);
+    af_tail_free(&s->tail);
     if (s->ownBands) { free(s->freBandArr); free(s->binBandArr); }
     xxccObj_free(s->cc);
-    stftObj_free(s->stream);
     bftObj_free(s->core);
     free(s);
 }

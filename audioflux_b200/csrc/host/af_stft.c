@@ -16,17 +16,13 @@ struct OpaqueSTFT {
     PaddingModeType mode;
     float padValue1, padValue2;
     /* device side (lazy) */
-    int devReady, windowDirty;
-    void *stream;
+    int windowDirty;
     float *dWindow;
-    AfDevBuf dIn, dRe, dIm, dFrames;
-    AfPipe pipe;                   /* host-pointer batches: chunked copy-in / transform / copy-out */
-    int pipeLength;
-    /* streaming (isContinue, stft_algorithm.c:474-599): the samples that did not complete a hop are carried to the next call */
+    AfDevBuf dFrames;              /* inverse: frames before the overlap-add */
+    AfPipe pipe;
+    /* streaming (isContinue, stft_algorithm.c:474-599) */
     int isContinue;
-    float *tail;                   /* host, fftLength + slideLength floats */
-    int tailLength;                /* may be negative when slideLength > fftLength: samples of the next call to skip */
-    float *cur; size_t curCap;     /* host staging: tail + new samples */
+    AfTail tail;
     int timeLength;                /* frames of the last stftObj_stft call */
 };
 
@@ -76,7 +72,7 @@ static int time_length(const struct OpaqueSTFT *s, int dataLength) {
 }
 int stftObj_calTimeLength(STFTObj s, int dataLength) {
     if (!s) return 0;
-    if (!s->isPad && s->isContinue) dataLength += s->tailLength;         /* stft_algorithm.c:242-245 */
+    if (!s->isPad && s->isContinue) dataLength += s->tail.length;         /* stft_algorithm.c:242-245 */
     return time_length(s, dataLength);
 }
 int stftObj_calDataLength(STFTObj s, int timeLength) { return s ? (timeLength - 1) * s->slideLength + s->fftLength : 0; }
@@ -87,10 +83,6 @@ void stftObj_debug(STFTObj s) {
 static int stft_device(STFTObj s) {
     int rc = af_device_ready();
     if (rc) return rc;
-    if (!s->devReady) {
-        if ((rc = af_stream_create(&s->stream))) return rc;
-        s->devReady = 1;
-    }
     if (s->windowDirty) {
         af_dev_free(s->dWindow); s->dWindow = NULL;
         if ((rc = af_dev_upload((void **)&s->dWindow, s->window, sizeof(float) * (size_t)s->fftLength))) return rc;
@@ -120,80 +112,76 @@ static int stft_frame_src(STFTObj s, int dataLength, int batch, AfFrameSrc *src)
     return AF_OK;
 }
 
-/* streaming bookkeeping of __stftObj_dealData (stft_algorithm.c:474-599, non-padding mode): returns the samples to
- * transform (tail of the previous calls + the new ones) in *cur / *curLength, or 0 when they do not fill a frame yet */
-static int stft_continue_assemble(STFTObj s, const float *data, int dataLength, const float **cur, int *curLength) {
-    const int n = s->fftLength, hop = s->slideLength;
-    if (!s->tail) {
-        s->tail = (float *)calloc((size_t)n + (size_t)hop + 1, sizeof(float));
-        if (!s->tail) return 0;
+/* streaming bookkeeping of __stftObj_dealData (stft_algorithm.c:474-599, non-padding mode) */
+int af_tail_assemble(AfTail *t, int n, int hop, const float *data, int dataLength, const float **cur, int *curLength) {
+    if (!t->buf) {
+        t->buf = (float *)calloc((size_t)n + (size_t)hop + 1, sizeof(float));
+        if (!t->buf) return 0;
     }
-    const int total = s->tailLength + dataLength;
+    const int total = t->length + dataLength;
     if (total < n) {                                          /* not a frame yet: keep everything */
-        if (s->tailLength >= 0) memcpy(s->tail + s->tailLength, data, sizeof(float) * (size_t)dataLength);
-        else if (dataLength + s->tailLength > 0) memcpy(s->tail, data - s->tailLength, sizeof(float) * (size_t)(dataLength + s->tailLength));
-        s->tailLength = total;
-        s->timeLength = 0;
+        if (t->length >= 0) memcpy(t->buf + t->length, data, sizeof(float) * (size_t)dataLength);
+        else if (dataLength + t->length > 0) memcpy(t->buf, data - t->length, sizeof(float) * (size_t)(dataLength + t->length));
+        t->length = total;
         return 0;
     }
     const int tailLen = (total - n) % hop + (n - hop);      /* __calTimeAndTailLen */
-    if ((size_t)total + (size_t)n > s->curCap) {
-        free(s->cur);
-        s->curCap = (size_t)total + (size_t)n;
-        s->cur = (float *)malloc(sizeof(float) * s->curCap);
-        if (!s->cur) { s->curCap = 0; return 0; }
+    if ((size_t)total + (size_t)n > t->curCap) {
+        free(t->cur);
+        t->curCap = (size_t)total + (size_t)n;
+        t->cur = (float *)malloc(sizeof(float) * t->curCap);
+        if (!t->cur) { t->curCap = 0; return 0; }
     }
     int len = 0;
-    if (s->tailLength < 0) {
-        len = dataLength + s->tailLength;
-        memcpy(s->cur, data - s->tailLength, sizeof(float) * (size_t)len);
+    if (t->length < 0) {
+        len = dataLength + t->length;
+        memcpy(t->cur, data - t->length, sizeof(float) * (size_t)len);
     } else {
-        if (s->tailLength > 0) memcpy(s->cur, s->tail, sizeof(float) * (size_t)s->tailLength);
-        memcpy(s->cur + s->tailLength, data, sizeof(float) * (size_t)dataLength);
-        len = s->tailLength + dataLength;
+        if (t->length > 0) memcpy(t->cur, t->buf, sizeof(float) * (size_t)t->length);
+        memcpy(t->cur + t->length, data, sizeof(float) * (size_t)dataLength);
+        len = t->length + dataLength;
     }
-    if (tailLen > 0) memcpy(s->tail, s->cur + (len - tailLen), sizeof(float) * (size_t)tailLen);
-    s->tailLength = tailLen;
-    *cur = s->cur; *curLength = len;
+    if (tailLen > 0) memcpy(t->buf, t->cur + (len - tailLen), sizeof(float) * (size_t)tailLen);
+    t->length = tailLen;
+    *cur = t->cur; *curLength = len;
     return 1;
 }
 
-/* the same bookkeeping for objects that frame through an STFT object of their own (SpectrogramObj streaming) */
-int af_stft_continue_assemble(STFTObj s, const float *data, int dataLength, const float **cur, int *curLength) {
-    if (!s || !data || dataLength <= 0) return 0;
-    return stft_continue_assemble(s, data, dataLength, cur, curLength);
+void af_tail_free(AfTail *t) { free(t->buf); free(t->cur); memset(t, 0, sizeof(*t)); }
+
+typedef struct { STFTObj s; int dataLength, mode; } StftCall;
+
+static int stft_chunk(void *p, int nb, float *const *d, void *st) {
+    const StftCall *c = (const StftCall *)p;
+    AfFrameSrc src;
+    int rc = stft_frame_src(c->s, c->dataLength, nb, &src);
+    if (rc) return rc;
+    src.data = d[0];
+    return af_launch_stft(&src, c->mode, 1.0f, d[1], d[2], st);
+}
+
+/* mode AF_STFT_HALF (planes batch x T x (n/2+1)) or AF_STFT_FULL (mirrored, batch x T x n) */
+static int stft_run(STFTObj s, const float *data, int dataLength, int batch, int mode, float *re, float *im,
+                    int memKind, void *stream) {
+    const size_t outPer = (size_t)time_length(s, dataLength) * (mode == AF_STFT_FULL ? s->fftLength : s->fftLength / 2 + 1);
+    StftCall c = {s, dataLength, mode};
+    const AfPlane pl[3] = {{data, (size_t)dataLength, AF_IN, 0}, {re, outPer, AF_OUT, 0}, {im, outPer, AF_OUT, 0}};
+    return af_run_batch(&s->pipe, memKind, stream, stft_chunk, &c, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 void stftObj_stft(STFTObj s, float *dataArr, int dataLength, float *mRealArr, float *mImageArr) {
     if (!s || !dataArr || dataLength <= 0 || !mRealArr || !mImageArr) return;
-    af_clear_error();
     const float *x = dataArr;
     int len = dataLength;
-    if (s->isContinue && !s->isPad) {
-        if (!stft_continue_assemble(s, dataArr, dataLength, &x, &len)) return;
+    if (s->isContinue && !s->isPad && !af_tail_assemble(&s->tail, s->fftLength, s->slideLength, dataArr, dataLength, &x, &len)) {
+        s->timeLength = 0;
+        return;
     }
+    af_clear_error();
     if (stft_device(s)) return;
-    AfFrameSrc src;
-    if (stft_frame_src(s, len, 1, &src)) return;
-    s->timeLength = src.timeLength;
-    if (src.timeLength <= 0) return;
-    size_t plane = sizeof(float) * (size_t)src.timeLength * s->fftLength;
-    if (af_devbuf_reserve(&s->dIn, sizeof(float) * (size_t)len) || af_devbuf_reserve(&s->dRe, plane) ||
-        af_devbuf_reserve(&s->dIm, plane)) return;
-    if (af_memcpy_h2d(s->dIn.ptr, x, sizeof(float) * (size_t)len, s->stream)) return;
-    src.data = (const float *)s->dIn.ptr;
-    if (af_launch_stft(&src, AF_STFT_FULL, 1.0f, (float *)s->dRe.ptr, (float *)s->dIm.ptr, s->stream)) return;
-    if (af_memcpy_d2h(mRealArr, s->dRe.ptr, plane, s->stream) || af_memcpy_d2h(mImageArr, s->dIm.ptr, plane, s->stream)) return;
-    af_stream_sync(s->stream);
-}
-
-static int stft_chunk(void *obj, const float *dIn, int nb, float *dOut0, float *dOut1, void *st) {
-    STFTObj s = (STFTObj)obj;
-    AfFrameSrc src;
-    int rc = stft_frame_src(s, s->pipeLength, nb, &src);
-    if (rc) return rc;
-    src.data = dIn;
-    return af_launch_stft(&src, AF_STFT_HALF, 1.0f, dOut0, dOut1, st);
+    s->timeLength = time_length(s, len);
+    if (s->timeLength <= 0) return;
+    stft_run(s, x, len, 1, AF_STFT_FULL, mRealArr, mImageArr, AFB200_MEM_HOST, NULL);
 }
 
 int stftObj_stftBatch(STFTObj s, const float *data, int dataLength, int batch, float *mReal, float *mImag,
@@ -202,25 +190,25 @@ int stftObj_stftBatch(STFTObj s, const float *data, int dataLength, int batch, f
     af_clear_error();
     int rc = stft_device(s);
     if (rc) return rc;
-    AfFrameSrc src;
-    if ((rc = stft_frame_src(s, dataLength, batch, &src))) return rc;
-    if (src.timeLength <= 0) return AF_OK;
-    void *st = stream ? stream : s->stream;
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;                      /* NULL = the CUDA default stream */
-        src.data = data;
-        if ((rc = af_launch_stft(&src, AF_STFT_HALF, 1.0f, mReal, mImag, st))) return rc;
-        return AF_OK;                       /* asynchronous on the caller's stream */
-    }
-    s->pipeLength = dataLength;
-    return af_pipe_run(&s->pipe, stft_chunk, s, data, (size_t)dataLength, batch, mReal, mImag,
-                       (size_t)src.timeLength * (s->fftLength / 2 + 1), st);
+    if (time_length(s, dataLength) <= 0) return AF_OK;
+    return stft_run(s, data, dataLength, batch, AF_STFT_HALF, mReal, mImag, memKind, stream);
 }
 
 /* ---- inverse: planes [batch x T x width] -> data [batch x ((T-1)*hop + n)]  (stft_algorithm.c:304-409) ----
  * width = fftLength (full mirrored planes, the reference layout) or fftLength/2+1 (what stftObj_stftBatch produces).
  * As in the reference the frames are ADDED to what `data` holds before the division by the window sum, so the
  * caller passes a zeroed buffer. */
+typedef struct { STFTObj s; int timeLength, specWidth, methodType; } IstftCall;
+
+static int istft_chunk(void *p, int nb, float *const *d, void *st) {
+    const IstftCall *c = (const IstftCall *)p;
+    STFTObj s = c->s;
+    int rc = af_devbuf_reserve(&s->dFrames, sizeof(float) * (size_t)nb * c->timeLength * s->fftLength);
+    if (rc) return rc;
+    return af_launch_istft(d[0], d[1], c->specWidth, s->fftLength, s->slideLength, c->timeLength, nb,
+                           s->useWindow ? s->dWindow : NULL, c->methodType, (float *)s->dFrames.ptr, d[2], st);
+}
+
 int stftObj_istftBatch(STFTObj s, const float *mReal, const float *mImag, int timeLength, int batch, int specWidth,
                        int methodType, float *data, int memKind, void *stream) {
     if (!s || !mReal || !mImag || !data || timeLength <= 0 || batch <= 0) return af_fail(AF_ERR_ARG, "stftObj_istftBatch: bad argument");
@@ -229,22 +217,11 @@ int stftObj_istftBatch(STFTObj s, const float *mReal, const float *mImag, int ti
     af_clear_error();
     int rc = stft_device(s);
     if (rc) return rc;
-    const int n = s->fftLength, dataLength = (timeLength - 1) * s->slideLength + n;
-    const size_t plane = sizeof(float) * (size_t)batch * timeLength * specWidth;
-    const size_t frameB = sizeof(float) * (size_t)batch * timeLength * n, dataB = sizeof(float) * (size_t)batch * dataLength;
-    if ((rc = af_devbuf_reserve(&s->dFrames, frameB))) return rc;
-    const float *win = s->useWindow ? s->dWindow : NULL;
-    if (memKind == AFB200_MEM_DEVICE)
-        return af_launch_istft(mReal, mImag, specWidth, n, s->slideLength, timeLength, batch, win, methodType,
-                               (float *)s->dFrames.ptr, data, stream);
-    void *st = stream ? stream : s->stream;
-    if ((rc = af_devbuf_reserve(&s->dRe, plane)) || (rc = af_devbuf_reserve(&s->dIm, plane)) || (rc = af_devbuf_reserve(&s->dIn, dataB))) return rc;
-    if ((rc = af_memcpy_h2d(s->dRe.ptr, mReal, plane, st)) || (rc = af_memcpy_h2d(s->dIm.ptr, mImag, plane, st)) ||
-        (rc = af_memcpy_h2d(s->dIn.ptr, data, dataB, st))) return rc;
-    if ((rc = af_launch_istft((const float *)s->dRe.ptr, (const float *)s->dIm.ptr, specWidth, n, s->slideLength, timeLength,
-                              batch, win, methodType, (float *)s->dFrames.ptr, (float *)s->dIn.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(data, s->dIn.ptr, dataB, st))) return rc;
-    return af_stream_sync(st);
+    IstftCall c = {s, timeLength, specWidth, methodType};
+    const size_t plane = (size_t)timeLength * specWidth;
+    const AfPlane pl[3] = {{mReal, plane, AF_IN, 0}, {mImag, plane, AF_IN, 0},
+                           {data, (size_t)(timeLength - 1) * s->slideLength + s->fftLength, AF_INOUT, 0}};
+    return af_run_batch(&s->pipe, memKind, stream, istft_chunk, &c, pl, 3, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 void stftObj_istft(STFTObj s, float *mRealArr, float *mImageArr, int timeLength, int methodType, float *dataArr) {
@@ -254,10 +231,10 @@ void stftObj_istft(STFTObj s, float *mRealArr, float *mImageArr, int timeLength,
 
 void stftObj_free(STFTObj s) {
     if (!s) return;
-    af_devbuf_free(&s->dIn); af_devbuf_free(&s->dRe); af_devbuf_free(&s->dIm); af_devbuf_free(&s->dFrames);
+    af_devbuf_free(&s->dFrames);
     af_pipe_free(&s->pipe);
     af_dev_free(s->dWindow);
-    af_stream_destroy(s->stream);
-    free(s->window); free(s->tail); free(s->cur);
+    free(s->window);
+    af_tail_free(&s->tail);
     free(s);
 }

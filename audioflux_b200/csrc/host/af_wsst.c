@@ -19,9 +19,9 @@ struct OpaqueWSST {
     int num, fftLength, samplate, order;
     float thresh;
     SpectralFilterBankScaleType scaleType;
-    void *stream;
     float *dNorm;                     /* freArr / samplate (mel / bark / erb index) */
-    AfDevBuf dIn, dW[4], dOut[2], dIdx;
+    AfDevBuf dW[4], dIdx;             /* W (when the caller does not take it) and W', row indices */
+    AfPipe pipe;
 };
 
 static int upload_norm(const float *fre, int num, int samplate, float **dNorm) {
@@ -86,35 +86,29 @@ int wsstObj_wsstDevice(WSSTObj w, const float *dData, float *dOutRe, float *dOut
     return af_launch_squeeze_scatter(wr, wi, (const int *)w->dIdx.ptr, num, n, w->thresh, dOutRe, dOutIm, st);
 }
 
+static int wsst_chunk(void *p, int nb, float *const *d, void *st) {
+    (void)nb;                                            /* one clip */
+    return wsstObj_wsstDevice((WSSTObj)p, d[0], d[1], d[2], d[3], d[4], st);
+}
+
 void wsstObj_wsst(WSSTObj w, float *dataArr, float *mRealArr4, float *mImageArr4, float *mRealArr5, float *mImageArr5) {
     if (!w || !dataArr || !mRealArr4 || !mImageArr4) return;
     af_clear_error();
     if (af_device_ready()) return;
-    if (!w->stream && af_stream_create(&w->stream)) return;
-    void *st = w->stream;
-    const int num = w->num, n = w->fftLength;
-    const size_t plane = sizeof(float) * (size_t)num * n;
-    if (af_devbuf_reserve(&w->dIn, sizeof(float) * (size_t)n) || af_devbuf_reserve(&w->dOut[0], plane) || af_devbuf_reserve(&w->dOut[1], plane)) return;
-    for (int i = 0; i < 2; i++) if (af_devbuf_reserve(&w->dW[i], plane)) return;
-    if (af_memcpy_h2d(w->dIn.ptr, dataArr, sizeof(float) * (size_t)n, st)) return;
     /* the reference ADDS into the caller's planes */
-    if (af_memcpy_h2d(w->dOut[0].ptr, mRealArr4, plane, st) || af_memcpy_h2d(w->dOut[1].ptr, mImageArr4, plane, st)) return;
-    if (wsstObj_wsstDevice(w, (const float *)w->dIn.ptr, (float *)w->dOut[0].ptr, (float *)w->dOut[1].ptr,
-                           (float *)w->dW[0].ptr, (float *)w->dW[1].ptr, st)) return;
-    if (af_memcpy_d2h(mRealArr4, w->dOut[0].ptr, plane, st) || af_memcpy_d2h(mImageArr4, w->dOut[1].ptr, plane, st)) return;
-    if (mRealArr5 && af_memcpy_d2h(mRealArr5, w->dW[0].ptr, plane, st)) return;
-    if (mImageArr5 && af_memcpy_d2h(mImageArr5, w->dW[1].ptr, plane, st)) return;
-    af_stream_sync(st);
+    const size_t plane = (size_t)w->num * w->fftLength;
+    const AfPlane pl[5] = {{dataArr, (size_t)w->fftLength, AF_IN, 0}, {mRealArr4, plane, AF_INOUT, 0}, {mImageArr4, plane, AF_INOUT, 0},
+                           {mRealArr5, plane, AF_OUT, 0}, {mImageArr5, plane, AF_OUT, 0}};
+    af_run_batch(&w->pipe, AFB200_MEM_HOST, NULL, wsst_chunk, w, pl, 5, 1, AF_PIPE_CHUNK_BYTES);
 }
 
 void wsstObj_free(WSSTObj w) {
     if (!w) return;
     cwtObj_free(w->cwt);
-    af_devbuf_free(&w->dIn); af_devbuf_free(&w->dIdx);
+    af_devbuf_free(&w->dIdx);
     for (int i = 0; i < 4; i++) af_devbuf_free(&w->dW[i]);
-    for (int i = 0; i < 2; i++) af_devbuf_free(&w->dOut[i]);
     af_dev_free(w->dNorm);
-    af_stream_destroy(w->stream);
+    af_pipe_free(&w->pipe);
     free(w);
 }
 
@@ -122,8 +116,8 @@ void wsstObj_free(WSSTObj w) {
 struct OpaqueSynsq {
     int num, fftLength, samplate, order;
     float thresh;
-    void *stream;
-    AfDevBuf dIn[2], dOut[2], dIdx, dNorm;
+    AfDevBuf dIdx, dNorm;
+    AfPipe pipe;
 };
 
 int synsqObj_new(SynsqObj *out, int num, int radix2Exp, int *samplate, int *order, float *thresh) {
@@ -164,28 +158,30 @@ int synsqObj_synsqDevice(SynsqObj s, const float *freArr /* host, num */, int sc
     return af_launch_squeeze_scatter(dRe, dIm, (const int *)s->dIdx.ptr, num, n, s->thresh, dOutRe, dOutIm, st);
 }
 
+typedef struct { SynsqObj s; const float *freArr; int scaleType; } SynsqCall;
+
+static int synsq_chunk(void *p, int nb, float *const *d, void *st) {
+    const SynsqCall *a = (const SynsqCall *)p;
+    (void)nb;                                            /* one matrix */
+    return synsqObj_synsqDevice(a->s, a->freArr, a->scaleType, d[0], d[1], d[2], d[3], st);
+}
+
 void synsqObj_synsq(SynsqObj s, float *freArr, SpectralFilterBankScaleType scaleType, float *mRealArr1, float *mImageArr1,
                     float *mRealArr2, float *mImageArr2) {
     if (!s || !freArr || !mRealArr1 || !mImageArr1 || !mRealArr2 || !mImageArr2) return;
     if (scaleType > SpectralFilterBankScale_Log) { printf("scaleType is error!\n"); return; }
     af_clear_error();
     if (af_device_ready()) return;
-    if (!s->stream && af_stream_create(&s->stream)) return;
-    void *st = s->stream;
-    const size_t plane = sizeof(float) * (size_t)s->num * s->fftLength;
-    for (int i = 0; i < 2; i++) if (af_devbuf_reserve(&s->dIn[i], plane) || af_devbuf_reserve(&s->dOut[i], plane)) return;
-    if (af_memcpy_h2d(s->dIn[0].ptr, mRealArr1, plane, st) || af_memcpy_h2d(s->dIn[1].ptr, mImageArr1, plane, st)) return;
-    if (af_memcpy_h2d(s->dOut[0].ptr, mRealArr2, plane, st) || af_memcpy_h2d(s->dOut[1].ptr, mImageArr2, plane, st)) return;
-    if (synsqObj_synsqDevice(s, freArr, (int)scaleType, (const float *)s->dIn[0].ptr, (const float *)s->dIn[1].ptr,
-                             (float *)s->dOut[0].ptr, (float *)s->dOut[1].ptr, st)) return;
-    if (af_memcpy_d2h(mRealArr2, s->dOut[0].ptr, plane, st) || af_memcpy_d2h(mImageArr2, s->dOut[1].ptr, plane, st)) return;
-    af_stream_sync(st);
+    SynsqCall a = {s, freArr, (int)scaleType};
+    const size_t plane = (size_t)s->num * s->fftLength;
+    const AfPlane pl[4] = {{mRealArr1, plane, AF_IN, 0}, {mImageArr1, plane, AF_IN, 0},
+                           {mRealArr2, plane, AF_INOUT, 0}, {mImageArr2, plane, AF_INOUT, 0}};
+    af_run_batch(&s->pipe, AFB200_MEM_HOST, NULL, synsq_chunk, &a, pl, 4, 1, AF_PIPE_CHUNK_BYTES);
 }
 
 void synsqObj_free(SynsqObj s) {
     if (!s) return;
-    for (int i = 0; i < 2; i++) { af_devbuf_free(&s->dIn[i]); af_devbuf_free(&s->dOut[i]); }
     af_devbuf_free(&s->dIdx); af_devbuf_free(&s->dNorm);
-    af_stream_destroy(s->stream);
+    af_pipe_free(&s->pipe);
     free(s);
 }

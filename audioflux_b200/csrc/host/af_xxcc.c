@@ -7,10 +7,8 @@
 
 struct OpaqueXXCC {
     int num, timeLength;
-    int devReady;
-    void *stream;
     float *dDctT;               /* device, transposed ortho DCT-II [num][num] */
-    AfDevBuf dIn, dOut, dEnergy, dD1, dD2;
+    AfPipe pipe;
 };
 
 int xxccObj_new(XXCCObj *out, int num) {
@@ -29,18 +27,21 @@ void xxccObj_setTimeLength(XXCCObj x, int timeLength) { if (x) x->timeLength = t
 static int xxcc_device(XXCCObj x) {
     int rc = af_device_ready();
     if (rc) return rc;
-    if (x->devReady) return AF_OK;
-    if ((rc = af_stream_create(&x->stream))) return rc;
-    const int n = x->num;
-    float *d = (float *)malloc(sizeof(float) * (size_t)n * n), *t = (float *)malloc(sizeof(float) * (size_t)n * n);
-    if (!d || !t) { free(d); free(t); return AF_ERR_NOMEM; }
-    af_dct2_matrix(n, n, d);
-    for (int k = 0; k < n; k++) for (int j = 0; j < n; j++) t[(size_t)j * n + k] = d[(size_t)k * n + j];
-    rc = af_dev_upload((void **)&x->dDctT, t, sizeof(float) * (size_t)n * n);
-    free(d); free(t);
-    if (rc) return rc;
-    x->devReady = 1;
-    return AF_OK;
+    return x->dDctT ? AF_OK : af_dct2_upload_transposed(&x->dDctT, x->num);
+}
+
+typedef struct { int num, ccNum, rectifyType, energyType, order; const float *dctT; } XxccCall;
+
+static int xxcc_chunk(void *p, int nb, float *const *d, void *st) {
+    const XxccCall *a = (const XxccCall *)p;
+    return af_launch_xxcc(d[0], nb, a->num, a->ccNum, a->rectifyType, a->dctT, d[1], st);
+}
+
+int af_xxcc_batch(AfPipe *pipe, const float *in, int rows, int num, int ccNum, int rectifyType, const float *dctT,
+                  float *out, int memKind, void *stream) {
+    XxccCall a = {num, ccNum, rectifyType, 0, 0, dctT};
+    const AfPlane pl[2] = {{in, (size_t)num, AF_IN, 0}, {out, (size_t)ccNum, AF_OUT, 0}};
+    return af_run_batch(pipe, memKind, stream, xxcc_chunk, &a, pl, 2, rows, AF_PIPE_CHUNK_BYTES);
 }
 
 int xxccObj_xxccBatch(XXCCObj x, const float *in, int rows, int ccNum, int rectifyType, float *out,
@@ -50,18 +51,7 @@ int xxccObj_xxccBatch(XXCCObj x, const float *in, int rows, int ccNum, int recti
     af_clear_error();
     int rc = xxcc_device(x);
     if (rc) return rc;
-    void *st = stream ? stream : x->stream;
-    if (memKind == AFB200_MEM_DEVICE) {
-        st = stream;                      /* NULL = the CUDA default stream */
-        if ((rc = af_launch_xxcc(in, rows, x->num, ccNum, rectifyType, x->dDctT, out, st))) return rc;
-        return AF_OK;                       /* asynchronous on the caller's stream */
-    }
-    size_t inB = sizeof(float) * (size_t)rows * x->num, outB = sizeof(float) * (size_t)rows * ccNum;
-    if ((rc = af_devbuf_reserve(&x->dIn, inB)) || (rc = af_devbuf_reserve(&x->dOut, outB))) return rc;
-    if ((rc = af_memcpy_h2d(x->dIn.ptr, in, inB, st))) return rc;
-    if ((rc = af_launch_xxcc((const float *)x->dIn.ptr, rows, x->num, ccNum, rectifyType, x->dDctT, (float *)x->dOut.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(out, x->dOut.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    return af_xxcc_batch(&x->pipe, in, rows, x->num, ccNum, rectifyType, x->dDctT, out, memKind, stream);
 }
 
 void xxccObj_xxcc(XXCCObj x, float *mDataArr1, int mLength, CepstralRectifyType *rectifyType, float *mDataArr2) {
@@ -70,6 +60,12 @@ void xxccObj_xxcc(XXCCObj x, float *mDataArr1, int mLength, CepstralRectifyType 
     if (x->timeLength <= 0 || mLength < 1) return;
     xxccObj_xxccBatch(x, mDataArr1, x->timeLength, mLength, rectifyType ? (int)*rectifyType : CepstralRectify_Log,
                       mDataArr2, AFB200_MEM_HOST, NULL);
+}
+
+static int xxcc_standard_chunk(void *p, int nb, float *const *d, void *st) {
+    const XxccCall *a = (const XxccCall *)p;
+    return af_launch_xxcc_standard(d[0], d[1], nb, a->num, a->ccNum, a->rectifyType, a->energyType, a->order, a->dctT,
+                                   d[2], d[3], d[4], st);
 }
 
 /* batched form of xxccObj_xxccStandard (xxcc_algorithm.c:168-296).  in: rows x num, energy: rows (may be NULL
@@ -87,23 +83,11 @@ int xxccObj_xxccStandardBatch(XXCCObj x, const float *in, const float *energy, i
     af_clear_error();
     int rc = xxcc_device(x);
     if (rc) return rc;
-    void *st = stream ? stream : x->stream;
-    const int W = ccNum + (energyType == CepstralEnergy_Append ? 1 : 0);
-    if (memKind == AFB200_MEM_DEVICE)
-        return af_launch_xxcc_standard(in, energy, rows, x->num, ccNum, rectifyType, energyType, order, x->dDctT,
-                                       coe, delta1, delta2, stream);
-    const size_t inB = sizeof(float) * (size_t)rows * x->num, outB = sizeof(float) * (size_t)rows * W;
-    if ((rc = af_devbuf_reserve(&x->dIn, inB)) || (rc = af_devbuf_reserve(&x->dOut, outB)) ||
-        (rc = af_devbuf_reserve(&x->dD1, outB)) || (rc = af_devbuf_reserve(&x->dD2, outB)) ||
-        (rc = af_devbuf_reserve(&x->dEnergy, sizeof(float) * (size_t)(rows > 0 ? rows : 1)))) return rc;
-    if ((rc = af_memcpy_h2d(x->dIn.ptr, in, inB, st))) return rc;
-    if (energy && (rc = af_memcpy_h2d(x->dEnergy.ptr, energy, sizeof(float) * (size_t)rows, st))) return rc;
-    if ((rc = af_launch_xxcc_standard((const float *)x->dIn.ptr, (const float *)x->dEnergy.ptr, rows, x->num, ccNum,
-                                      rectifyType, energyType, order, x->dDctT, (float *)x->dOut.ptr,
-                                      (float *)x->dD1.ptr, (float *)x->dD2.ptr, st))) return rc;
-    if ((rc = af_memcpy_d2h(coe, x->dOut.ptr, outB, st)) || (rc = af_memcpy_d2h(delta1, x->dD1.ptr, outB, st)) ||
-        (rc = af_memcpy_d2h(delta2, x->dD2.ptr, outB, st))) return rc;
-    return af_stream_sync(st);
+    XxccCall a = {x->num, ccNum, rectifyType, energyType, order, x->dDctT};
+    const size_t W = (size_t)ccNum + (energyType == CepstralEnergy_Append ? 1 : 0);
+    const AfPlane pl[5] = {{in, (size_t)x->num, AF_IN, 0}, {energy, 1, AF_IN, 0},
+                           {coe, W, AF_OUT, 0}, {delta1, W, AF_OUT, 0}, {delta2, W, AF_OUT, 0}};
+    return af_run_batch(&x->pipe, memKind, stream, xxcc_standard_chunk, &a, pl, 5, rows, AF_PIPE_CHUNK_BYTES);
 }
 
 void xxccObj_xxccStandard(XXCCObj x, float *mDataArr1, int mLength, float *energyArr, int *deltaWindowLength,
@@ -121,9 +105,7 @@ void xxccObj_xxccStandard(XXCCObj x, float *mDataArr1, int mLength, float *energ
 
 void xxccObj_free(XXCCObj x) {
     if (!x) return;
-    af_devbuf_free(&x->dIn); af_devbuf_free(&x->dOut);
-    af_devbuf_free(&x->dEnergy); af_devbuf_free(&x->dD1); af_devbuf_free(&x->dD2);
+    af_pipe_free(&x->pipe);
     af_dev_free(x->dDctT);
-    af_stream_destroy(x->stream);
     free(x);
 }

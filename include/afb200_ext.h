@@ -4,7 +4,9 @@
  * loops channels in Python); fed that way a GPU is PCIe/launch bound.  These entry points
  * take a whole batch and either host or device pointers.
  *
- *   memKind 0: host pointers (pageable or pinned) -- copies + sync happen inside the call.
+ *   memKind 0: host pointers (pageable or pinned) -- the call stages the batch through the device in
+ *              bounded chunks (about 64 MB, copies overlapping the compute) and returns synchronised;
+ *              it never holds the whole batch on the device.
  *   memKind 1: device pointers on the current device -- asynchronous on `stream`
  *              (a cudaStream_t passed as void*; NULL = the CUDA default stream).  The call
  *              returns without synchronising; results are ordered on that stream.

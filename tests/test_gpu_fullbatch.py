@@ -1,7 +1,7 @@
 """Full-batch parity for BASELINE configs 3 and 4 and for the chunkers (VERDICT r1, item 8): scattered clips of a
 full-size batch -- first, chunk boundary +-1, last -- must equal the single-clip result BIT FOR BIT, and one of them
 the oracle.  Catches clip-offset bugs in the device-side chunk loops (af_cwt.c:cwt_compute, bft_compute) and in the
-host-pointer pipeline (af_ctx.c:af_pipe_run) that one-clip tests cannot see."""
+host-pointer pipeline (af_ctx.c:af_run_batch) that one-clip tests cannot see."""
 import os
 
 import numpy as np
@@ -39,7 +39,7 @@ def test_cqt_config3_full_batch_device(cuda_device):
 
 
 def test_cqt_host_pipeline_chunk_boundaries(cuda_device):
-    """host pointers: af_pipe_run cuts the batch into ~64 MB chunks (66 clips of 5 s); compare around every boundary"""
+    """host pointers: af_run_batch cuts the batch into ~64 MB chunks (66 clips of 5 s); compare around every boundary"""
     af = _af()
     B, L = 200, 240000
     x = (0.1 * np.random.default_rng(5).standard_normal((B, L))).astype(np.float32)

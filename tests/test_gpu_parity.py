@@ -292,7 +292,7 @@ def test_mfcc_host_pointer_pipeline(torch_cuda):
 
 
 def test_host_pointer_pipelines_bft_cqt_stft(torch_cuda):
-    """Every batched host-pointer entry point runs the same chunked 3-stream pipeline (af_pipe_run): several chunks,
+    """Every batched host-pointer entry point runs the same chunked 3-stream pipeline (af_run_batch): several chunks,
     the last one partial, results bit-identical to the device-pointer entry."""
     torch = torch_cuda
     g = torch.Generator().manual_seed(6)

@@ -151,6 +151,7 @@ EXTENSION_API = {
     "xxccObj_xxccBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp]),
     "cqtObj_cqtBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp]),
     "cqtObj_getKernelBank": (C.c_int, [vp, vp, vp]),
+    "cqtObj_octavePlan": (C.c_int, [vp, vp, vp, vp, vp, vp, vp]),
     "cqtObj_chromaBatch": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp]),
     "cqtObj_cqccBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp]),
     "cqtObj_cqhcBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),

@@ -60,6 +60,21 @@ class CQT(BandAxis, FrameAxis, Base):
         check(fn(self._obj, np_ptr(kr), np_ptr(ki)), "cqtObj_getKernelBank")
         return kr, ki
 
+    OCTAVE_KERNELS = ("wgmma", "mma.sync", "fp32 loop", "direct")
+
+    def octave_plan(self):
+        """Additive diagnostics: per octave, top octave first, a dict of the kernel that computes it (a name of
+        OCTAVE_KERNELS), its hop, frames per CTA (0: direct kernel), threads per CTA, tap segments and dynamic shared memory
+        bytes (cqtObj_octavePlan; host only, needs no device)."""
+        fn = self._require_ext("cqtObj_octavePlan")
+        octs = self.num // self.bin_per_octave
+        cols = {k: np.zeros(octs, np.int32) for k in ("kernel", "hop", "frames", "threads", "segs", "smem")}
+        n = fn(self._obj, *(np_ptr(cols[k]) for k in ("kernel", "hop", "frames", "threads", "segs", "smem")))
+        if n != octs:
+            raise RuntimeError(f"cqtObj_octavePlan returned {n} for {octs} octaves")
+        return [dict(kernel=self.OCTAVE_KERNELS[cols["kernel"][k]], **{c: int(cols[c][k]) for c in cols if c != "kernel"})
+                for k in range(octs)]
+
     def cqt_planes(self, data_arr):
         x = as_f32(data_arr)
         T = self.cal_time_length(x.shape[-1])

@@ -223,27 +223,55 @@ int af_launch_mel2(void *plan, const float *data, int dataLength, int batch, int
 
 int af_launch_decimate2(const float *in, int inLength, int inStride, int batch, const float *left32,
                         const float *right31, float *out, int outStride, void *stream);
+
+/* CQT octave plan (host/af_cqt.c): the one function that picks the kernel and tile of an octave, shared by the compute
+ * path and the cqtObj_octavePlan query.  Tile constants the kernels are compiled with (cqt.cu, cqt_wgmma.cu): */
+#define AF_CQT_BINS_PER_PASS 12   /* FP32 loop: bins whose kernels sit in shared memory together */
+#define AF_CQT_FT 4               /* FP32 loop: frames per thread */
+#define AF_CQT_JG 2               /* FP32 loop: thread groups over bins */
+#define AF_CQT_BT 6               /* FP32 loop: bins per thread */
+#define AF_CQT_TC_MT 2            /* mma.sync: 16-frame m-tiles per warp */
+#define AF_CQT_TC_KC 16           /* mma.sync: k-steps (8 taps) of kernel fragments resident in shared memory */
+#define AF_CQT_WG_CHUNK_K 128     /* wgmma: taps per kernel chunk in shared memory */
+#define AF_CQT_WG_MT 2            /* wgmma: 64-frame m-tiles per warpgroup, at most */
+enum { AF_CQT_WGMMA = 0, AF_CQT_TC = 1, AF_CQT_LOOP = 2, AF_CQT_DIRECT = 3 };
+typedef struct {
+    int kernel;           /* AF_CQT_* */
+    int TT;               /* frames per CTA (0: direct kernel) */
+    int threads;          /* threads per CTA */
+    int segs;             /* FP32 loop: tap segments summed through shared memory (else 1) */
+    int smem;             /* dynamic shared-memory bytes */
+    int rowLen;           /* polyphase row pitch in floats (FP32 loop; mma.sync / wgmma with hop >= 8) */
+    int rowsA, nChunk;    /* FP32 loop: ceil(fftLength / hop), kernel taps resident in shared memory at a time */
+    int warps;            /* mma.sync: warps per CTA */
+    int wg, mt;           /* wgmma: warpgroups per CTA, m-tiles per warpgroup */
+} AfCqtOctPlan;
+/* device kernel tables an object of this shape uploads: mma.sync B fragments / wgmma B images */
+int af_cqt_tc_tables(int fftLength, int bpo);
+int af_cqt_wgmma_tables(int fftLength, int bpo);
+/* kernel and tile of one octave with hop `hop`: wgmma where the hop allows it, else mma.sync 3xTF32, else the FP32 loop,
+ * else (no polyphase tile fits) the direct kernel.  Host only. */
+void af_cqt_octave_plan(int fftLength, int hop, int bpo, AfCqtOctPlan *plan);
+
 /* out[b][t][colOff + j] (row stride num) = scale[j] * sum_n xpad[t*hop + n] * kappa[j][n];
- * kappa2 = interleaved (re, im) pairs [bpo][fftLength] */
-int af_launch_cqt_octave(const float *sig, int sigLength, int sigStride, int batch, int validLength,
+ * kappa2 = interleaved (re, im) pairs [bpo][fftLength]; plan: AF_CQT_LOOP or AF_CQT_DIRECT */
+int af_launch_cqt_octave(const AfCqtOctPlan *plan, const float *sig, int sigLength, int sigStride, int batch, int validLength,
                          int fftLength, int hop, int padLeft, int timeLength, int bpo, const float *kappa2,
                          const float *scale, int num, int colOff,
                          float *outRe, float *outIm, void *stream);
 
-/* tensor-core octave kernel (3xTF32 mma.sync): 12 bins per octave, power-of-two hop >= 2 */
-int af_cqt_tc_supported(int fftLength, int hop, int bpo);
+/* tensor-core octave kernel (3xTF32 mma.sync): 12 bins per octave, power-of-two hop >= 2; plan: AF_CQT_TC */
 void af_cqt_tc_fragments(const float *kappa2, int fftLength, float *out /* fftLength/8 * 96 * 4 floats */);
-int af_launch_cqt_octave_tc(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
-                            int padLeft, int timeLength, const float *bfrag, const float *scale, int num, int colOff,
+int af_launch_cqt_octave_tc(const AfCqtOctPlan *plan, const float *sig, int sigStride, int batch, int validLength, int fftLength,
+                            int hop, int padLeft, int timeLength, const float *bfrag, const float *scale, int num, int colOff,
                             float *outRe, float *outIm, void *stream);
 
 /* wgmma octave kernel (kernels/cqt_wgmma.cu): Hankel A fragments from the staged signal, B images in swizzled shared
- * memory; power-of-two hops 2 .. 128 */
-int af_cqt_wgmma_supported(int fftLength, int hop, int bpo);
+ * memory; power-of-two hops 2 .. 128; plan: AF_CQT_WGMMA */
 void af_cqt_wgmma_bimage(const float *kappa2, int fftLength, unsigned char *out /* fftLength/128 * 32768 bytes */);
-int af_launch_cqt_octave_wgmma(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
-                               int padLeft, int timeLength, const unsigned char *bimg, const float *scale, int num, int colOff,
-                               float *outRe, float *outIm, void *stream);
+int af_launch_cqt_octave_wgmma(const AfCqtOctPlan *plan, const float *sig, int sigStride, int batch, int validLength, int fftLength,
+                               int hop, int padLeft, int timeLength, const unsigned char *bimg, const float *scale, int num,
+                               int colOff, float *outRe, float *outIm, void *stream);
 
 typedef struct {
     int log2n, num, batch, padLength, dataLength;

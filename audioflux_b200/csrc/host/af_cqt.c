@@ -97,6 +97,110 @@ int cqtObj_getKernelBank(CQTObj c, float *kr, float *ki) {
     return AF_OK;
 }
 
+/* ---- octave plan: which kernel, which tile (the launchers in kernels/cqt.cu and cqt_wgmma.cu take it as given) ---- */
+int af_cqt_tc_tables(int fftLength, int bpo) { return bpo == 12 && fftLength > 0 && fftLength % 64 == 0; }
+int af_cqt_wgmma_tables(int fftLength, int bpo) { return bpo == 12 && fftLength % AF_CQT_WG_CHUNK_K == 0 && fftLength >= 2 * AF_CQT_WG_CHUNK_K; }
+
+static int is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
+
+/* wgmma: two warpgroups x AF_CQT_WG_MT m-tiles (256 frames) when the CTA fits ~113 KB (two CTAs per SM), else smaller
+ * tiles, then the same shapes up to 227 KB; 0 when not even one 64-frame tile fits */
+static int wgmma_geometry(int fftLength, int hop, AfCqtOctPlan *p) {
+    static const int shapes[][2] = {{2, AF_CQT_WG_MT}, {2, 1}, {1, 1}};
+    const size_t chunkBytes = (size_t)64 * AF_CQT_WG_CHUNK_K * 4;
+    for (int pass = 0; pass < 2; pass++)
+        for (int s = 0; s < 3; s++) {
+            const int wg = shapes[s][0], mt = shapes[s][1], TT = wg * 64 * mt;
+            int rowLen = TT + fftLength / hop + 1;
+            rowLen = ((rowLen + 31) / 32) * 32 + 8;                           /* == 8 (mod 32): conflict-free fragment reads */
+            const size_t sigFloats = hop >= 8 ? (size_t)hop * rowLen : (size_t)(TT - 1) * hop + fftLength;
+            const size_t smem = 2 * chunkBytes + ((sigFloats * 4 + 15) & ~(size_t)15) + 16;
+            if (smem <= (size_t)(pass == 0 ? 113 : 227) * 1024) {
+                p->kernel = AF_CQT_WGMMA; p->wg = wg; p->mt = mt; p->TT = TT; p->threads = wg * 128;
+                p->rowLen = rowLen; p->smem = (int)smem;
+                return 1;
+            }
+        }
+    return 0;
+}
+
+/* mma.sync: 8 warps x AF_CQT_TC_MT m-tiles = 256 frames when the signal tile fits ~100 KB (two CTAs per SM), else fewer
+ * warps (one warp up to 227 KB); 0 when even one warp does not fit */
+static int tc_geometry(int fftLength, int hop, AfCqtOctPlan *p) {
+    const size_t bBytes = (size_t)16 * AF_CQT_TC_KC * 96;                    /* float4 B fragments of AF_CQT_TC_KC k-steps */
+    for (int warps = 8; warps >= 1; warps /= 2) {
+        const int TT = warps * 16 * AF_CQT_TC_MT;
+        int rowLen = TT + fftLength / hop + 1;
+        rowLen = ((rowLen + 31) / 32) * 32 + 8;                               /* == 8 (mod 32): conflict-free fragment reads */
+        const size_t sigFloats = hop >= 8 ? (size_t)hop * rowLen : (size_t)(TT - 1) * hop + fftLength;
+        const size_t smem = bBytes + sizeof(float) * sigFloats;
+        if (smem <= (size_t)100 * 1024 || (warps == 1 && smem <= (size_t)227 * 1024)) {
+            p->kernel = AF_CQT_TC; p->warps = warps; p->TT = TT; p->threads = warps * 32;
+            p->rowLen = rowLen; p->smem = (int)smem;
+            return 1;
+        }
+    }
+    return 0;
+}
+
+/* FP32 loop: frames per CTA -- the largest tile that still lets two CTAs share an SM (<= 100 KB); if that would drop
+ * below 256 frames (large hops: the polyphase signal tile is hop x TT floats) the largest tile that fits 200 KB at all;
+ * 0 when none does */
+static int loop_geometry(int fftLength, int hop, AfCqtOctPlan *p) {
+    static const int ttChoices[] = {512, 256, 128, 64, 32, 16, 8};
+    p->rowsA = (fftLength + hop - 1) / hop;
+    p->nChunk = fftLength < 512 ? fftLength : 512;
+    const size_t kBytes = 2 * sizeof(float) * (size_t)AF_CQT_BINS_PER_PASS * p->nChunk;
+    for (int pass = 0; pass < 2; pass++) {
+        for (int c = 0; c < 7; c++) {
+            const int tt = ttChoices[c];
+            if (pass == 0 && tt < 256) break;
+            int rowLen = tt + p->rowsA + 1;
+            /* pitch chosen so consecutive samples (r fastest) land in different banks while staging */
+            if (hop >= 32) rowLen |= 1; else { int want = 32 / hop; rowLen = ((rowLen + 31) / 32) * 32 + want; }
+            const size_t bytes = kBytes + sizeof(float) * (size_t)hop * rowLen;
+            if (bytes <= (size_t)(pass == 0 ? 100 : 200) * 1024) {
+                p->kernel = AF_CQT_LOOP; p->TT = tt; p->rowLen = rowLen; p->smem = (int)bytes;
+                /* enough threads per CTA: split the taps of a frame over up to rowsA segments until the CTA has >= 512
+                 * threads; the reduction scratch of the segments must fit the kernel buffer */
+                p->segs = 1;
+                while (p->segs * 2 <= p->rowsA && (tt / AF_CQT_FT) * AF_CQT_JG * p->segs * 2 <= 512) p->segs *= 2;
+                if ((size_t)(tt / AF_CQT_FT) * AF_CQT_JG * 2 * AF_CQT_FT * AF_CQT_BT * sizeof(float) > kBytes) p->segs = 1;
+                p->threads = (tt / AF_CQT_FT) * AF_CQT_JG * p->segs;
+                return 1;
+            }
+        }
+    }
+    return 0;
+}
+
+void af_cqt_octave_plan(int fftLength, int hop, int bpo, AfCqtOctPlan *p) {
+    memset(p, 0, sizeof(*p));
+    p->segs = 1;
+    if (af_cqt_wgmma_tables(fftLength, bpo) && hop >= 2 && hop <= 128 && is_pow2(hop) && wgmma_geometry(fftLength, hop, p)) return;
+    if (af_cqt_tc_tables(fftLength, bpo) && hop >= 2 && is_pow2(hop) && tc_geometry(fftLength, hop, p)) return;
+    if (loop_geometry(fftLength, hop, p)) return;
+    /* no tile of the polyphase kernel fits: one warp per (frame, bin) */
+    memset(p, 0, sizeof(*p));
+    p->kernel = AF_CQT_DIRECT; p->threads = 256; p->segs = 1;
+}
+
+int cqtObj_octavePlan(CQTObj c, int *kernel, int *hop, int *framesPerCta, int *threadsPerCta, int *segs, int *smemBytes) {
+    if (!c) { af_fail(AF_ERR_ARG, "cqtObj_octavePlan: bad argument"); return -1; }
+    for (int k = 0; k < c->octaveNum; k++) {
+        const int h = c->slideLength >> k;                                    /* the recursion halves the hop per octave */
+        AfCqtOctPlan p;
+        af_cqt_octave_plan(c->fftLength, h, c->binPerOctave, &p);
+        if (kernel) kernel[k] = p.kernel;
+        if (hop) hop[k] = h;
+        if (framesPerCta) framesPerCta[k] = p.TT;
+        if (threadsPerCta) threadsPerCta[k] = p.threads;
+        if (segs) segs[k] = p.segs;
+        if (smemBytes) smemBytes[k] = p.smem;
+    }
+    return c->octaveNum;
+}
+
 static int cqt_device(CQTObj c) {
     int rc = af_device_ready();
     if (rc) return rc;
@@ -105,7 +209,7 @@ static int cqt_device(CQTObj c) {
         const int sets = c->bank.vqt ? c->octaveNum : 1;
         const size_t setFloats = 2 * (size_t)c->binPerOctave * c->fftLength;
         if ((rc = af_dev_upload((void **)&c->dKappa2, c->kappa2, sizeof(float) * setFloats * sets))) return rc;
-        if (c->binPerOctave == 12 && c->fftLength % 64 == 0) {
+        if (af_cqt_tc_tables(c->fftLength, c->binPerOctave)) {
             const size_t nf = (size_t)(c->fftLength / 8) * 96 * 4;
             float *bf = (float *)malloc(sizeof(float) * nf * sets);
             if (!bf) return AF_ERR_NOMEM;
@@ -114,7 +218,7 @@ static int cqt_device(CQTObj c) {
             free(bf);
             if (rc) return rc;
         }
-        if (c->binPerOctave == 12 && c->fftLength % 128 == 0 && c->fftLength >= 256) {
+        if (af_cqt_wgmma_tables(c->fftLength, c->binPerOctave)) {
             const size_t nb = (size_t)(c->fftLength / 128) * 32768;
             unsigned char *img = (unsigned char *)malloc(nb * sets);
             if (!img) return AF_ERR_NOMEM;
@@ -175,20 +279,20 @@ static int cqt_compute_ex(CQTObj c, const float *dData, int dataLength, int batc
         const unsigned char *bimg = c->dBimg ? c->dBimg + set * (size_t)(c->fftLength / 128) * 32768 : NULL;
         const float *bfrag = c->dBfrag ? c->dBfrag + set * (size_t)(c->fftLength / 8) * 96 * 4 : NULL;
         const float *kappa = c->dKappa2 + set * 2 * (size_t)c->binPerOctave * c->fftLength;
-        /* wgmma where the hop allows it, else mma.sync 3xTF32, else the FP32 loop */
-        if (c->dBimg && af_cqt_wgmma_supported(c->fftLength, hop, c->binPerOctave)) {
-            if ((rc = af_launch_cqt_octave_wgmma(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bimg,
-                                                c->dScale + (size_t)k * c->binPerOctave, c->num, o * c->binPerOctave, dRe, dIm, st))) return rc;
-            continue;
-        }
-        if (c->dBfrag && af_cqt_tc_supported(c->fftLength, hop, c->binPerOctave)) {
-            if ((rc = af_launch_cqt_octave_tc(sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bfrag,
-                                              c->dScale + (size_t)k * c->binPerOctave, c->num, o * c->binPerOctave, dRe, dIm, st))) return rc;
-            continue;
-        }
-        if ((rc = af_launch_cqt_octave(sig, len, stride, batch, valid, c->fftLength, hop, padLeft, T, c->binPerOctave,
-                                       kappa, c->dScale + (size_t)k * c->binPerOctave, c->num,
-                                       o * c->binPerOctave, dRe, dIm, st))) return rc;
+        /* wgmma where the hop allows it, else mma.sync 3xTF32, else the FP32 loop (cqtObj_octavePlan reports the same) */
+        AfCqtOctPlan plan;
+        af_cqt_octave_plan(c->fftLength, hop, c->binPerOctave, &plan);
+        const float *scale = c->dScale + (size_t)k * c->binPerOctave;
+        if (plan.kernel == AF_CQT_WGMMA)
+            rc = af_launch_cqt_octave_wgmma(&plan, sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bimg, scale, c->num,
+                                            o * c->binPerOctave, dRe, dIm, st);
+        else if (plan.kernel == AF_CQT_TC)
+            rc = af_launch_cqt_octave_tc(&plan, sig, stride, batch, valid, c->fftLength, hop, padLeft, T, bfrag, scale, c->num,
+                                         o * c->binPerOctave, dRe, dIm, st);
+        else
+            rc = af_launch_cqt_octave(&plan, sig, len, stride, batch, valid, c->fftLength, hop, padLeft, T, c->binPerOctave,
+                                      kappa, scale, c->num, o * c->binPerOctave, dRe, dIm, st);
+        if (rc) return rc;
     }
     return AF_OK;
 }

@@ -120,10 +120,12 @@ struct OctParams {
                                   // memory, so the taps of one frame are split to get enough threads), summed at the end
 };
 
-constexpr int kBinsPerPass = 12;  // bins whose kernels sit in shared memory together
-constexpr int kFT = 4;            // frames per thread
-constexpr int kJG = 2;            // thread groups over bins
-constexpr int kBT = 6;            // bins per thread: 4 x 6 complex accumulators, 10 shared loads per 48 FMAs
+// (the tile planner in host/af_cqt.c sizes tiles from the same constants)
+constexpr int kBinsPerPass = AF_CQT_BINS_PER_PASS;  // bins whose kernels sit in shared memory together
+constexpr int kFT = AF_CQT_FT;                      // frames per thread
+constexpr int kJG = AF_CQT_JG;                      // thread groups over bins
+constexpr int kBT = AF_CQT_BT;                      // bins per thread: 4 x 6 complex accumulators, 10 shared loads per 48 FMAs
+static_assert(kJG * kBT == kBinsPerPass, "the bin groups cover one pass");
 
 __global__ void k_cqt_octave(OctParams p) {
     extern __shared__ __align__(16) unsigned char smemRaw[];
@@ -293,8 +295,8 @@ __global__ void __launch_bounds__(256) k_cqt_octave_direct(OctParams p) {
 //     addresses for hop 2: broadcast);
 //   * warp w owns kTcMT m-tiles (16 frames each); per k-step it reads 3 LDS.128 of B fragments (shared by its m-tiles)
 //     and, per m-tile, 4 LDS.32 + 8 ALU (split) + 9 HMMA: ~140 MAC per issued instruction (FP32 loop: ~26).
-constexpr int kTcMT = 2;                          // m-tiles (16 frames) per warp
-constexpr int kTcKC = 16;                         // k-steps (8 taps) of kernel fragments resident in shared memory at a time
+constexpr int kTcMT = AF_CQT_TC_MT;               // m-tiles (16 frames) per warp
+constexpr int kTcKC = AF_CQT_TC_KC;               // k-steps (8 taps) of kernel fragments resident in shared memory at a time
 
 struct OctTcParams {
     const float *sig; long long sigStride; int validLength;
@@ -426,55 +428,35 @@ extern "C" int af_launch_decimate2(const float *in, int inLength, int inStride, 
     return AF_OK;
 }
 
-extern "C" int af_launch_cqt_octave(const float *sig, int sigLength, int sigStride, int batch, int validLength,
-                                    int fftLength, int hop, int padLeft, int timeLength, int bpo, const float *kappa2,
-                                    const float *scale, int num, int colOff,
+// tile geometry from af_cqt_octave_plan (host/af_cqt.c): frames per CTA, row pitch, tap segments, shared memory
+extern "C" int af_launch_cqt_octave(const AfCqtOctPlan *plan, const float *sig, int sigLength, int sigStride, int batch,
+                                    int validLength, int fftLength, int hop, int padLeft, int timeLength, int bpo,
+                                    const float *kappa2, const float *scale, int num, int colOff,
                                     float *outRe, float *outIm, void *stream) {
     if (batch <= 0 || timeLength <= 0) return AF_OK;
     if (hop < 1) return af_fail(AF_ERR_ARG, "cqt octave: hop < 1");
+    if (plan->kernel != AF_CQT_LOOP && plan->kernel != AF_CQT_DIRECT)
+        return af_fail(AF_ERR_ARG, "cqt octave: plan of kernel %d given to the FP32 launcher", plan->kernel);
     if (batch > 65535) return af_fail(AF_ERR_ARG, "cqt octave: batch %d > 65535 per launch", batch);
     OctParams p;
     p.sig = sig; p.sigStride = sigStride; p.sigLength = sigLength; p.validLength = validLength;
     p.N = fftLength; p.hop = hop; p.T = timeLength; p.bpo = bpo; p.padLeft = padLeft;
     p.kappa = reinterpret_cast<const float2 *>(kappa2); p.scale = scale;
     p.outRe = outRe; p.outIm = outIm; p.outStride = (long long)timeLength * num; p.num = num; p.colOff = colOff;
-    p.rowsA = (fftLength + hop - 1) / hop;
-    p.nChunk = fftLength < 512 ? fftLength : 512;
-    const size_t kBytes = sizeof(float2) * (size_t)kBinsPerPass * p.nChunk;
-    // frames per CTA: the largest tile that still lets two CTAs share an SM (<= 100 KB); if that would drop below
-    // 256 frames (large hops: the polyphase signal tile is hop x TT floats) take the largest tile that fits at all
-    static const int ttChoices[] = {512, 256, 128, 64, 32, 16, 8};
-    int TT = 0;
-    size_t smem = 0;
-    for (int pass = 0; pass < 2 && TT == 0; pass++) {
-        for (int c = 0; c < 7; c++) {
-            const int tt = ttChoices[c];
-            if (pass == 0 && tt < 256) break;
-            int rowLen = tt + p.rowsA + 1;
-            // pitch chosen so consecutive samples (r fastest) land in different banks while staging
-            if (hop >= 32) rowLen |= 1; else { int want = 32 / hop; rowLen = ((rowLen + 31) / 32) * 32 + want; }
-            const size_t bytes = kBytes + sizeof(float) * (size_t)hop * rowLen;
-            if (bytes <= (size_t)(pass == 0 ? 100 : 200) * 1024) { TT = tt; p.rowLen = rowLen; smem = bytes; break; }
-        }
-    }
-    if (TT == 0) {
+    p.rowsA = plan->rowsA; p.nChunk = plan->nChunk;
+    p.TT = plan->TT; p.rowLen = plan->rowLen; p.segs = plan->segs;
+    if (plan->kernel == AF_CQT_DIRECT) {
         // no tile of the polyphase kernel fits (hop x (8 + fftLength / hop) floats > 150 KB): warp-per-output kernel
-        p.TT = 0; p.rowLen = 0; p.segs = 1;
         const long long outs = (long long)timeLength * bpo;
         const dim3 g((unsigned)((outs + 7) / 8), (unsigned)batch);
-        k_cqt_octave_direct<<<g, 256, 0, (cudaStream_t)stream>>>(p);
+        k_cqt_octave_direct<<<g, plan->threads, 0, (cudaStream_t)stream>>>(p);
         AF_LAUNCH_CHECK("k_cqt_octave_direct");
         return AF_OK;
     }
-    p.TT = TT;
-    // enough threads per CTA: split the taps of a frame over up to rowsA segments until the CTA has >= 512 threads
-    p.segs = 1;
-    while (p.segs * 2 <= p.rowsA && (TT / kFT) * kJG * p.segs * 2 <= 512) p.segs *= 2;
-    if ((size_t)(TT / kFT) * kJG * 2 * kFT * kBT * sizeof(float) > kBytes) p.segs = 1;   // reduction scratch must fit the kernel buffer
-    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
     if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave)");
-    dim3 grid((unsigned)((timeLength + TT - 1) / TT), (unsigned)batch);
-    k_cqt_octave<<<grid, (TT / kFT) * kJG * p.segs, smem, (cudaStream_t)stream>>>(p);
+    dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
+    k_cqt_octave<<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK("k_cqt_octave");
     return AF_OK;
 }
@@ -501,35 +483,14 @@ extern "C" void af_cqt_tc_fragments(const float *kappa2 /* [12][N] (re, im) */, 
             }
 }
 
-// tile geometry of the tensor-core kernel: 8 warps x 2 m-tiles = 256 frames when the signal tile fits ~100 KB (two CTAs
-// per SM), else fewer warps; returns the dynamic shared-memory bytes, 0 when even one warp does not fit
-static size_t cqt_tc_geometry(int fftLength, int hop, int *warpsOut, int *ttOut, int *rowLenOut) {
-    const size_t bBytes = sizeof(float4) * kTcKC * 96;
-    for (int warps = 8; warps >= 1; warps /= 2) {
-        const int TT = warps * 16 * kTcMT;
-        int rowLen = TT + fftLength / hop + 1;
-        rowLen = ((rowLen + 31) / 32) * 32 + 8;                      // == 8 (mod 32): conflict-free fragment reads
-        const size_t sigFloats = hop >= 8 ? (size_t)hop * rowLen : (size_t)(TT - 1) * hop + fftLength;
-        const size_t smem = bBytes + sizeof(float) * sigFloats;
-        if (smem <= (size_t)100 * 1024 || (warps == 1 && smem <= (size_t)227 * 1024)) {
-            *warpsOut = warps; *ttOut = TT; *rowLenOut = rowLen;
-            return smem;
-        }
-    }
-    return 0;
-}
-
-extern "C" int af_cqt_tc_supported(int fftLength, int hop, int bpo) {
-    int w, tt, rl;
-    return bpo == 12 && fftLength >= 64 && fftLength % 64 == 0 && hop >= 2 && (hop & (hop - 1)) == 0 &&
-           cqt_tc_geometry(fftLength, hop, &w, &tt, &rl) > 0;
-}
-
-extern "C" int af_launch_cqt_octave_tc(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
-                                       int padLeft, int timeLength, const float *bfrag, const float *scale, int num, int colOff,
-                                       float *outRe, float *outIm, void *stream) {
+// tile geometry from af_cqt_octave_plan (host/af_cqt.c): 8 warps x 2 m-tiles = 256 frames when the signal tile fits
+// ~100 KB (two CTAs per SM), else fewer warps
+extern "C" int af_launch_cqt_octave_tc(const AfCqtOctPlan *plan, const float *sig, int sigStride, int batch, int validLength,
+                                       int fftLength, int hop, int padLeft, int timeLength, const float *bfrag, const float *scale,
+                                       int num, int colOff, float *outRe, float *outIm, void *stream) {
     if (batch <= 0 || timeLength <= 0) return AF_OK;
-    if (!af_cqt_tc_supported(fftLength, hop, 12)) return af_fail(AF_ERR_UNSUPPORTED, "cqt octave (tensor core): fftLength %d hop %d", fftLength, hop);
+    if (plan->kernel != AF_CQT_TC || !bfrag)
+        return af_fail(AF_ERR_UNSUPPORTED, "cqt octave (tensor core): fftLength %d hop %d", fftLength, hop);
     if (batch > 65535) return af_fail(AF_ERR_ARG, "cqt octave: batch %d > 65535 per launch", batch);
     OctTcParams p;
     p.sig = sig; p.sigStride = sigStride; p.validLength = validLength;
@@ -537,11 +498,11 @@ extern "C" int af_launch_cqt_octave_tc(const float *sig, int sigStride, int batc
     p.hs = 0; while ((1 << p.hs) < hop) p.hs++;
     p.bfrag = reinterpret_cast<const float4 *>(bfrag); p.scale = scale;
     p.outRe = outRe; p.outIm = outIm; p.outStride = (long long)timeLength * num; p.num = num; p.colOff = colOff;
-    const size_t smem = cqt_tc_geometry(fftLength, hop, &p.warps, &p.TT, &p.rowLen);
-    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    p.warps = plan->warps; p.TT = plan->TT; p.rowLen = plan->rowLen;
+    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
     if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_tc)");
     dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
-    k_cqt_octave_tc<<<grid, p.warps * 32, smem, (cudaStream_t)stream>>>(p);
+    k_cqt_octave_tc<<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK("k_cqt_octave_tc");
     return AF_OK;
 }

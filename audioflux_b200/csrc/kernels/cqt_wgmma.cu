@@ -17,9 +17,9 @@
 
 namespace {
 
-constexpr int kWgChunkK = 128;                           // taps per kernel chunk in shared memory
+constexpr int kWgChunkK = AF_CQT_WG_CHUNK_K;             // taps per kernel chunk in shared memory
 constexpr int kWgChunkBytes = 64 * kWgChunkK * 4;        // one chunk image: 64 rows (32 hi + 32 lo) x 128 taps = 32 KB
-constexpr int kWgMT = 2;                                 // 64-frame m-tiles per warpgroup
+constexpr int kWgMT = AF_CQT_WG_MT;                      // 64-frame m-tiles per warpgroup
 
 struct WgParams {
     const float *sig; long long sigStride; int validLength;
@@ -216,37 +216,14 @@ extern "C" void af_cqt_wgmma_bimage(const float *kappa2 /* [12][N] (re, im) */, 
             }
 }
 
-// tile geometry: two warpgroups x kWgMT m-tiles (256 frames) when the CTA fits ~113 KB (two CTAs per SM), else smaller
-// tiles; returns the dynamic shared-memory bytes (0: not even one 64-frame tile fits) and the warpgroups / m-tiles
-static size_t cqt_wgmma_geometry(int fftLength, int hop, int *wgOut, int *mtOut, int *rowLenOut) {
-    static const int shapes[][2] = {{2, kWgMT}, {2, 1}, {1, 1}};
-    for (int pass = 0; pass < 2; pass++)
-        for (int s = 0; s < 3; s++) {
-            const int wg = shapes[s][0], mt = shapes[s][1], TT = wg * 64 * mt;
-            int rowLen = TT + fftLength / hop + 1;
-            rowLen = ((rowLen + 31) / 32) * 32 + 8;                           // == 8 (mod 32): conflict-free fragment reads
-            const size_t sigFloats = hop >= 8 ? (size_t)hop * rowLen : (size_t)(TT - 1) * hop + fftLength;
-            const size_t smem = 2 * (size_t)kWgChunkBytes + ((sigFloats * 4 + 15) & ~(size_t)15) + 16;
-            if (smem <= (size_t)(pass == 0 ? 113 : 227) * 1024) {
-                *wgOut = wg; *mtOut = mt; *rowLenOut = rowLen;
-                return smem;
-            }
-        }
-    return 0;
-}
-
-extern "C" int af_cqt_wgmma_supported(int fftLength, int hop, int bpo) {
-    if (bpo != 12 || fftLength % kWgChunkK != 0 || fftLength < 2 * kWgChunkK) return 0;
-    if (hop < 2 || hop > 128 || (hop & (hop - 1)) != 0) return 0;
-    int wg, mt, rl;
-    return cqt_wgmma_geometry(fftLength, hop, &wg, &mt, &rl) > 0;
-}
-
-extern "C" int af_launch_cqt_octave_wgmma(const float *sig, int sigStride, int batch, int validLength, int fftLength, int hop,
-                                          int padLeft, int timeLength, const unsigned char *bimg, const float *scale, int num, int colOff,
-                                          float *outRe, float *outIm, void *stream) {
+// tile geometry from af_cqt_octave_plan (host/af_cqt.c): two warpgroups x kWgMT m-tiles (256 frames) when the CTA fits
+// ~113 KB (two CTAs per SM), else smaller tiles
+extern "C" int af_launch_cqt_octave_wgmma(const AfCqtOctPlan *plan, const float *sig, int sigStride, int batch, int validLength,
+                                          int fftLength, int hop, int padLeft, int timeLength, const unsigned char *bimg,
+                                          const float *scale, int num, int colOff, float *outRe, float *outIm, void *stream) {
     if (batch <= 0 || timeLength <= 0) return AF_OK;
-    if (!af_cqt_wgmma_supported(fftLength, hop, 12)) return af_fail(AF_ERR_UNSUPPORTED, "cqt octave (wgmma): fftLength %d hop %d", fftLength, hop);
+    if (plan->kernel != AF_CQT_WGMMA || !bimg)
+        return af_fail(AF_ERR_UNSUPPORTED, "cqt octave (wgmma): fftLength %d hop %d", fftLength, hop);
     if (batch > 65535) return af_fail(AF_ERR_ARG, "cqt octave: batch %d > 65535 per launch", batch);
     WgParams p;
     p.sig = sig; p.sigStride = sigStride; p.validLength = validLength;
@@ -254,19 +231,18 @@ extern "C" int af_launch_cqt_octave_wgmma(const float *sig, int sigStride, int b
     p.hs = 0; while ((1 << p.hs) < hop) p.hs++;
     p.bimg = bimg; p.scale = scale;
     p.outRe = outRe; p.outIm = outIm; p.outStride = (long long)timeLength * num; p.num = num; p.colOff = colOff;
-    int wg, mt;
-    const size_t smem = cqt_wgmma_geometry(fftLength, hop, &wg, &mt, &p.rowLen);
-    p.TT = wg * 64 * mt;
+    p.rowLen = plan->rowLen;
+    p.TT = plan->TT;
     const dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
     cudaError_t e;
-    if (mt == kWgMT) {
-        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<kWgMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (plan->mt == kWgMT) {
+        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<kWgMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
         if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_wgmma)");
-        k_cqt_octave_wgmma<kWgMT><<<grid, wg * 128, smem, (cudaStream_t)stream>>>(p);
+        k_cqt_octave_wgmma<kWgMT><<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     } else {
-        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
         if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_wgmma)");
-        k_cqt_octave_wgmma<1><<<grid, wg * 128, smem, (cudaStream_t)stream>>>(p);
+        k_cqt_octave_wgmma<1><<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     }
     AF_LAUNCH_CHECK("k_cqt_octave_wgmma");
     return AF_OK;

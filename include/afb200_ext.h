@@ -98,6 +98,11 @@ int cqtObj_chromaBatch(CQTObj cqtObj, const float *mReal, const float *mImag, in
 int cqtObj_cqccBatch(CQTObj cqtObj, const float *in, int rows, int ccNum, int rectifyType, float *out,
                      int memKind, void *stream);
 int cqtObj_getKernelBank(CQTObj cqtObj, float *kr, float *ki /* binPerOctave x (fftLength/2+1) host */);
+/* diagnostics: per octave, top octave first -- kernel (0 wgmma, 1 mma.sync, 2 FP32 loop, 3 direct), the octave's hop,
+   frames per CTA (0 for direct), threads per CTA, tap segments (FP32 loop; else 1), dynamic shared memory bytes.
+   Each array holds octaveNum ints; any may be NULL.  Returns octaveNum, or < 0 on error.  Host only: needs no device. */
+int cqtObj_octavePlan(CQTObj cqtObj, int *kernel, int *hop, int *framesPerCta, int *threadsPerCta, int *segs,
+                      int *smemBytes);
 /* data: batch x 2^radix2Exp; out planes: batch x num x 2^radix2Exp */
 int cwtObj_cwtBatch(CWTObj cwtObj, const float *data, int batch, float *mReal4, float *mImag4,
                     int memKind, void *stream);

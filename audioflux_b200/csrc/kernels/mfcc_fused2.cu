@@ -49,13 +49,15 @@ constexpr int kMaxPieces = 256;     // pieces the intervals may be cut into (slo
 constexpr int kMaxPass = kMaxPieces / (kEW * 32);   // bank passes: one piece per helper lane and pass
 constexpr int kSpecPitch = 17;      // c64 slots per n2 row of the special-column buffer (odd -> conflict-free both ways)
 constexpr int kScratchFloats = 33 * 32;
+constexpr int kTrPitch = 34;        // transpose rows (floats): 34 % 32 == 2 -> 16 lanes' float2 reads hit 16 bank pairs
+static_assert(31 * kTrPitch <= kScratchFloats, "31 transpose rows fit the frame warp's scratch");
 constexpr int kPitchPairs = kFW | 1;   // power-tile row pitch (frames): odd -> conflict-free column walks; always kFW wide
 constexpr int kBarBytes = 128;      // 12 mbarriers at the start of shared memory (128 keeps the TMA span aligned)
-constexpr int kTwRows = 31;         // stage-C twiddles W_2048^(lane k1), k1 = 1..31: one complex product per column
+constexpr int kTwRows = 31;         // stage-D twiddles W_2048^(n2 k1) = g (1 - i t), n2 = 1..31 (row n2 - 1), lane k1
 
 struct Plan {
     float2 *dWinPairs;              // [32 m][32 lane]  0.5 * (w[64 m + lane], w[64 m + 32 + lane])
-    float2 *dTw;                    // [kTwRows][32]  W_2048^(lane * k1), k1 = 1..31 (row k1 - 1)
+    float2 *dTw;                    // [kTwRows][32 k1]  (g, t) of W_2048^(n2 k1) = g (1 - i t), n2 = 1..31 (row n2 - 1)
     float *dDct;                    // [128 m][dctPitch]
     int num, ccNum, ct, dataType;
     unsigned ivDesc[kMaxNum + 4];   // (first bin pair << 16) | table offset; entries num+1.. = end sentinels
@@ -204,7 +206,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 float a, b;
                 c_unpack(sp[n2 * kSpecPitch], a, b);
                 const float v = kind ? b : a;
-                u[n2] = kind ? af_mul_w64(c_pack(v, 0.0f), n2 & 15) : c_pack(v, 0.0f);
+                u[n2] = kind ? af_mul_w64_real(v, n2 & 15) : c_pack(v, 0.0f);
                 if (n2 >= 16 && kind) u[n2] = c_mul_mi(u[n2]);                        // W_64^16 = -i
             }
             af_fft32_fma(u);
@@ -464,11 +466,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
 
         c64 z[32];
         if (active) {
-            // ---- A: x[32 n1 + lane], n1 = 0..63, times 0.5 w; packed z[m] = (s[2m], s[2m+1]) ----
+            // ---- A: x[32 n1 + lane], n1 = 0..63; packed z[m] = (s[2m], s[2m+1]) (0.5 w is applied in B) ----
             const float *sp = span + (size_t)stage * p.spanFloats + warp * p.hop + lane;
 #pragma unroll
-            for (int m = 0; m < 32; m++)
-                z[m] = v_mul(c_pack(sp[64 * m], sp[64 * m + 32]), sWinC[m * 32 + lane]);
+            for (int m = 0; m < 32; m++) z[m] = c_pack(sp[64 * m], sp[64 * m + 32]);
         }
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&emptyBar[stage]);           // span slot may be refilled
@@ -481,37 +482,43 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             continue;
         }
 
-        // ---- B: 64-point real DFT of the lane's column: packed complex 32-point DFT + in-lane post-pass ----
-        af_fft32_fma(z);                                           // Z[k] at AF_BR5(k)
+        // ---- B: 64-point real DFT of the windowed column: packed complex 32-point DFT + in-lane post-pass ----
+        af_fft32_fma_win(z, sWinC + lane);                         // Z[k] at AF_BR5(k)
         // R[k] = (Z[k] + conj Z[32-k]) - i W_64^k (Z[k] - conj Z[32-k]) at AF_BR5(k), (R[0], R[32]) in z[0]
         af_rfft64_post_fma(z);
         sSpec[((size_t)sb * 32 + lane) * kSpecPitch + warp] = z[0];
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&specFull[sb]);
 
-        // ---- C: columns k1 = 1..31 times W_2048^(lane k1), 32 x 32 transpose (real plane, then imaginary plane) ----
+        // ---- C: columns k1 = 1..31, 32 x 32 transpose (real plane, then imaginary plane).  Row k1 - 1 of a plane holds
+        // column k1 at pitch kTrPitch: the writers' 32-bit stores are one wavefront, and lane k1 reads its row as 16
+        // float2 (n2, n2 + 1) -- rows 2 apart in banks, so each half-warp's 64-bit loads are one wavefront.  Lane 0 has no
+        // column; it reads row 0 with lane 1 (same addresses) and its spectrum is never stored. ----
         {
             float yr[32], yi[32];
+            const float2 *row = reinterpret_cast<const float2 *>(scratch + (lane ? lane - 1 : 0) * kTrPitch);
 #pragma unroll
-            for (int k1 = 1; k1 < 32; k1++) {
-                const c64 y = c_mul_fma(z[AF_BR5(k1)], sTwC[(k1 - 1) * 32 + lane]);
-                c_unpack(y, yr[k1], yi[k1]);
+            for (int k1 = 1; k1 < 32; k1++) c_unpack(z[AF_BR5(k1)], yr[k1], yi[k1]);
+#pragma unroll
+            for (int k1 = 1; k1 < 32; k1++) scratch[(k1 - 1) * kTrPitch + lane] = yr[k1];
+            __syncwarp();
+#pragma unroll
+            for (int j = 0; j < 16; j++) { const float2 v = row[j]; yr[2 * j] = v.x; yr[2 * j + 1] = v.y; }
+            __syncwarp();
+#pragma unroll
+            for (int k1 = 1; k1 < 32; k1++) scratch[(k1 - 1) * kTrPitch + lane] = yi[k1];
+            __syncwarp();
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const float2 v = row[j];
+                z[2 * j] = c_pack(yr[2 * j], v.x);
+                z[2 * j + 1] = c_pack(yr[2 * j + 1], v.y);
             }
-#pragma unroll
-            for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yr[k1];
-            __syncwarp();
-#pragma unroll
-            for (int n2 = 0; n2 < 32; n2++) yr[n2] = scratch[lane * 33 + n2];
-            __syncwarp();
-#pragma unroll
-            for (int k1 = 1; k1 < 32; k1++) scratch[k1 * 33 + lane] = yi[k1];
-            __syncwarp();
-#pragma unroll
-            for (int n2 = 0; n2 < 32; n2++) z[n2] = c_pack(yr[n2], scratch[lane * 33 + n2]);
             __syncwarp();
         }
-        // ---- D: 32-point DFT over n2 in lane k1: bins k1 + 64 k2 and, mirrored, 64 (32 - k2) - k1 ----
-        af_fft32_fma(z);
+        // ---- D: 32-point DFT over n2 of the column times W_2048^(n2 k1), in lane k1: bins k1 + 64 k2 and, mirrored,
+        // 64 (32 - k2) - k1.  The twiddle is applied as (1 - i t) and a gain g inside the first butterflies. ----
+        af_fft32_fma_tw(z, sTwC + lane);
         af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);      // bank done with the previous tile's spectra
         if (lane) {
             if (p.dataType == SpectralData_Mag) {                  // (uniform branch: no sqrt sequence in the power path)
@@ -707,10 +714,12 @@ extern "C" int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int c
     for (int m = 0; m < 32; m++)
         for (int l = 0; l < 32; l++) wp[m * 32 + l] = make_float2(0.5f * window[64 * m + l], 0.5f * window[64 * m + 32 + l]);
     rc = af_dev_upload(reinterpret_cast<void **>(&pl->dWinPairs), wp, sizeof(float2) * 1024);
-    for (int k1 = 1; k1 <= kTwRows; k1++)
-        for (int l = 0; l < 32; l++) {
-            const double a = -2.0 * M_PI * (double)(k1 * l) / 2048.0;
-            wp[(k1 - 1) * 32 + l] = make_float2((float)cos(a), (float)sin(a));
+    // g = cos, t = tan for every entry (u = 1): the factor u in {1, -i} that would keep |t| <= 1 differs between the
+    // lanes of one instruction.  n2 k1 <= 961 never hits 512 (cos = 0); |t| <= 326, and g (x + t y) still rounds as c x + s y.
+    for (int n2 = 1; n2 <= kTwRows; n2++)
+        for (int k1 = 0; k1 < 32; k1++) {
+            const double a = 2.0 * M_PI * (double)(n2 * k1) / 2048.0;
+            wp[(n2 - 1) * 32 + k1] = make_float2((float)cos(a), (float)tan(a));
         }
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dTw), wp, sizeof(float2) * kTwRows * 32);
     free(wp);

@@ -238,6 +238,22 @@ NSGT_API = {
     "nsgtObj_nsgtBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, vp]),
 }
 
+# Stockwell transforms (src/st_algorithm.h:17-24, src/fst_algorithm.h:16-20, include/afb200_st.h) and the additive
+# entry points (include/afb200_ext.h)
+ST_API = {
+    "stObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, C.c_int, c_float_p, c_float_p]),
+    "stObj_useBinArr": (None, [vp, vp, C.c_int]),
+    "stObj_setValue": (None, [vp, C.c_float, C.c_float]),
+    "stObj_st": (None, [vp, vp, vp, vp]),
+    "stObj_free": (None, [vp]),
+    "fstObj_new": (C.c_int, [P(vp), C.c_int]),
+    "fstObj_fst": (None, [vp, vp, C.c_int, C.c_int, vp, vp]),
+    "fstObj_free": (None, [vp]),
+    "stObj_stBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_int, vp]),
+    "stObj_getBinLength": (C.c_int, [vp]),
+    "fstObj_fstBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -251,7 +267,7 @@ REFERENCE_BUILDERS = {
 }
 
 
-def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, REFERENCE_BUILDERS)) -> dict:
+def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -380,6 +380,19 @@ typedef struct {
 } AfNsgtArgs;
 int af_launch_nsgt(const AfNsgtArgs *a, void *stream);
 
+/* Stockwell transforms (kernels/st.cu), N = 2^log2n <= AF_ST_MAX_N.
+ * ST: spec = FULL spectrum planes batch x N (af_launch_stft); per row r of `bins`, out[clip][r] = IFFT_N(X[(m + bin) mod N]
+ * * (expf(v m^2) + expf(v (m-N)^2))), v = vArr[r]; bin 0 gives the clip's mean and an imaginary row of 0.
+ * FST: spec = HALF spectrum planes batch x (N/2+1); part = scratch batch x (N/2+1) complex (the right half of the dyadic
+ * partition, from position N/2-1); out row k (frequency minIndex+k) column l = part[(seg[f] >> 5) + (l >> (log2n - (seg[f] & 31)))]
+ * with seg[f] = (offset << 5) | log2 of the segment length, f = minIndex + k. */
+#define AF_ST_MAX_EXP 14
+#define AF_ST_MAX_N (1 << AF_ST_MAX_EXP)
+int af_launch_st(const float *data, const float *specRe, const float *specIm, const int *bins, const float *vArr, int rows,
+                 int log2n, int batch, float *outRe, float *outIm, void *stream);
+int af_launch_fst(const float *specRe, const float *specIm, float *part, const int *seg, int minIndex, int rows, int log2n,
+                  int batch, float *outRe, float *outIm, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

@@ -42,9 +42,9 @@ __global__ void k_istft_frames(const float *__restrict__ re, const float *__rest
     }
 }
 
-// same transform for frames whose ping-pong buffers do not fit shared memory (fftLength 16384: 2 x 128 KB): in-place
-// radix-2 decimation-in-frequency passes over ONE buffer, result in bit-reversed order, undone while the frame is
-// written out.  Only this size takes the path; the Stockham kernel above is 2-3x faster where it fits.
+// same transform for frames whose ping-pong buffers do not fit shared memory (fftLength 16384: 2 x 128 KB): the in-place
+// passes of af_fft_inplace_dif over ONE buffer, result in bit-reversed order, undone while the frame is written out.
+// Only this size takes the path; the Stockham kernel above is 2-3x faster where it fits.
 __global__ void k_istft_frames_inplace(const float *__restrict__ re, const float *__restrict__ im, int width, int n, int log2n,
                                        const float *__restrict__ window, int weightMode, float *__restrict__ frames,
                                        const float2 *__restrict__ tw) {
@@ -59,17 +59,7 @@ __global__ void k_istft_frames_inplace(const float *__restrict__ re, const float
         a[k] = make_float2(xr, -xi);
     }
     __syncthreads();
-    for (int half = n >> 1, shift = 0; half >= 1; half >>= 1, shift++) {
-        for (int i = threadIdx.x; i < (n >> 1); i += blockDim.x) {
-            const int k = i & (half - 1), base = ((i - k) << 1) + k;
-            const float2 u = a[base], v = a[base + half];
-            a[base] = make_float2(u.x + v.x, u.y + v.y);
-            float2 d = make_float2(u.x - v.x, u.y - v.y);
-            if (k) d = af_cmul(d, af_tw(tw, k, shift, 2 * half));               // exp(-2 pi i k / (2 half)) = tw[k << shift]
-            a[base + half] = d;
-        }
-        __syncthreads();
-    }
+    af_fft_inplace_dif(a, n, tw);
     const float inv = 1.0f / (float)n;
     float *f = frames + row * n;
     for (int j = threadIdx.x; j < n; j += blockDim.x) {

@@ -59,6 +59,23 @@ __device__ __forceinline__ float2 *af_stockham(float2 *a, float2 *b, int nc, int
     return a;
 }
 
+// same forward transform over ONE buffer, for sizes whose two Stockham buffers do not fit shared memory (16384 points:
+// 2 x 128 KB): in-place radix-2 decimation-in-frequency passes.  The result is in bit-reversed order: element j of the
+// transform is a[__brev(j) >> (32 - log2nc)].  All threads of the block must call it.
+__device__ __forceinline__ void af_fft_inplace_dif(float2 *a, int nc, const float2 *tw = nullptr) {
+    for (int half = nc >> 1, shift = 0; half >= 1; half >>= 1, shift++) {
+        for (int i = threadIdx.x; i < (nc >> 1); i += blockDim.x) {
+            const int k = i & (half - 1), base = ((i - k) << 1) + k;
+            const float2 u = a[base], v = a[base + half];
+            a[base] = make_float2(u.x + v.x, u.y + v.y);
+            float2 d = make_float2(u.x - v.x, u.y - v.y);
+            if (k) d = af_cmul(d, af_tw(tw, k, shift, 2 * half));               // exp(-2 pi i k / (2 half)) = tw[k << shift]
+            a[base + half] = d;
+        }
+        __syncthreads();
+    }
+}
+
 // host side: cached device tables per (device, log2 n): [0, n) exp(-2 pi i j / n) and, behind it, [0, n] exp(-2 pi i j / (2n))
 // (the real-FFT post-pass twiddles of a 2n-point real transform packed into n complex points)
 const float2 *af_twiddle_table(int log2n);

@@ -24,6 +24,7 @@
 #include "afb200_pwt.h"
 #include "afb200_spectral.h"
 #include "afb200_nsgt.h"
+#include "afb200_st.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -176,6 +177,16 @@ int spectralObj_spectralBatch(SpectralObj spectralObj, const float *spec, const 
  * Each clip's result is bit-identical to nsgtObj_nsgt on that clip, whatever the batch. */
 int nsgtObj_nsgtBatch(NSGTObj nsgtObj, const float *data, int batch, float *mReal, float *mImag,
                       float *cellReal, float *cellImag, int memKind, void *stream);
+
+/* S-transform of a batch: data batch x 2^radix2Exp -> planes batch x binLength x 2^radix2Exp, rows in the order of the
+ * object's bin list.  Each clip's result is bit-identical to stObj_st on that clip, whatever the batch. */
+int stObj_stBatch(STObj stObj, const float *data, int batch, float *mReal, float *mImag, int memKind, void *stream);
+/* rows of the current bin list (stObj_useBinArr may change it) */
+int stObj_getBinLength(STObj stObj);
+/* fast S-transform of a batch: planes batch x rows x 2^radix2Exp, rows = maxIndex - minIndex + 1 after the range rules of
+ * fstObj_fst.  Each clip's result is bit-identical to fstObj_fst on that clip, whatever the batch. */
+int fstObj_fstBatch(FSTObj fstObj, const float *data, int batch, int minIndex, int maxIndex, float *mReal, float *mImag,
+                    int memKind, void *stream);
 
 #ifdef __cplusplus
 }

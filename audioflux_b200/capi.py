@@ -254,6 +254,19 @@ ST_API = {
     "fstObj_fstBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp]),
 }
 
+# cepstrogram (include/cepstrogram_algorithm.h:21-39, include/afb200_cepstrogram.h) and the additive entry points
+# (include/afb200_ext.h)
+CEPSTROGRAM_API = {
+    "cepstrogramObj_new": (C.c_int, [P(vp), C.c_int, c_int_p, c_int_p]),
+    "cepstrogramObj_calTimeLength": (C.c_int, [vp, C.c_int]),
+    "cepstrogramObj_cepstrogram": (None, [vp, C.c_int, vp, C.c_int, vp, vp, vp]),
+    "cepstrogramObj_cepstrogram2": (None, [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp]),
+    "cepstrogramObj_enableDebug": (None, [vp, C.c_int]),
+    "cepstrogramObj_free": (None, [vp]),
+    "cepstrogramObj_cepstrogramBatch": (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]),
+    "cepstrogramObj_cepstrogram2Batch": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -267,7 +280,8 @@ REFERENCE_BUILDERS = {
 }
 
 
-def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, REFERENCE_BUILDERS)) -> dict:
+def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
+                              REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

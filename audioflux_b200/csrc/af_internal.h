@@ -393,6 +393,23 @@ int af_launch_st(const float *data, const float *specRe, const float *specIm, co
 int af_launch_fst(const float *specRe, const float *specIm, float *part, const int *seg, int minIndex, int rows, int log2n,
                   int batch, float *outRe, float *outIm, void *stream);
 
+/* Cepstrogram (kernels/cepstrogram.cu), N = 2^log2n <= AF_CEPS_MAX_N, one launch per call.  Frames come either from
+ * clips (data batch x dataLength, frame t at t * hop, times `window` unless NULL) or from STFT planes (specRe / specIm
+ * rows x specWidth, specWidth N or N/2+1; data == NULL).  Per frame L = logf(max(|X|^2, 1e-16)) (the even part over N
+ * bins at specWidth N), y = Re IFFT_N(L): cep = y[0 .. N/2], env = Re FFT_N(y liftered to quefrencies {0..c, N-c..N-1}),
+ * det = Re FFT_N(y on {c+1 .. N-c}); each output rows x (N/2+1) and skipped when NULL. */
+#define AF_CEPS_MAX_EXP 14
+#define AF_CEPS_MAX_N (1 << AF_CEPS_MAX_EXP)
+typedef struct {
+    int log2n, cepNum;
+    const float *data, *window;   /* clips: batch x dataLength; window device N floats or NULL (Rect) */
+    int dataLength, hop, timeLength, batch;
+    const float *specRe, *specIm; /* planes: rows x specWidth (data == NULL) */
+    int rows, specWidth;
+    float *cep, *env, *det;       /* device, frames x (N/2+1) each, or NULL */
+} AfCepsArgs;
+int af_launch_cepstrogram(const AfCepsArgs *a, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

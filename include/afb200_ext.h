@@ -25,6 +25,7 @@
 #include "afb200_spectral.h"
 #include "afb200_nsgt.h"
 #include "afb200_st.h"
+#include "afb200_cepstrogram.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -187,6 +188,17 @@ int stObj_getBinLength(STObj stObj);
  * fstObj_fst.  Each clip's result is bit-identical to fstObj_fst on that clip, whatever the batch. */
 int fstObj_fstBatch(FSTObj fstObj, const float *data, int batch, int minIndex, int maxIndex, float *mReal, float *mImag,
                     int memKind, void *stream);
+
+/* cepstrogram of a batch: data batch x dataLength -> cep / env / det batch x T x (N/2+1), T = cepstrogramObj_calTimeLength.
+ * Any of the three may be NULL (its work is skipped), not all three.  Each clip's result is bit-identical to
+ * cepstrogramObj_cepstrogram on that clip, whatever the batch. */
+int cepstrogramObj_cepstrogramBatch(CepstrogramObj cepstrogramObj, int cepNum, const float *data, int dataLength, int batch,
+                                    float *cep, float *env, float *det, int memKind, void *stream);
+/* the same from STFT planes rows x specWidth, one frame per row -> rows x (N/2+1).  specWidth = N (the mirrored layout of
+ * stftObj_stft: the even part of log S is used) or N/2+1 (the layout stftObj_stftBatch writes: taken as Hermitian).
+ * The planes are read only.  Each row's result is bit-identical to cepstrogramObj_cepstrogram2 on that row. */
+int cepstrogramObj_cepstrogram2Batch(CepstrogramObj cepstrogramObj, int cepNum, const float *mReal, const float *mImag,
+                                     int rows, int specWidth, float *cep, float *env, float *det, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

@@ -192,34 +192,31 @@ int af_launch_xxcc_standard(const float *in, const float *energy, int rows, int 
 int af_launch_chroma(const float *re, const float *im, int rows, int num, int chromaNum, int isMag,
                      int normType, const float *bank, float *out, void *stream);
 
+/* Fused MFCC at fftLength 2048: framed STFT -> |X|^2 / |X| -> banded bank (-> log10 / cbrt -> DCT-II) in one kernel.
+ * v2 (kernels/mfcc_fused2.cu) serves banks in which at most two consecutive filters overlap on a bin, v1
+ * (kernels/mfcc_fused.cu) the other banks its weight table holds; everything else takes the composed kernels. */
+enum { AF_MFCC_COMPOSED = -1, AF_MFCC_V1 = 0, AF_MFCC_V2 = 1 };
 typedef struct {
-    int fftLength, slideLength, num, ccNum, rectifyType, dataType;
+    int bankOnly, realMode, ccNum;    /* bftObj_bft's bank output (fused only in real mode), or ccNum cepstral coefficients */
+    int reassign, linear, banded;     /* the object: reassigned spectrum, Linear scale, banded device bank */
     float normValue;
-    const float *window, *dct;    /* device */
-    AfBankDev bank;
-    /* fused-kernel specific tables (device), built by af_mfcc_plan_build */
-    void *plan;
-} AfMfccArgs;
-int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const AfBands *bands);
-int af_mfcc_plan_build(void **plan, int fftLength, int num, int ccNum, const float *window,
-                       const float *bank, const AfBands *bands, const float *dct, int dataType);
-int af_launch_mel_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
-                        int slideLength, float *out, void *stream);   /* stops after the bank: batch x T x num */
-int af_mfcc_plan_mode(void *plan);      /* 0: a plan (the fused kernel serves the object), -1: no plan */
-void af_mfcc_plan_free(void *plan);
-int af_launch_mfcc_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
-                         int slideLength, int rectifyType, float *out, int nPeer, float *const *peerOut,
-                         void *stream);
-
-/* second-generation fused kernel (kernels/mfcc_fused2.cu): banks in which at most two consecutive filters overlap */
-int af_mfcc2_supported(int fftLength, int num, int ccNum, const float *bank /* num x (fftLength/2+1) */);
-int af_mfcc2_plan_build(void **plan, int fftLength, int num, int ccNum, const float *window, const float *bank,
-                        const float *dct, int dataType);
-void af_mfcc2_plan_free(void *plan);
-int af_launch_mfcc2(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                    int rectifyType, float *out, int nPeer, float *const *peerOut, void *stream);
-int af_launch_mel2(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                   float *out, void *stream);
+    int fftLength, num, slideLength, dataLength;
+    const float *data, *bank;         /* device clips; host bank num x (fftLength/2+1) */
+    const AfBands *bands;
+    int *v2Bank;                      /* the object's cache of v2's verdict on its bank: 0 unknown, 1 accepted, -1 rejected */
+} AfMfccCall;
+/* AF_MFCC_V2 / AF_MFCC_V1 / AF_MFCC_COMPOSED for one call (host only); reads the test hooks AFB200_MFCC_KERNEL=v1 and
+ * AFB200_BFT_GENERAL (bank output through the composed kernels) */
+int af_mfcc_route(const AfMfccCall *call);
+typedef struct AfMfccPlan AfMfccPlan;   /* device tables of one kernel (AF_MFCC_V1 | AF_MFCC_V2), bank-only or ccNum coefficients */
+int af_mfcc_plan_build(AfMfccPlan **plan, int kernel, int bankOnly, int fftLength, int num, int ccNum, const float *window,
+                       const float *bank, const AfBands *bands, int dataType);
+int af_mfcc_plan_kind(const AfMfccPlan *plan);     /* its kernel, AF_MFCC_COMPOSED for NULL */
+void af_mfcc_plan_free(AfMfccPlan *plan);
+/* out: batch x T x num (bank-only plan) or batch x T x ccNum, the latter also stored at the same offset of every
+ * peerOut[0..nPeer) (fused all-gather) */
+int af_launch_mfcc(const AfMfccPlan *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
+                   int rectifyType, float *out, int nPeer, float *const *peerOut, void *stream);
 
 int af_launch_decimate2(const float *in, int inLength, int inStride, int batch, const float *left32,
                         const float *right31, float *out, int outStride, void *stream);

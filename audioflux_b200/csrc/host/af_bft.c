@@ -1,7 +1,7 @@
 /* af_bft.c -- BFT object of the C ABI: STFT -> power / magnitude -> filter bank (-> fused MFCC).
  * Interface spec: src/bft_algorithm.h:14-57; behaviour src/bft_algorithm.c:87-276
  * (parameter rules), :397-540 (compute).  Compute = kernels/stft_generic.cu + kernels/bank_xxcc.cu,
- * or kernels/mfcc_fused.cu for the fftLength=2048 MFCC path. */
+ * or one of the fused kernels at fftLength 2048 (af_mfcc_route: kernels/mfcc_fused.cu, kernels/mfcc_fused2.cu). */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -30,12 +30,11 @@ struct OpaqueBFT {
     int *dStart, *dLen, *dOff;
     AfBankDev bankDev;
     AfDevBuf dSpecRe, dSpecIm, dMel;     /* spectrum planes; mel planes of the general MFCC path */
-    /* fused MFCC plan cache */
-    void *mfccPlan;
-    int mfccPlanCc;
-    void *melPlan;                       /* same fused kernel stopped after the bank (real-mode bftObj_bft at n = 2048) */
-    void *mfccPlan2, *melPlan2;          /* second-generation fused kernel (kernels/mfcc_fused2.cu), preferred when the bank qualifies */
-    int mfccPlan2Cc, v2State;            /* v2State: 0 unknown, 1 usable, -1 not (bank structure / AFB200_MFCC_KERNEL=v1) */
+    /* fused plans: the bank-only one (real-mode bftObj_bft) and the MFCC one for mfccCc coefficients */
+    AfMfccPlan *bankPlan, *mfccPlan;
+    int mfccCc;
+    int mfccRoute;                       /* AF_MFCC_* that served the last MFCC call (bftObj_mfccPlanMode) */
+    int v2Bank;                          /* v2's verdict on the bank (AfMfccCall) */
     float *dDctT;                        /* general path: transposed DCT [num][num] */
     AfPipe pipe;
     int isTemporal;                      /* bft_algorithm.c:376, 532-534: energy / rms / zcr of the frames of the last bftObj_bft call */
@@ -103,6 +102,7 @@ int af_bft_create(const AfBftSpec *p, BFTObj *out) {
     b->styleType = (SpectralFilterBankStyleType)p->styleType;
     b->normalType = (SpectralFilterBankNormalType)p->normalType;
     b->normValue = 1.0f;
+    b->mfccRoute = AF_MFCC_COMPOSED;
 
     const int width = n / 2 + 1;
     b->window = (float *)malloc(sizeof(float) * (size_t)n);
@@ -142,20 +142,11 @@ void bftObj_getTemporalData(BFTObj b, float **e, float **r, float **z) {
     if (r) *r = b->tempHost + b->tempLength;
     if (z) *z = b->tempHost + 2 * (size_t)b->tempLength;
 }
-int bftObj_mfccPlanMode(BFTObj b) { return b ? af_mfcc_plan_mode(b->mfccPlan) : -1; }
+int bftObj_mfccPlanMode(BFTObj b) { return b ? b->mfccRoute : AF_MFCC_COMPOSED; }
 int bftObj_getFilterBankArr(BFTObj b, float *bank) {
     if (!b || !bank) return af_fail(AF_ERR_ARG, "bftObj_getFilterBankArr: bad argument");
     memcpy(bank, b->bank, sizeof(float) * (size_t)b->num * (b->fftLength / 2 + 1));
     return AF_OK;
-}
-
-/* the v2 fused kernel needs fftLength 2048 and a bank whose bins are covered by at most two consecutive filters */
-static int bft_v2_usable(BFTObj b, int ccNum) {
-    if (b->v2State == 0) {
-        const char *k = getenv("AFB200_MFCC_KERNEL");
-        b->v2State = (k && !strcmp(k, "v1")) ? -1 : (af_mfcc2_supported(b->fftLength, b->num, 1, b->bank) ? 1 : -1);
-    }
-    return b->v2State > 0 && ccNum >= 1 && ccNum <= 64;
 }
 
 int af_bft_device(BFTObj b) {
@@ -192,49 +183,55 @@ int af_bft_device(BFTObj b) {
     return AF_OK;
 }
 
-/* device-resident compute: dData [batch x dataLength] -> dRe (and dIm) [batch x T x num] */
-static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, float *dRe, float *dIm, void *st) {
+/* the kernel that serves a fused call on these clips: ccNum 0 = the bank output (real or complex mode) */
+static int bft_route(BFTObj b, const float *dData, int dataLength, int ccNum, int realMode) {
+    const AfMfccCall c = {ccNum == 0, realMode, ccNum, b->reassign != NULL, b->scaleType == SpectralFilterBankScale_Linear,
+                          b->bankDev.banded, b->normValue, b->fftLength, b->num, b->slideLength, dataLength, dData, b->bank,
+                          &b->bands, &b->v2Bank};
+    return af_mfcc_route(&c);
+}
+
+/* the object's cached plan in *slot, rebuilt when it was made for another kernel (or another ccNum) */
+static int bft_plan(BFTObj b, AfMfccPlan **slot, int kernel, int ccNum) {
+    const int bankOnly = slot == &b->bankPlan;
+    if (*slot && af_mfcc_plan_kind(*slot) == kernel && (bankOnly || b->mfccCc == ccNum)) return AF_OK;
+    af_mfcc_plan_free(*slot);
+    *slot = NULL;
+    const int rc = af_mfcc_plan_build(slot, kernel, bankOnly, b->fftLength, b->num, ccNum, b->window, b->bank, &b->bands, b->dataType);
+    if (!rc && !bankOnly) b->mfccCc = ccNum;
+    return rc;
+}
+
+/* clips per chunk of a device workspace of perClip bytes per clip: a quarter of the free memory, at most cap bytes */
+static int bft_chunk_clips(size_t perClip, size_t cap, int batch) {
+    size_t budget = af_dev_free_bytes() / 4;
+    if (budget < perClip) budget = perClip;
+    if (budget > cap) budget = cap;
+    int chunk = (int)(budget / perClip);
+    if (chunk < 1) chunk = 1;
+    return chunk > batch ? batch : chunk;
+}
+
+/* device-resident compute: dData [batch x dataLength] -> dRe (and, complex mode, dIm) [batch x T x num] */
+static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, float *dRe, float *dIm, int realMode, void *st) {
     const int T = bftObj_calTimeLength(b, dataLength);
     const int width = b->fftLength / 2 + 1;
     if (T <= 0) return AF_OK;
-    /* real mode at fftLength 2048 with a banded bank: the fused TMA-fed kernel of the MFCC path, stopped after the
-     * filter bank (one launch, no spectrum round trip through HBM: 3.3x the general composition below) */
-    if (!b->reassign && b->resultType && b->normValue == 1.0f && b->scaleType != SpectralFilterBankScale_Linear && b->bankDev.banded &&
-        af_mfcc_fused_supported(b->fftLength, b->num, 1, &b->bands) && b->slideLength % 4 == 0 && dataLength % 4 == 0 &&
-        ((size_t)dData & 15) == 0 && !getenv("AFB200_BFT_GENERAL")) {
-        int rc = AF_OK;
-        if (bft_v2_usable(b, 1)) {
-            if (!b->melPlan2) {
-                float *dct = (float *)calloc((size_t)b->num, sizeof(float));      /* unused by this mode */
-                if (!dct) return AF_ERR_NOMEM;
-                rc = af_mfcc2_plan_build(&b->melPlan2, b->fftLength, b->num, 1, b->window, b->bank, dct, b->dataType);
-                free(dct);
-                if (rc) return rc;
-            }
-            return af_launch_mel2(b->melPlan2, dData, dataLength, batch, T, b->slideLength, dRe, st);
-        }
-        if (!b->melPlan) {
-            float *dct = (float *)calloc((size_t)b->num, sizeof(float));      /* unused by this mode */
-            if (!dct) return AF_ERR_NOMEM;
-            rc = af_mfcc_plan_build(&b->melPlan, b->fftLength, b->num, 1, b->window, b->bank, &b->bands, dct, b->dataType);
-            free(dct);
-            if (rc) return rc;
-        }
-        return af_launch_mel_fused(b->melPlan, dData, dataLength, batch, T, b->slideLength, dRe, st);
+    /* real mode at fftLength 2048 with a banded bank: a fused kernel stopped after the filter bank (one launch, no
+     * spectrum round trip through HBM: 3.3x the general composition below) */
+    const int route = bft_route(b, dData, dataLength, 0, realMode);
+    int rc;
+    if (route != AF_MFCC_COMPOSED) {
+        if ((rc = bft_plan(b, &b->bankPlan, route, 1))) return rc;
+        return af_launch_mfcc(b->bankPlan, dData, dataLength, batch, T, b->slideLength, 0, dRe, 0, NULL, st);
     }
     const int linear = b->scaleType == SpectralFilterBankScale_Linear;
     const int count = b->highIndex - b->lowIndex + 1 < b->num ? b->highIndex - b->lowIndex + 1 : b->num;
     /* the spectrum workspace is bounded: process the batch in chunks of clips */
     const size_t perClip = sizeof(float) * (size_t)T * width;
-    size_t budget = af_dev_free_bytes() / 4;
-    if (budget < perClip) budget = perClip;
-    if (budget > ((size_t)3 << 30)) budget = (size_t)3 << 30;
-    int chunk = (int)(budget / perClip);
-    if (chunk < 1) chunk = 1;
-    if (chunk > batch) chunk = batch;
-    int rc;
+    const int chunk = bft_chunk_clips(perClip, (size_t)3 << 30, batch);
     if ((rc = af_devbuf_reserve(&b->dSpecRe, perClip * chunk))) return rc;
-    if (!b->resultType && (rc = af_devbuf_reserve(&b->dSpecIm, perClip * chunk))) return rc;
+    if (!realMode && (rc = af_devbuf_reserve(&b->dSpecIm, perClip * chunk))) return rc;
     for (int c0 = 0; c0 < batch; c0 += chunk) {
         const int nb = batch - c0 < chunk ? batch - c0 : chunk;
         AfFrameSrc src;
@@ -252,11 +249,11 @@ static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, 
             sIm = (float *)b->dSpecIm.ptr;
             if ((rc = af_memset_d(sRe, 0, perClip * nb, st)) || (rc = af_memset_d(sIm, 0, perClip * nb, st))) return rc;
             if ((rc = reassignObj_reassignBatch(b->reassign, src.data, dataLength, nb, sRe, sIm, NULL, NULL, AFB200_MEM_DEVICE, st))) return rc;
-            const int mode = b->resultType ? (b->dataType == SpectralData_Mag ? AF_STFT_MAG : AF_STFT_POWER)
+            const int mode = realMode ? (b->dataType == SpectralData_Mag ? AF_STFT_MAG : AF_STFT_POWER)
                                            : (b->dataType == SpectralData_Power ? AF_STFT_SQUARE : AF_STFT_HALF);
             if ((rc = af_launch_spec_post(sRe, sIm, (long long)rows * width, mode, b->normValue, st))) return rc;
         }
-        if (b->resultType) {                                  /* real: sum_k w |z|^2 (or |z|) */
+        if (realMode) {                                       /* real: sum_k w |z|^2 (or |z|) */
             const int mode = b->dataType == SpectralData_Mag ? AF_STFT_MAG : AF_STFT_POWER;
             if (!b->reassign && (rc = af_launch_stft(&src, mode, b->normValue, sRe, NULL, st))) return rc;
             const float post = (b->dataType == SpectralData_Mag) ? b->normValue : 1.0f;
@@ -285,7 +282,7 @@ typedef struct { BFTObj b; int dataLength, ccNum, rectifyType; } BftCall;
 
 static int bft_chunk(void *p, int nb, float *const *d, void *st) {
     const BftCall *a = (const BftCall *)p;
-    return bft_compute(a->b, d[0], a->dataLength, nb, d[1], d[2], st);
+    return bft_compute(a->b, d[0], a->dataLength, nb, d[1], d[2], a->b->resultType, st);
 }
 
 int bftObj_bftBatch(BFTObj b, const float *data, int dataLength, int batch, float *mReal3, float *mImag3,
@@ -336,16 +333,11 @@ void bftObj_bft(BFTObj b, float *dataArr, int dataLength, float *mRealArr3, floa
  * atan2f(im, re < 1e-16 ? 1e-16 : re).  phase: batch x T x count. */
 int af_bft_spectrogram(BFTObj b, const float *dData, int dataLength, int batch, float *dSpect, int lowIndex, int count,
                        float *dPhase, void *st) {
-    int rc = bft_compute(b, dData, dataLength, batch, dSpect, NULL, st);
+    int rc = bft_compute(b, dData, dataLength, batch, dSpect, NULL, b->resultType, st);
     if (rc || !dPhase) return rc;
     const int T = bftObj_calTimeLength(b, dataLength), width = b->fftLength / 2 + 1;
     const size_t perClip = sizeof(float) * (size_t)T * width;
-    size_t budget = af_dev_free_bytes() / 4;
-    if (budget < perClip) budget = perClip;
-    if (budget > ((size_t)2 << 30)) budget = (size_t)2 << 30;
-    int chunk = (int)(budget / perClip);
-    if (chunk < 1) chunk = 1;
-    if (chunk > batch) chunk = batch;
+    const int chunk = bft_chunk_clips(perClip, (size_t)2 << 30, batch);
     if ((rc = af_devbuf_reserve(&b->dSpecRe, perClip * chunk)) || (rc = af_devbuf_reserve(&b->dSpecIm, perClip * chunk))) return rc;
     for (int c0 = 0; c0 < batch; c0 += chunk) {
         const int nb = batch - c0 < chunk ? batch - c0 : chunk;
@@ -366,44 +358,16 @@ static int mfcc_compute(BFTObj b, const float *dData, int dataLength, int batch,
                         float *dOut, int nPeer, float *const *peerOut, void *st) {
     const int T = bftObj_calTimeLength(b, dataLength);
     int rc;
-    const int fusable = !b->reassign && b->normValue == 1.0f && b->scaleType != SpectralFilterBankScale_Linear &&
-                        b->bankDev.banded && af_mfcc_fused_supported(b->fftLength, b->num, ccNum, &b->bands) &&
-                        b->slideLength % 4 == 0 && dataLength % 4 == 0 && ((size_t)dData & 15) == 0;
-    if (fusable && bft_v2_usable(b, ccNum)) {
-        if (!b->mfccPlan2 || b->mfccPlan2Cc != ccNum) {
-            af_mfcc2_plan_free(b->mfccPlan2); b->mfccPlan2 = NULL;
-            float *dct = (float *)malloc(sizeof(float) * (size_t)ccNum * b->num);
-            if (!dct) return AF_ERR_NOMEM;
-            af_dct2_matrix(b->num, ccNum, dct);
-            rc = af_mfcc2_plan_build(&b->mfccPlan2, b->fftLength, b->num, ccNum, b->window, b->bank, dct, b->dataType);
-            free(dct);
-            if (rc) return rc;
-            b->mfccPlan2Cc = ccNum;
-        }
-        return af_launch_mfcc2(b->mfccPlan2, dData, dataLength, batch, T, b->slideLength, rectifyType, dOut, nPeer, peerOut, st);
-    }
-    if (fusable) {
-        if (!b->mfccPlan || b->mfccPlanCc != ccNum) {
-            af_mfcc_plan_free(b->mfccPlan); b->mfccPlan = NULL;
-            float *dct = (float *)malloc(sizeof(float) * (size_t)ccNum * b->num);
-            if (!dct) return AF_ERR_NOMEM;
-            af_dct2_matrix(b->num, ccNum, dct);
-            rc = af_mfcc_plan_build(&b->mfccPlan, b->fftLength, b->num, ccNum, b->window, b->bank, &b->bands, dct, b->dataType);
-            free(dct);
-            if (rc) return rc;
-            b->mfccPlanCc = ccNum;
-        }
-        return af_launch_mfcc_fused(b->mfccPlan, dData, dataLength, batch, T, b->slideLength, rectifyType, dOut, nPeer, peerOut, st);
+    b->mfccRoute = bft_route(b, dData, dataLength, ccNum, 1);
+    if (b->mfccRoute != AF_MFCC_COMPOSED) {
+        if ((rc = bft_plan(b, &b->mfccPlan, b->mfccRoute, ccNum))) return rc;
+        return af_launch_mfcc(b->mfccPlan, dData, dataLength, batch, T, b->slideLength, rectifyType, dOut, nPeer, peerOut, st);
     }
     if (nPeer > 0) return af_fail(AF_ERR_UNSUPPORTED, "bftObj_mfccBatchScatter: only the fused fftLength=2048 path can store to peers");
     /* general composition (any fftLength / bank / alignment), still entirely on the device */
     if (!b->dDctT && (rc = af_dct2_upload_transposed(&b->dDctT, b->num))) return rc;
-    const int savedType = b->resultType;
-    b->resultType = 1;
-    rc = af_devbuf_reserve(&b->dMel, sizeof(float) * (size_t)batch * T * b->num);
-    if (!rc) rc = bft_compute(b, dData, dataLength, batch, (float *)b->dMel.ptr, NULL, st);
-    b->resultType = savedType;
-    if (rc) return rc;
+    if ((rc = af_devbuf_reserve(&b->dMel, sizeof(float) * (size_t)batch * T * b->num)) ||
+        (rc = bft_compute(b, dData, dataLength, batch, (float *)b->dMel.ptr, NULL, 1, st))) return rc;
     return af_launch_xxcc((const float *)b->dMel.ptr, batch * T, b->num, ccNum, rectifyType, b->dDctT, dOut, st);
 }
 
@@ -443,8 +407,7 @@ int bftObj_mfccBatchScatter(BFTObj b, const float *data, int dataLength, int bat
 
 void bftObj_free(BFTObj b) {
     if (!b) return;
-    af_mfcc_plan_free(b->mfccPlan); af_mfcc_plan_free(b->melPlan);
-    af_mfcc2_plan_free(b->mfccPlan2); af_mfcc2_plan_free(b->melPlan2);
+    af_mfcc_plan_free(b->mfccPlan); af_mfcc_plan_free(b->bankPlan);
     reassignObj_free(b->reassign);
     free(b->tempHost);
     af_devbuf_free(&b->dSpecRe); af_devbuf_free(&b->dSpecIm); af_devbuf_free(&b->dMel);

@@ -28,10 +28,8 @@
 //     log-mel rows into a multi-buffered (kLBufs) 16 x 128 shared tile and a dedicated epilogue warp contracts the
 //     whole tile on the tensor cores (mma.sync m16n8k8 TF32, 3xTF32 split so the result keeps fp32 accuracy)
 //     while the frame warps are already transforming the next tile.
-#include <math.h>
-#include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
+#include "mfcc_common.cuh"
 #include "fft32_gen.cuh"
 
 namespace {
@@ -41,7 +39,6 @@ constexpr int kNC = 1024;           // packed complex points
 constexpr int kFrameWarps = 13;     // consumer warps = max frames per tile (<= 16: one mma M tile)
 constexpr int kEpiWarps = 2;        // DCT epilogue warps; tile `it` is served by warp it % kEpiWarps
 constexpr int kThreads = (kFrameWarps + 1 + kEpiWarps) * 32;   // + TMA producer warp + DCT epilogue warps
-constexpr int kMaxPeers = 15;      // extra destinations of the output tile (P2P stores to peer GPUs)
 constexpr int kLPitch = 132;        // log-mel tile row pitch (floats): 4g + t -> 32 distinct banks for mma A fragments
 constexpr int kLRows = 16;          // stored rows of the mma M=16 tile (rows >= kFrameWarps are zeros)
 constexpr int kStages = 2;
@@ -86,7 +83,7 @@ struct Params {
     // fused all-gather: every finished tile is also stored at the same offset of up to kMaxPeers other buffers
     // (peer GPUs' gathered arrays mapped over NVLink, opened with cudaIpcOpenMemHandle by the host side)
     int nPeer;
-    float *peerOut[kMaxPeers];
+    float *peerOut[kMfccMaxPeers];
 };
 
 // shared-memory carve-up (bytes), all 16-byte aligned
@@ -103,7 +100,7 @@ __host__ __device__ inline Smem carve(int spanFloats, int melWFloats, int ct) {
     s.tw2Off = o;      o += 32 * 8;
     s.melWOff = o;     o += ((melWFloats * 4 + 15) / 16) * 16;
     s.melStartOff = o; o += kMaxNum * 4;
-    s.dctOff = o;      o += kMaxNum * (ct <= 5 ? 40 : 72) * 4;
+    s.dctOff = o;      o += kMaxNum * af_mfcc_dct_pitch(ct) * 4;
     s.lOff = o;        o += kLBufs * kLRows * kLPitch * 4;
     s.stageOff = o;    o += kEpiWarps * kStageBytes;
     s.barOff = o;      o += (2 * kStages + 2 * kLBufs) * 8;
@@ -128,7 +125,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
     uint64_t *emptyBar = fullBar + kStages;
     uint64_t *lFull = emptyBar + kStages;                                  // [kLBufs] frame warps -> epilogue
     uint64_t *lEmpty = lFull + kLBufs;                                     // [kLBufs] epilogue -> frame warps
-    constexpr int kDctPitch = CT <= 5 ? 40 : 72;
+    constexpr int kDctPitch = af_mfcc_dct_pitch(CT);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -193,29 +190,18 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
                 acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.0f;
                 acx[n][0] = acx[n][1] = acx[n][2] = acx[n][3] = 0.0f;
             }
-#define AF_MMA_TF32(ACC, A0, A1, A2, A3, B0, B1)                                                              \
-    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};" \
-        : "+f"(ACC[0]), "+f"(ACC[1]), "+f"(ACC[2]), "+f"(ACC[3])                                              \
-        : "r"(A0), "r"(A1), "r"(A2), "r"(A3), "r"(B0), "r"(B1))
 #pragma unroll 2
             for (int k0 = 0; k0 < kMaxNum; k0 += 8) {
                 const float af[4] = {A[g * kLPitch + k0 + t], A[(g + 8) * kLPitch + k0 + t],
                                      A[g * kLPitch + k0 + t + 4], A[(g + 8) * kLPitch + k0 + t + 4]};
-                // TF32 split by truncation: hi = top 19 bits, lo = (x - hi) (exact), again cut to 19 bits
                 uint32_t ah[4], al[4], bh[CT][2], bl[CT][2];
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    ah[i] = __float_as_uint(af[i]) & 0xffffe000u;
-                    al[i] = __float_as_uint(af[i] - __uint_as_float(ah[i])) & 0xffffe000u;
-                }
+                for (int i = 0; i < 4; i++) af_tf32_split(af[i], ah[i], al[i]);
 #pragma unroll
                 for (int n = 0; n < CT; n++) {
                     const float bf[2] = {sDct[(k0 + t) * kDctPitch + n * 8 + g], sDct[(k0 + t + 4) * kDctPitch + n * 8 + g]};
 #pragma unroll
-                    for (int i = 0; i < 2; i++) {
-                        bh[n][i] = __float_as_uint(bf[i]) & 0xffffe000u;
-                        bl[n][i] = __float_as_uint(bf[i] - __uint_as_float(bh[n][i])) & 0xffffe000u;
-                    }
+                    for (int i = 0; i < 2; i++) af_tf32_split(bf[i], bh[n][i], bl[n][i]);
                 }
 #pragma unroll
                 for (int n = 0; n < CT; n++) AF_MMA_TF32(acx[n], al[0], al[1], al[2], al[3], bh[n][0], bh[n][1]);
@@ -224,7 +210,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
 #pragma unroll
                 for (int n = 0; n < CT; n++) AF_MMA_TF32(acx[n], ah[0], ah[1], ah[2], ah[3], bl[n][0], bl[n][1]);
             }
-#undef AF_MMA_TF32
 #pragma unroll
             for (int n = 0; n < CT; n++)
 #pragma unroll
@@ -238,7 +223,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
             const long long tileOff = ((long long)clip * p.timeLength + f0) * p.ccNum;
             if (p.bulkStore) {
                 float *stage = reinterpret_cast<float *>(smem + L.stageOff + epi * kStageBytes);
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");       // this warp's previous stores have read the staging tile
+                af_bulk_wait_read0();                                        // this warp's previous stores have read the staging tile
                 __syncwarp();
 #pragma unroll
                 for (int n = 0; n < CT; n++) {
@@ -252,13 +237,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
                         if (c + 1 < p.ccNum) stage[(g + 8) * p.ccNum + c + 1] = acc[n][3];
                     }
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                af_fence_proxy_async_smem();
                 __syncwarp();
                 if (lane <= p.nPeer) {
                     float *o = (lane == 0 ? p.out : p.peerOut[lane - 1]) + tileOff;
-                    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                                 ::"l"(o), "r"(af_smem_u32(stage)), "r"((uint32_t)(nf * p.ccNum * 4)) : "memory");
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    af_bulk_store(o, stage, (uint32_t)(nf * p.ccNum * 4));
+                    af_bulk_commit();
                 }
             } else {
                 for (int d = 0; d <= p.nPeer; d++) {
@@ -278,7 +262,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
                 }
             }
         }
-        if (p.bulkStore) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        if (p.bulkStore) af_bulk_wait0();
         return;
     }
 
@@ -413,9 +397,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused(Params p) {
                 wg4 += len4 * 32;
                 continue;
             }
-            if (p.rectify == CepstralRectify_CubicRoot) v = powf(v, 1.0f / 3.0f);
-            else v = __log2f(v < 1e-8f ? 1e-8f : v) * 0.30102999566398120f;   // log10 via MUFU.LG2
-            lrow[g * 32 + lane] = v;
+            lrow[g * 32 + lane] = af_mfcc_rectify(v, p.rectify);
             wg4 += len4 * 32;
         }
         if (!p.rawMel) for (int g = p.melGroups; g < 4; g++) lrow[g * 32 + lane] = 0.0f;
@@ -474,7 +456,7 @@ static int plan_mel(const AfBands *bands, int num, int *startShifted /* kMaxNum 
     return total + 8 * 32;                                    // two stages of padding for the pipelined prefetch
 }
 
-extern "C" int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const AfBands *bands) {
+int af_mfcc1_supported(int fftLength, int num, int ccNum, const AfBands *bands) {
     if (fftLength != kN || num < 1 || num > kMaxNum || ccNum < 1 || ccNum > 64 || !bands) return 0;
     int starts[kMaxNum], groupLen[4];
     const int floats = plan_mel(bands, num, starts, groupLen);
@@ -482,18 +464,16 @@ extern "C" int af_mfcc_fused_supported(int fftLength, int num, int ccNum, const 
     return floats * 4 <= 24 * 1024;                              // weight table budget in shared memory
 }
 
-extern "C" void af_mfcc_plan_free(void *plan) { free_plan(static_cast<Plan *>(plan)); }
-extern "C" int af_mfcc_plan_mode(void *plan) { return plan ? 0 : -1; }
+void af_mfcc1_plan_free(void *plan) { free_plan(static_cast<Plan *>(plan)); }
 
-extern "C" int af_mfcc_plan_build(void **planOut, int fftLength, int num, int ccNum, const float *window,
-                                  const float *bank, const AfBands *bands, const float *dct /* ccNum x num */,
-                                  int dataType) {
+int af_mfcc1_plan_build(void **planOut, int fftLength, int num, int ccNum, const float *window, const float *bank,
+                        const AfBands *bands, const float *dct /* ccNum x num */, int dataType) {
     *planOut = NULL;
-    if (!af_mfcc_fused_supported(fftLength, num, ccNum, bands)) return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC plan: unsupported configuration");
+    if (!af_mfcc1_supported(fftLength, num, ccNum, bands)) return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC plan: unsupported configuration");
     Plan *pl = static_cast<Plan *>(calloc(1, sizeof(Plan)));
     if (!pl) return AF_ERR_NOMEM;
     pl->num = num; pl->ccNum = ccNum; pl->dataType = dataType;
-    pl->ct = ccNum <= 16 ? 2 : ccNum <= 24 ? 3 : ccNum <= 40 ? 5 : 8;
+    pl->ct = af_mfcc_ct(ccNum);
     int rc = AF_OK;
 
     float *wh = static_cast<float *>(malloc(sizeof(float) * kN));
@@ -536,29 +516,16 @@ extern "C" int af_mfcc_plan_build(void **planOut, int fftLength, int num, int cc
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelW), mw, sizeof(float) * (size_t)(total > 0 ? total : 1));
     free(mw);
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dMelStart), starts, sizeof(int) * kMaxNum);
-
-    // DCT table as the mma B operand: D^T[m][c] with row pitch 40 (72 for cc > 40): pitch % 32 == 8 makes the
-    // (k0 + t, n0 + g) fragment reads hit 32 different banks; rows m >= num and columns c >= ccNum are zero
-    const int ct = pl->ct, pitch = ct <= 5 ? 40 : 72;
-    float *dt = static_cast<float *>(calloc((size_t)kMaxNum * pitch, sizeof(float)));
-    for (int m = 0; m < num; m++)
-        for (int c = 0; c < ccNum; c++) dt[(size_t)m * pitch + c] = dct[(size_t)c * num + m];
-    if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dDct), dt, sizeof(float) * (size_t)kMaxNum * pitch);
-    free(dt);
+    if (rc == AF_OK) rc = af_mfcc_dct_upload(&pl->dDct, dct, num, ccNum, pl->ct);
 
     if (rc != AF_OK) { free_plan(pl); return rc; }
     *planOut = pl;
     return AF_OK;
 }
 
-static int launch_fused(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                        int rectifyType, float *out, int nPeer, float *const *peerOut, int rawMel, void *stream) {
+int af_mfcc1_launch(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
+                    int rectifyType, float *out, int nPeer, float *const *peerOut, int rawMel, void *stream) {
     Plan *pl = static_cast<Plan *>(plan);
-    if (!pl) return af_fail(AF_ERR_ARG, "fused MFCC: no plan");
-    if (batch <= 0 || timeLength <= 0) return AF_OK;
-    if (slideLength % 4 || dataLength % 4 || (reinterpret_cast<uintptr_t>(data) & 15))
-        return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC needs 16-byte aligned clips and slideLength %% 4 == 0 (TMA bulk copy)");
-
     Params p;
     memset(&p, 0, sizeof(p));
     p.data = data; p.out = out; p.windowHalf = pl->dWindowHalf; p.tw1 = pl->dTw1; p.tw2 = pl->dTw2;
@@ -569,14 +536,9 @@ static int launch_fused(void *plan, const float *data, int dataLength, int batch
     for (int g = 0; g < 4; g++) p.melGroupLen[g] = pl->melGroupLen[g];
     p.ccNum = pl->ccNum; p.rectify = rectifyType; p.dataType = pl->dataType;
     p.rawMel = rawMel;
-    if (nPeer < 0 || nPeer > kMaxPeers || (nPeer > 0 && !peerOut)) return af_fail(AF_ERR_ARG, "fused MFCC: nPeer=%d outside [0, %d]", nPeer, kMaxPeers);
     p.nPeer = nPeer;
     for (int d = 0; d < nPeer; d++) p.peerOut[d] = peerOut[d];
-    {   // one bulk store per destination needs 16-byte aligned tiles: ccNum % 4 == 0 and aligned bases
-        int bulk = !rawMel && pl->ccNum % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-        for (int d = 0; d < nPeer; d++) if (reinterpret_cast<uintptr_t>(peerOut[d]) & 15) bulk = 0;
-        p.bulkStore = bulk;
-    }
+    p.bulkStore = !rawMel && af_mfcc_bulk_store_ok(pl->ccNum, out, nPeer, peerOut);   // (the bank output leaves row by row)
 
     // frames per tile: as many as fit the shared-memory budget (<= kFrameWarps)
     const int budget = 227 * 1024;
@@ -592,35 +554,6 @@ static int launch_fused(void *plan, const float *data, int dataLength, int batch
     p.tilesPerClip = (timeLength + F - 1) / F;
     p.totalTiles = (long long)p.tilesPerClip * batch;
     const int smemBytes = carve(p.spanFloats, pl->melWFloats, pl->ct).total;
-
-    int sms = af_sm_count();
-    if (sms <= 0) sms = 132;
-    long long grid = p.totalTiles < (long long)sms ? p.totalTiles : (long long)sms;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaSuccess;
-#define AF_MFCC_LAUNCH(CT_)                                                                                       \
-    e = cudaFuncSetAttribute(k_mfcc_fused<CT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smemBytes);         \
-    if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_mfcc_fused)");                          \
-    k_mfcc_fused<CT_><<<(unsigned)grid, kThreads, smemBytes, st>>>(p)
-    switch (pl->ct) {
-    case 2: AF_MFCC_LAUNCH(2); break;
-    case 3: AF_MFCC_LAUNCH(3); break;
-    case 5: AF_MFCC_LAUNCH(5); break;
-    default: AF_MFCC_LAUNCH(8); break;
-    }
-#undef AF_MFCC_LAUNCH
-    AF_LAUNCH_CHECK("k_mfcc_fused");
-    return AF_OK;
-}
-
-extern "C" int af_launch_mfcc_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
-                                    int slideLength, int rectifyType, float *out, int nPeer, float *const *peerOut,
-                                    void *stream) {
-    return launch_fused(plan, data, dataLength, batch, timeLength, slideLength, rectifyType, out, nPeer, peerOut, 0, stream);
-}
-
-// same kernel stopped after the filter bank: out[batch][T][num] = bank . |X|^2 (or |X|), i.e. bftObj_bft in real mode
-extern "C" int af_launch_mel_fused(void *plan, const float *data, int dataLength, int batch, int timeLength,
-                                   int slideLength, float *out, void *stream) {
-    return launch_fused(plan, data, dataLength, batch, timeLength, slideLength, 0, out, 0, NULL, 1, stream);
+    static void (*const kernels[4])(Params) = {k_mfcc_fused<2>, k_mfcc_fused<3>, k_mfcc_fused<5>, k_mfcc_fused<8>};
+    return af_mfcc_launch_ct(kernels, "k_mfcc_fused", pl->ct, p.totalTiles, kThreads, smemBytes, stream, p);
 }

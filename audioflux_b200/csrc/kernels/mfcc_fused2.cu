@@ -25,10 +25,8 @@
 //    tile rows its pass has finished reading, and are added up per band in a fixed order (bit-stable);
 //  * the 13 x cc result tile is staged in shared memory and leaves as one TMA bulk store per destination (this GPU and,
 //    for the fused all-gather, every peer GPU): full lines over NVLink instead of 32-bit stores.
-#include <math.h>
-#include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
+#include "mfcc_common.cuh"
 #include "fft32_gen.cuh"
 
 namespace {
@@ -41,7 +39,6 @@ constexpr int kBW = 4;              // filter-bank warps (one interval per lane)
 constexpr int kDW = 2;              // DCT (tensor-core) + store warps, one tile behind the bank warps
 constexpr int kEW = kBW;                        // (planner: helper lanes that walk intervals)
 constexpr int kThreads = (kFW + 1 + kBW + kDW) * 32;  // + producer / special-column warp: 20 warps at <= 96 registers
-constexpr int kMaxPeers = 15;
 constexpr int kMaxNum = 128;
 constexpr int kLPitch = 132;        // log-mel tile row pitch (floats): 4g + t -> 32 distinct banks for mma A fragments
 constexpr int kMaxTab = 1408;       // bank table entries (one float4 per bin pair of an interval) in the parameter block
@@ -83,7 +80,7 @@ struct Params {
     int batch, timeLength, hop, framesPerTile, tilesPerClip, spanFloats, stages;
     int num, ccNum, rectify, dataType, rawMel, bulkStore, dctPitch;
     int nPeer;
-    float *peerOut[kMaxPeers];
+    float *peerOut[kMfccMaxPeers];
     int offSpan, offScratch, offP, offWin, offTw, offSpec, offDct, offL, offStage, offTab, offDesc, offAssign, offPrefix, stageBytes;   // offL: two log-mel tiles
     int nPass, passLen[kMaxPass];
     const unsigned short *assign;
@@ -95,19 +92,6 @@ struct Params {
 
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void bulk_store(void *dstGmem, const void *srcSmem, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                 ::"l"(dstGmem), "r"(af_smem_u32(srcSmem)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-__device__ __forceinline__ float rectify_value(float v, int rectify) {
-    if (rectify == CepstralRectify_CubicRoot) return powf(v, 1.0f / 3.0f);
-    return __log2f(v < 1e-8f ? 1e-8f : v) * 0.30102999566398120f;      // log10 via MUFU.LG2
 }
 
 template <int CT>
@@ -288,7 +272,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             float *L = sL + (size_t)lbuf * 16 * kLPitch;
             float *stage = sStage + (size_t)lbuf * (p.stageBytes / 8);   // (filter-bank output mode: two staging tiles)
             const int stagePitch = p.num + 4;                              // padded rows (bank conflicts)
-            if (p.rawMel && e == 0) bulk_wait_read0();             // the store of tile it - 2 has read this staging tile
+            if (p.rawMel && e == 0) af_bulk_wait_read0();             // the store of tile it - 2 has read this staging tile
             named_bar_sync(1, kBW * 32);                           // every partial sum of the tile is in shared memory
             // ---- phase 2: mel_m = sum of the rise parts of interval m + the fall parts of interval m + 1 (pieces in
             // ascending order), rectified (cepstra) or staged as the result row (filter bank) ----
@@ -316,7 +300,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
 #pragma unroll
                 for (int f = 0; f < kFW; f++) {
                     if (p.rawMel) { if (f < nf) stage[f * stagePitch + m] = v[f]; }
-                    else L[f * kLPitch + m] = rectify_value(v[f], p.rectify);
+                    else L[f * kLPitch + m] = af_mfcc_rectify(v[f], p.rectify);
                 }
             }
             if (!p.rawMel) {
@@ -324,20 +308,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 if (lane == 0) af_mbar_arrive(&lFull[lbuf]);       // the DCT warps take the tile from here
                 continue;
             }
-            fence_proxy_async_smem();
+            af_fence_proxy_async_smem();
             named_bar_sync(3, kBW * 32);                           // the result rows are staged
             const long long tileOff = ((long long)clip * p.timeLength + f0) * rowFloats;
             if (p.bulkStore) {
                 if (e == 0) {                                       // one row per lane (padded staging rows)
-                    if (lane < nf) bulk_store(p.out + tileOff + (long long)lane * rowFloats, stage + lane * stagePitch, (uint32_t)(rowFloats * 4));
-                    bulk_commit();
+                    if (lane < nf) af_bulk_store(p.out + tileOff + (long long)lane * rowFloats, stage + lane * stagePitch, (uint32_t)(rowFloats * 4));
+                    af_bulk_commit();
                 }
             } else {
                 for (int r = 0; r < nf; r++)
                     for (int i = e * 32 + lane; i < rowFloats; i += kBW * 32) p.out[tileOff + (long long)r * rowFloats + i] = stage[r * stagePitch + i];
             }
         }
-        if (e == 0) bulk_wait0();
+        if (e == 0) af_bulk_wait0();
         return;
     }
 
@@ -364,20 +348,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.0f;
                 acx[n][0] = acx[n][1] = acx[n][2] = acx[n][3] = 0.0f;
             }
-#define AF_MMA_TF32(ACC, A0, A1, A2, A3, B0, B1)                                                              \
-    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};" \
-        : "+f"(ACC[0]), "+f"(ACC[1]), "+f"(ACC[2]), "+f"(ACC[3])                                              \
-        : "r"(A0), "r"(A1), "r"(A2), "r"(A3), "r"(B0), "r"(B1))
 #pragma unroll 2
             for (int k0 = 0; k0 < kMaxNum; k0 += 8) {
                 const float af[4] = {L[g * kLPitch + k0 + t], L[(g + 8) * kLPitch + k0 + t],
                                      L[g * kLPitch + k0 + t + 4], L[(g + 8) * kLPitch + k0 + t + 4]};
                 uint32_t ah[4], al[4];
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    ah[i] = __float_as_uint(af[i]) & 0xffffe000u;
-                    al[i] = __float_as_uint(af[i] - __uint_as_float(ah[i])) & 0xffffe000u;
-                }
+                for (int i = 0; i < 4; i++) af_tf32_split(af[i], ah[i], al[i]);
 #pragma unroll
                 for (int n = 0; n < kNB; n++) {
                     const int nb = d + n * kDW;
@@ -385,20 +362,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                         const float bf[2] = {sDct[(k0 + t) * p.dctPitch + nb * 8 + g], sDct[(k0 + t + 4) * p.dctPitch + nb * 8 + g]};
                         uint32_t bh[2], bl[2];
 #pragma unroll
-                        for (int i = 0; i < 2; i++) {
-                            bh[i] = __float_as_uint(bf[i]) & 0xffffe000u;
-                            bl[i] = __float_as_uint(bf[i] - __uint_as_float(bh[i])) & 0xffffe000u;
-                        }
+                        for (int i = 0; i < 2; i++) af_tf32_split(bf[i], bh[i], bl[i]);
                         AF_MMA_TF32(acx[n], al[0], al[1], al[2], al[3], bh[0], bh[1]);
                         AF_MMA_TF32(acc[n], ah[0], ah[1], ah[2], ah[3], bh[0], bh[1]);
                         AF_MMA_TF32(acx[n], ah[0], ah[1], ah[2], ah[3], bl[0], bl[1]);
                     }
                 }
             }
-#undef AF_MMA_TF32
             __syncwarp();
             if (lane == 0) af_mbar_arrive(&lEmpty[lbuf]);          // the bank warps may refill this log-mel tile
-            if (d == 0) bulk_wait_read0();                         // the previous tile's bulk stores have read the staging tile
+            if (d == 0) af_bulk_wait_read0();                         // the previous tile's bulk stores have read the staging tile
             named_bar_sync(2, kDW * 32);
             // C fragment: rows g and g+8, columns nb*8 + 2t, +1 -> dense staging tile [nf][ccNum]
 #pragma unroll
@@ -417,15 +390,15 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                     if (c + 1 < p.ccNum) stage[(g + 8) * p.ccNum + c + 1] = v3;
                 }
             }
-            fence_proxy_async_smem();
+            af_fence_proxy_async_smem();
             named_bar_sync(4, kDW * 32);                           // the result tile is staged
             // ---- the tile leaves: destination 0 is this GPU's buffer, 1..nPeer the peers' gathered arrays (NVLink) ----
             const long long tileOff = ((long long)clip * p.timeLength + f0) * p.ccNum;
             if (p.bulkStore) {
                 if (d == 0 && lane <= p.nPeer) {                   // one destination per lane, the whole tile at once
                     float *o = (lane == 0 ? p.out : p.peerOut[lane - 1]) + tileOff;
-                    bulk_store(o, stage, (uint32_t)(nf * p.ccNum * 4));
-                    bulk_commit();
+                    af_bulk_store(o, stage, (uint32_t)(nf * p.ccNum * 4));
+                    af_bulk_commit();
                 }
             } else {
                 const int n = nf * p.ccNum;
@@ -436,7 +409,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 named_bar_sync(2, kDW * 32);                       // staging tile read before the next tile's fragments land
             }
         }
-        if (d == 0) bulk_wait0();
+        if (d == 0) af_bulk_wait0();
         return;
     }
 
@@ -686,7 +659,7 @@ int plan_pieces(int num, const unsigned *desc /* num + 2 */, PiecePlan *pp) {
 
 }  // namespace
 
-extern "C" int af_mfcc2_supported(int fftLength, int num, int ccNum, const float *bank) {
+int af_mfcc2_supported(int fftLength, int num, int ccNum, const float *bank) {
     if (fftLength != kN || num < 1 || num > kMaxNum || ccNum < 1 || ccNum > 64 || !bank) return 0;
     Intervals *iv = static_cast<Intervals *>(malloc(sizeof(Intervals)));
     float4 *tab = static_cast<float4 *>(malloc(sizeof(float4) * kMaxTab));
@@ -698,16 +671,16 @@ extern "C" int af_mfcc2_supported(int fftLength, int num, int ccNum, const float
     return ok;
 }
 
-extern "C" void af_mfcc2_plan_free(void *plan) { free_plan(static_cast<Plan *>(plan)); }
+void af_mfcc2_plan_free(void *plan) { free_plan(static_cast<Plan *>(plan)); }
 
-extern "C" int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int ccNum, const float *window,
-                                   const float *bank, const float *dct /* ccNum x num */, int dataType) {
+int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int ccNum, const float *window, const float *bank,
+                        const float *dct /* ccNum x num */, int dataType) {
     *planOut = NULL;
     if (!af_mfcc2_supported(fftLength, num, ccNum, bank)) return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC v2 plan: unsupported configuration");
     Plan *pl = static_cast<Plan *>(calloc(1, sizeof(Plan)));
     if (!pl) return AF_ERR_NOMEM;
     pl->num = num; pl->ccNum = ccNum; pl->dataType = dataType;
-    pl->ct = ccNum <= 16 ? 2 : ccNum <= 24 ? 3 : ccNum <= 40 ? 5 : 8;
+    pl->ct = af_mfcc_ct(ccNum);
     int rc = AF_OK;
 
     float2 *wp = static_cast<float2 *>(malloc(sizeof(float2) * 1024));
@@ -745,44 +718,28 @@ extern "C" int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int c
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dTab), pl->tab, sizeof(float4) * (size_t)(pl->tabLen > 0 ? pl->tabLen : 1));
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dDesc), pl->pieceDesc, sizeof(pl->pieceDesc));
     if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dPrefix), pl->piecePrefix, sizeof(pl->piecePrefix));
-
-    // DCT table as the mma B operand: D^T[m][c], row pitch % 32 == 8 -> conflict-free fragment reads
-    const int pitch = pl->ct <= 5 ? 40 : 72;
-    float *dt = static_cast<float *>(calloc((size_t)kMaxNum * pitch, sizeof(float)));
-    for (int m = 0; m < num; m++)
-        for (int c = 0; c < ccNum; c++) dt[(size_t)m * pitch + c] = dct[(size_t)c * num + m];
-    if (rc == AF_OK) rc = af_dev_upload(reinterpret_cast<void **>(&pl->dDct), dt, sizeof(float) * (size_t)kMaxNum * pitch);
-    free(dt);
+    if (rc == AF_OK) rc = af_mfcc_dct_upload(&pl->dDct, dct, num, ccNum, pl->ct);
     if (rc != AF_OK) { free_plan(pl); return rc; }
     *planOut = pl;
     return AF_OK;
 }
 
-static int launch_fused2(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                         int rectifyType, float *out, int nPeer, float *const *peerOut, int rawMel, void *stream) {
+int af_mfcc2_launch(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
+                    int rectifyType, float *out, int nPeer, float *const *peerOut, int rawMel, void *stream) {
     Plan *pl = static_cast<Plan *>(plan);
-    if (!pl) return af_fail(AF_ERR_ARG, "fused MFCC v2: no plan");
-    if (batch <= 0 || timeLength <= 0) return AF_OK;
-    if (slideLength % 4 || dataLength % 4 || (reinterpret_cast<uintptr_t>(data) & 15))
-        return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC needs 16-byte aligned clips and slideLength %% 4 == 0 (TMA bulk copy)");
-    if (nPeer < 0 || nPeer > kMaxPeers || (nPeer > 0 && !peerOut)) return af_fail(AF_ERR_ARG, "fused MFCC: nPeer=%d outside [0, %d]", nPeer, kMaxPeers);
-
     Params *pp = static_cast<Params *>(malloc(sizeof(Params)));     // 24 KB: off the stack
     if (!pp) return AF_ERR_NOMEM;
     memset(pp, 0, sizeof(Params));
     pp->data = data; pp->out = out; pp->winPairs = pl->dWinPairs; pp->tw = pl->dTw; pp->dct = pl->dDct;
     pp->dataStride = dataLength; pp->batch = batch; pp->timeLength = timeLength; pp->hop = slideLength;
     pp->num = pl->num; pp->ccNum = pl->ccNum; pp->rectify = rectifyType; pp->dataType = pl->dataType; pp->rawMel = rawMel;
-    pp->dctPitch = pl->ct <= 5 ? 40 : 72;
+    pp->dctPitch = af_mfcc_dct_pitch(pl->ct);
     pp->nPeer = nPeer;
     for (int d = 0; d < nPeer; d++) pp->peerOut[d] = peerOut[d];
     pp->nPass = pl->nPass; pp->assign = pl->dAssign;
     for (int i = 0; i < kMaxPass; i++) pp->passLen[i] = pl->passLen[i];
     pp->bankTab = pl->dTab; pp->pieceDesc = pl->dDesc; pp->piecePrefix = pl->dPrefix; pp->tabLen = pl->tabLen;
-    const int rowFloats = rawMel ? pl->num : pl->ccNum;
-    int bulk = rowFloats % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-    for (int d = 0; d < nPeer; d++) if (reinterpret_cast<uintptr_t>(peerOut[d]) & 15) bulk = 0;
-    pp->bulkStore = bulk;
+    pp->bulkStore = af_mfcc_bulk_store_ok(rawMel ? pl->num : pl->ccNum, out, nPeer, peerOut);
 
     // shared-memory carve-up: as many frames per tile as fit (<= kFW), two TMA stages when they fit, else one
     const int budget = 227 * 1024;
@@ -815,37 +772,10 @@ static int launch_fused2(void *plan, const float *data, int dataLength, int batc
     pp->tilesPerClip = (timeLength + F - 1) / F;
     if ((long long)pp->tilesPerClip * batch >= (1ll << 31)) { free(pp); return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC: more than 2^31 tiles in one launch"); }
     pp->totalTiles = (unsigned)((long long)pp->tilesPerClip * batch);
-
-    int sms = af_sm_count();
-    if (sms <= 0) sms = 132;
-    const long long grid = (long long)pp->totalTiles < (long long)sms ? (long long)pp->totalTiles : (long long)sms;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaSuccess;
-#define AF_MFCC2_LAUNCH(CT_)                                                                                      \
-    e = cudaFuncSetAttribute(k_mfcc_fused2<CT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, total);            \
-    if (e == cudaSuccess) k_mfcc_fused2<CT_><<<(unsigned)grid, kThreads, total, st>>>(*pp)
-    switch (pl->ct) {
-    case 2: AF_MFCC2_LAUNCH(2); break;
-    case 3: AF_MFCC2_LAUNCH(3); break;
-    case 5: AF_MFCC2_LAUNCH(5); break;
-    default: AF_MFCC2_LAUNCH(8); break;
-    }
-#undef AF_MFCC2_LAUNCH
+    static void (*const kernels[4])(Params) = {k_mfcc_fused2<2>, k_mfcc_fused2<3>, k_mfcc_fused2<5>, k_mfcc_fused2<8>};
+    const int launched = af_mfcc_launch_ct(kernels, "k_mfcc_fused2", pl->ct, (long long)pp->totalTiles, kThreads, total, stream, *pp);
     free(pp);
-    if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_mfcc_fused2)");
-    AF_LAUNCH_CHECK("k_mfcc_fused2");
-    return AF_OK;
-}
-
-extern "C" int af_launch_mfcc2(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                               int rectifyType, float *out, int nPeer, float *const *peerOut, void *stream) {
-    return launch_fused2(plan, data, dataLength, batch, timeLength, slideLength, rectifyType, out, nPeer, peerOut, 0, stream);
-}
-
-// same kernel stopped after the filter bank: out[batch][T][num] = bank . |X|^2 (or |X|), i.e. bftObj_bft in real mode
-extern "C" int af_launch_mel2(void *plan, const float *data, int dataLength, int batch, int timeLength, int slideLength,
-                              float *out, void *stream) {
-    return launch_fused2(plan, data, dataLength, batch, timeLength, slideLength, 0, out, 0, NULL, 1, stream);
+    return launched;
 }
 
 // Diagnostic / test hook (host only): the interval form the planner derives from a bank [num][1025], its cut into pieces

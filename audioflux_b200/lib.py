@@ -13,8 +13,8 @@ from . import capi
 
 _HERE = os.path.dirname(os.path.realpath(__file__))
 LIB_NAME = "libaudioflux_b200.so"
-# AFB200_LIB_PATH: another build of the SAME library (sanitizer build of the host code, tools/asan_host_check.sh; kernel
-# variants, tools/sweep_variants.py) -- never a different implementation: there is no CPU fallback to select
+# AFB200_LIB_PATH: another build of the SAME library (sanitizer build of the host code, tools/asan_host_check.sh) --
+# never a different implementation: there is no CPU fallback to select
 LIB_PATH = os.environ.get("AFB200_LIB_PATH") or os.path.join(_HERE, "lib", LIB_NAME)
 
 __LIBRARY = {"lib": None, "present": None}

@@ -80,7 +80,7 @@ int afb200_peerFree(void *devPtr);
 int afb200_ipcGetHandle(void *devPtr, void *handle64);
 int afb200_ipcOpenHandle(const void *handle64, void **devPtr);
 int afb200_ipcCloseHandle(void *devPtr);
-/* diagnostics, after a bftObj_mfccBatch call: 0: the v1 fused kernel serves this object, -1: it does not */
+/* diagnostics: the kernel that served the object's last bftObj_mfccBatch call: 1 fused v2, 0 fused v1, -1 composed (or none yet) */
 int bftObj_mfccPlanMode(BFTObj bftObj);
 int bftObj_getFilterBankArr(BFTObj bftObj, float *bank /* num x (fftLength/2+1) host */);
 /* in: rows x num; out: rows x ccNum */

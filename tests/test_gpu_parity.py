@@ -239,16 +239,18 @@ def test_mfcc_fused_bank_loop_modes(torch_cuda, product_lib, monkeypatch, scale,
     x = np.stack([tones(31, 20480, sr), noise(32, 20480)])
     xd = torch.from_numpy(x).cuda()
     cc = min(20, num)
-    outs = {}
+    outs, modes = {}, {}
     for kernel in ("default", "v1"):
         if kernel == "v1":
             monkeypatch.setenv("AFB200_MFCC_KERNEL", "v1")
         b = af.BFT(num, 11, sr, slide_length=512, scale_type=scale, style_type=style, normal_type=norm, data_type=dt)
         outs[kernel] = b.mfcc_batch(xd, cc).cpu().numpy()
-    # -1 = this shape is outside the v1 kernel (composed path); the Slaney mel-128 banks must really run v1
-    assert product_lib.bftObj_mfccPlanMode(b._obj) in (0, -1)
+        modes[kernel] = product_lib.bftObj_mfccPlanMode(b._obj)
+    # 1 = v2, 0 = v1, -1 = this shape is outside the fused kernels (composed path); the Slaney mel-128 banks must
+    # really run v2 by default and v1 under the hook
+    assert modes["default"] in (1, -1) and modes["v1"] in (0, -1) and (modes["default"] == -1) == (modes["v1"] == -1)
     if scale == S.MEL and style == ST.SLANEY and num == 128:
-        assert product_lib.bftObj_mfccPlanMode(b._obj) == 0
+        assert modes == {"default": 1, "v1": 0}
     lo, hi, _, _ = O.bft_revise_range(num, 2048, sr, None, None, af.enum_value(scale), 12)
     bank, _, _ = O.auditory_filterbank(num, 2048, sr, af.enum_value(scale), af.enum_value(style), af.enum_value(norm),
                                        float(lo), float(hi), 12)

@@ -31,17 +31,17 @@ def nvcc_path():
 
 
 def compile_cubin(src, nvcc, out_dir):
-    cubin = os.path.join(out_dir, "mfcc_fused2.cubin")
+    cubin = os.path.join(out_dir, os.path.splitext(os.path.basename(src))[0] + ".cubin")
     r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-cubin",
                         "-Xptxas", "-v", "-o", cubin, src], capture_output=True, text=True, check=True)
     return cubin, r.stderr
 
 
-def ptxas_report(log):
-    """{CT: (registers, spill store bytes, spill load bytes)} from the -Xptxas -v log."""
+def ptxas_report(log, kernel="k_mfcc_fused2"):
+    """{CT: (registers, spill store bytes, spill load bytes)} of kernel<CT> from the -Xptxas -v log."""
     rep, ct = {}, None
     for line in log.splitlines():
-        m = re.search(r"k_mfcc_fused2ILi(\d+)E", line)
+        m = re.search(kernel + r"ILi(\d+)E", line)
         if "Compiling entry function" in line:
             ct = int(m.group(1)) if m else None
             continue

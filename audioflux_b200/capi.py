@@ -267,6 +267,21 @@ CEPSTROGRAM_API = {
     "cepstrogramObj_cepstrogram2Batch": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]),
 }
 
+# resampler (src/dsp/resample_algorithm.h, include/afb200_resample.h) and the additive batched entry point
+# (include/afb200_ext.h)
+RESAMPLE_API = {
+    "resampleObj_new": (C.c_int, [P(vp), c_int_p, c_int_p, c_int_p]),
+    "resampleObj_newWithWindow": (C.c_int, [P(vp), c_int_p, c_int_p, c_int_p, c_float_p, c_float_p, c_int_p, c_int_p]),
+    "resampleObj_calDataLength": (C.c_int, [vp, C.c_int]),
+    "resampleObj_setSamplate": (None, [vp, C.c_int, C.c_int]),
+    "resampleObj_setSamplateRatio": (None, [vp, C.c_float]),
+    "resampleObj_enableContinue": (None, [vp, C.c_int]),
+    "resampleObj_resample": (C.c_int, [vp, vp, C.c_int, vp]),
+    "resampleObj_free": (None, [vp]),
+    "resampleObj_debug": (None, [vp]),
+    "resampleObj_resampleBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -281,7 +296,7 @@ REFERENCE_BUILDERS = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -67,6 +67,11 @@ typedef int (*AfChunkFn)(void *ctx, int nb, float *const *d, void *stream);
 int af_run_batch(AfPipe *pipe, int memKind, void *stream, AfChunkFn fn, void *ctx, const AfPlane *planes, int nPlanes,
                  int batch, size_t chunkBytes);
 void af_pipe_free(AfPipe *pipe);
+/* host-side ordering of a table rebuild after the kernels that read the old table: *ev records the end of the last
+ * launch on `stream` (created on first use); af_fence_wait blocks until it has passed (no-op when NULL) */
+int af_fence_record(void **ev, void *stream);
+int af_fence_wait(void *ev);
+void af_fence_free(void *ev);
 
 /* streaming bookkeeping shared by STFT, CQT and SpectrogramObj (stft_algorithm.c:474-599, cqt_algorithm.c:346-456):
  * the samples that did not complete a hop are carried to the next call */
@@ -406,6 +411,21 @@ typedef struct {
     float *cep, *env, *det;       /* device, frames x (N/2+1) each, or NULL */
 } AfCepsArgs;
 int af_launch_cepstrogram(const AfCepsArgs *a, void *stream);
+
+/* Resampler (kernels/resample.cu), one launch per call: out[b][i] for i < outLen of every clip b of `data` (batch x inLen),
+ * the windowed-sinc sum of src/dsp/resample_algorithm.c:430-521 in its order and rounding; the sum starts from out[b][i]
+ * when `accumulate` (the legacy call adds into the caller's buffer), else from 0, and is divided by `scaleDiv` when it is
+ * not 0.  `table` holds the float32 table (tableLength floats); the weight of entry o is
+ * table[o] + delta * (table[o+1] - table[o]), with 0 for the last entry's difference.  Taps read x[0 .. srcLen-1];
+ * left-tap positions at or beyond inLen read 0. */
+typedef struct {
+    const float *data, *table;
+    float *out;
+    int inLen, srcLen, outLen, batch, tableLength, bitLength, step;
+    float ratio, scale, scaleDiv;
+    int accumulate;
+} AfResampleArgs;
+int af_launch_resample(const AfResampleArgs *a, void *stream);
 
 void af_count_launch(int n);
 

@@ -210,6 +210,14 @@ int af_run_batch(AfPipe *pp, int memKind, void *stream, AfChunkFn fn, void *ctx,
     return af_cuda_check(e1 ? e1 : e2 ? e2 : e3, "cudaStreamSynchronize");
 }
 
+int af_fence_record(void **ev, void *stream) {
+    int rc;
+    if (!*ev && (rc = af_event_create(ev))) return rc;
+    return af_event_record(*ev, stream);
+}
+int af_fence_wait(void *ev) { return ev ? af_cuda_check(cudaEventSynchronize((cudaEvent_t)ev), "cudaEventSynchronize") : AF_OK; }
+void af_fence_free(void *ev) { af_event_destroy(ev); }
+
 void af_pipe_free(AfPipe *pp) {
     af_stream_destroy(pp->stream); af_stream_destroy(pp->inStream); af_stream_destroy(pp->outStream);
     for (int s = 0; s < 2; s++) {

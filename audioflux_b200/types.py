@@ -122,5 +122,12 @@ class WaveletContinueType(Enum):
     RICKER = 7
 
 
+class ResampleQualityType(Enum):
+    """src/dsp/resample_algorithm.h"""
+    BEST = 0
+    MID = 1
+    FAST = 2
+
+
 def enum_value(v):
     return int(v.value) if isinstance(v, Enum) else int(v)

@@ -26,6 +26,7 @@
 #include "afb200_nsgt.h"
 #include "afb200_st.h"
 #include "afb200_cepstrogram.h"
+#include "afb200_resample.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -199,6 +200,13 @@ int cepstrogramObj_cepstrogramBatch(CepstrogramObj cepstrogramObj, int cepNum, c
  * The planes are read only.  Each row's result is bit-identical to cepstrogramObj_cepstrogram2 on that row. */
 int cepstrogramObj_cepstrogram2Batch(CepstrogramObj cepstrogramObj, int cepNum, const float *mReal, const float *mImag,
                                      int rows, int specWidth, float *cep, float *env, float *det, int memKind, void *stream);
+
+/* resampler of a batch: data batch x dataLength -> out batch x resampleObj_calDataLength(dataLength); out is overwritten.
+ * Each clip's result is bit-identical to resampleObj_resample on that clip into a zeroed buffer, whatever the batch.
+ * Refused while the object is in continue mode (a mode for one stream fed chunk by chunk through resampleObj_resample),
+ * and wherever resampleObj_resample refuses.  One kernel launch per staging chunk. */
+int resampleObj_resampleBatch(ResampleObj resampleObj, const float *data, int dataLength, int batch, float *out,
+                              int memKind, void *stream);
 
 #ifdef __cplusplus
 }

@@ -1,8 +1,8 @@
 """audioflux_b200: H100-native (sm_90a) drop-in for audioFlux's time-frequency hot path.
 
 Host-side mirror of the reference's operator interface (same class / method / argument
-names as python/audioflux/{stft,bft,cqt,cwt,nsgt,st,fst,cepstrogram,spectrogram}.py, feature/xxcc.py and
-dsp/resample.py) over the C-ABI
+names as python/audioflux/{stft,bft,cqt,cwt,nsgt,st,fst,cepstrogram,spectrogram}.py, feature/xxcc.py,
+dsp/resample.py and mir/hpss.py) over the C-ABI
 library ``lib/libaudioflux_b200.so``.  No CPU fallback exists.
 """
 from .types import *  # noqa: F401,F403
@@ -20,6 +20,7 @@ from .nsgt import NSGT  # noqa: F401
 from .st import ST, FST  # noqa: F401
 from .cepstrogram import Cepstrogram  # noqa: F401
 from .resample import Resample, WindowResample  # noqa: F401
+from .hpss import HPSS  # noqa: F401
 from . import lib  # noqa: F401
 
 __version__ = "0.1.0"

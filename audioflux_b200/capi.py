@@ -282,6 +282,17 @@ RESAMPLE_API = {
     "resampleObj_resampleBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
 }
 
+# harmonic-percussive separation (include/mir/hpss_algorithm.h, include/afb200_hpss.h) and the additive batched entry
+# point (include/afb200_ext.h)
+HPSS_API = {
+    "hpssObj_new": (C.c_int, [P(vp), C.c_int, c_int_p, c_int_p, c_int_p, c_int_p]),
+    "hpssObj_calDataLength": (C.c_int, [vp, C.c_int]),
+    "hpssObj_hpss": (None, [vp, vp, C.c_int, vp, vp]),
+    "hpssObj_free": (None, [vp]),
+    "hpssObj_debug": (None, [vp]),
+    "hpssObj_hpssBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -296,7 +307,7 @@ REFERENCE_BUILDERS = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

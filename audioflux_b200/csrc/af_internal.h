@@ -72,6 +72,9 @@ void af_pipe_free(AfPipe *pipe);
 int af_fence_record(void **ev, void *stream);
 int af_fence_wait(void *ev);
 void af_fence_free(void *ev);
+/* clips per group of a device workspace of perClip bytes per clip: a quarter of the free memory, at most cap bytes,
+ * at least one clip and at most `batch` */
+int af_chunk_clips(size_t perClip, size_t cap, int batch);
 
 /* streaming bookkeeping shared by STFT, CQT and SpectrogramObj (stft_algorithm.c:474-599, cqt_algorithm.c:346-456):
  * the samples that did not complete a hop are carried to the next call */
@@ -426,6 +429,17 @@ typedef struct {
     int accumulate;
 } AfResampleArgs;
 int af_launch_resample(const AfResampleArgs *a, void *stream);
+
+/* Masks of harmonic-percussive separation (kernels/hpss.cu), one launch: from the half-spectrum planes re / im
+ * [clips * timeLength][width] the masked planes of H (hRe / hIm) and P (pRe / pIm) in the same layout, either pair NULL
+ * to skip it.  Medians over hOrder frames of one clip (zeros beyond its first and last frame) and over pOrder bins (zeros
+ * beyond the plane), orders odd, 1 .. AFB200_HPSS_MAX_ORDER; an order of 1 gives a median of 0. */
+typedef struct {
+    const float *re, *im;
+    float *hRe, *hIm, *pRe, *pIm;
+    int clips, timeLength, width, hOrder, pOrder;
+} AfHpssArgs;
+int af_launch_hpss_mask(const AfHpssArgs *a, void *stream);
 
 void af_count_launch(int n);
 

@@ -202,16 +202,6 @@ static int bft_plan(BFTObj b, AfMfccPlan **slot, int kernel, int ccNum) {
     return rc;
 }
 
-/* clips per chunk of a device workspace of perClip bytes per clip: a quarter of the free memory, at most cap bytes */
-static int bft_chunk_clips(size_t perClip, size_t cap, int batch) {
-    size_t budget = af_dev_free_bytes() / 4;
-    if (budget < perClip) budget = perClip;
-    if (budget > cap) budget = cap;
-    int chunk = (int)(budget / perClip);
-    if (chunk < 1) chunk = 1;
-    return chunk > batch ? batch : chunk;
-}
-
 /* device-resident compute: dData [batch x dataLength] -> dRe (and, complex mode, dIm) [batch x T x num] */
 static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, float *dRe, float *dIm, int realMode, void *st) {
     const int T = bftObj_calTimeLength(b, dataLength);
@@ -229,7 +219,7 @@ static int bft_compute(BFTObj b, const float *dData, int dataLength, int batch, 
     const int count = b->highIndex - b->lowIndex + 1 < b->num ? b->highIndex - b->lowIndex + 1 : b->num;
     /* the spectrum workspace is bounded: process the batch in chunks of clips */
     const size_t perClip = sizeof(float) * (size_t)T * width;
-    const int chunk = bft_chunk_clips(perClip, (size_t)3 << 30, batch);
+    const int chunk = af_chunk_clips(perClip, (size_t)3 << 30, batch);
     if ((rc = af_devbuf_reserve(&b->dSpecRe, perClip * chunk))) return rc;
     if (!realMode && (rc = af_devbuf_reserve(&b->dSpecIm, perClip * chunk))) return rc;
     for (int c0 = 0; c0 < batch; c0 += chunk) {
@@ -337,7 +327,7 @@ int af_bft_spectrogram(BFTObj b, const float *dData, int dataLength, int batch, 
     if (rc || !dPhase) return rc;
     const int T = bftObj_calTimeLength(b, dataLength), width = b->fftLength / 2 + 1;
     const size_t perClip = sizeof(float) * (size_t)T * width;
-    const int chunk = bft_chunk_clips(perClip, (size_t)2 << 30, batch);
+    const int chunk = af_chunk_clips(perClip, (size_t)2 << 30, batch);
     if ((rc = af_devbuf_reserve(&b->dSpecRe, perClip * chunk)) || (rc = af_devbuf_reserve(&b->dSpecIm, perClip * chunk))) return rc;
     for (int c0 = 0; c0 < batch; c0 += chunk) {
         const int nb = batch - c0 < chunk ? batch - c0 : chunk;

@@ -210,6 +210,15 @@ int af_run_batch(AfPipe *pp, int memKind, void *stream, AfChunkFn fn, void *ctx,
     return af_cuda_check(e1 ? e1 : e2 ? e2 : e3, "cudaStreamSynchronize");
 }
 
+int af_chunk_clips(size_t perClip, size_t cap, int batch) {
+    size_t budget = af_dev_free_bytes() / 4;
+    if (budget < perClip) budget = perClip;
+    if (budget > cap) budget = cap;
+    int chunk = (int)(budget / perClip);
+    if (chunk < 1) chunk = 1;
+    return chunk > batch ? batch : chunk;
+}
+
 int af_fence_record(void **ev, void *stream) {
     int rc;
     if (!*ev && (rc = af_event_create(ev))) return rc;

@@ -27,6 +27,7 @@
 #include "afb200_st.h"
 #include "afb200_cepstrogram.h"
 #include "afb200_resample.h"
+#include "afb200_hpss.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -207,6 +208,15 @@ int cepstrogramObj_cepstrogram2Batch(CepstrogramObj cepstrogramObj, int cepNum, 
  * and wherever resampleObj_resample refuses.  One kernel launch per staging chunk. */
 int resampleObj_resampleBatch(ResampleObj resampleObj, const float *data, int dataLength, int batch, float *out,
                               int memKind, void *stream);
+
+/* harmonic-percussive separation of a batch: data batch x dataLength -> h and p, each batch x
+ * hpssObj_calDataLength(dataLength), both overwritten.  Either output may be NULL (its inverse STFT is skipped), not
+ * both.  Each clip's result is bit-identical to hpssObj_hpss on that clip into zeroed buffers, whatever the batch.
+ * Refused wherever hpssObj_hpss refuses.  The device workspace (six half-spectrum planes and the inverse STFT's frames)
+ * is bounded by processing the clips in groups; per group, up to fftLength 2^14: one STFT launch, one mask launch and
+ * two inverse STFT launches per requested output. */
+int hpssObj_hpssBatch(HPSSObj hpssObj, const float *data, int dataLength, int batch, float *h, float *p, int memKind,
+                      void *stream);
 
 #ifdef __cplusplus
 }

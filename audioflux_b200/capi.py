@@ -175,6 +175,7 @@ EXTENSION_API = {
                                             C.c_float, C.c_float, C.c_int, vp, vp, vp]),
     "afb200_decimatorTaps": (C.c_int, [vp, vp]),
     "afb200_mfccBankPlan2": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
+    "afb200_mfccCarve2": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]),
     "afb200_chromaCqtFilterBank": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_float, vp]),
 }
 

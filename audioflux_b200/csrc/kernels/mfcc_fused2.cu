@@ -39,17 +39,28 @@ constexpr int kBW = 4;              // filter-bank warps (one interval per lane)
 constexpr int kDW = 2;              // DCT (tensor-core) + store warps, one tile behind the bank warps
 constexpr int kEW = kBW;                        // (planner: helper lanes that walk intervals)
 constexpr int kThreads = (kFW + 1 + kBW + kDW) * 32;  // + producer / special-column warp: 20 warps at <= 96 registers
+// Warp roles.  Warps w and w + 4 issue from the same SM sub-partition, so frame warps 0..12 put four frames on the
+// sub-partition of warp 16 and three on each of the others.  Warp 16 is a DCT warp: the DCT warps issue the fewest
+// instructions per tile (dependent tensor-core steps, not FP32 work).  No bank warp, the critical path, shares a
+// sub-partition with four frames: the producer is warp 13, the bank warps 14, 15, 17 and 18, the other DCT warp 19.
+constexpr int kProducerWarp = 13;
+__device__ __forceinline__ int bank_warp_index(int warp) { return warp >= 14 && warp <= 18 && warp != 16 ? warp - 14 - (warp > 16) : -1; }
+__device__ __forceinline__ int dct_warp_index(int warp) { return warp == 16 || warp == 19 ? (warp - 16) / 3 : -1; }
 constexpr int kMaxNum = 128;
 constexpr int kLPitch = 132;        // log-mel tile row pitch (floats): 4g + t -> 32 distinct banks for mma A fragments
 constexpr int kMaxTab = 1408;       // bank table entries (one float4 per bin pair of an interval) in the parameter block
 constexpr int kMaxPieces = 256;     // pieces the intervals may be cut into (slots = rows of the power tile)
 constexpr int kMaxPass = kMaxPieces / (kEW * 32);   // bank passes: one piece per helper lane and pass
 constexpr int kSpecPitch = 17;      // c64 slots per n2 row of the special-column buffer (odd -> conflict-free both ways)
-constexpr int kScratchFloats = 33 * 32;
-constexpr int kTrPitch = 34;        // transpose rows (floats): 34 % 32 == 2 -> 16 lanes' float2 reads hit 16 bank pairs
-static_assert(31 * kTrPitch <= kScratchFloats, "31 transpose rows fit the frame warp's scratch");
 constexpr int kPitchPairs = kFW | 1;   // power-tile row pitch (frames): odd -> conflict-free column walks; always kFW wide
-constexpr int kBarBytes = 128;      // 12 mbarriers at the start of shared memory (128 keeps the TMA span aligned)
+constexpr int kTileFloats = kPairs * kPitchPairs * 2;   // one power tile; there are two, used by alternate tiles
+// Stage C transposes through frame w's own column of the power tile (float2 slot 13 s + w, s < 513), which is free from
+// the bank's release of the buffer until the frame's power stores.  Element pair j = n2 / 2 of plane row r = k1 - 1
+// sits at slot s = r + 31 j: the writers' 32-bit stores hit words 26 r + 6 j + 2 w + (n2 & 1) (mod 32), 32 banks; the
+// readers' float2 loads hit bank pairs 13 r + 13 * 31 j + w (mod 16), 16 per half-warp.  Both: one wavefront.
+constexpr int kTrRows = 31;
+static_assert(kPitchPairs == 13 && (kTrRows - 1) + kTrRows * 15 < kPairs, "the transpose slot map fits a power-tile column");
+constexpr int kBarBytes = 128;      // 16 mbarriers at the start of shared memory (128 keeps the TMA span aligned)
 constexpr int kTwRows = 31;         // stage-D twiddles W_2048^(n2 k1) = g (1 - i t), n2 = 1..31 (row n2 - 1), lane k1
 
 struct Plan {
@@ -58,7 +69,7 @@ struct Plan {
     float *dDct;                    // [128 m][dctPitch]
     int num, ccNum, ct, dataType;
     unsigned ivDesc[kMaxNum + 4];   // (first bin pair << 16) | table offset; entries num+1.. = end sentinels
-    int nPass, passLen[kMaxPass];   // bank passes and the longest piece (bin pairs) of each
+    int nPass;                      // bank passes
     int nPieces, lmax, firstPass2;  // pieces 0 .. firstPass2-1 run in pass 0
     unsigned pieceDesc[kMaxPieces];                  // (first bin pair << 20) | (pairs << 16) | table offset
     unsigned short piecePrefix[kMaxNum + 4];         // first piece of interval i; [num + 1 ..] = nPieces
@@ -81,8 +92,8 @@ struct Params {
     int num, ccNum, rectify, dataType, rawMel, bulkStore, dctPitch;
     int nPeer;
     float *peerOut[kMfccMaxPeers];
-    int offSpan, offScratch, offP, offWin, offTw, offSpec, offDct, offL, offStage, offTab, offDesc, offAssign, offPrefix, stageBytes;   // offL: two log-mel tiles
-    int nPass, passLen[kMaxPass];
+    int offSpan, offP, offWin, offTw, offSpec, offDct, offL, offStage, offTab, offDesc, offAssign, offPrefix, stageBytes;   // offL: two log-mel tiles
+    int nPass;
     const unsigned short *assign;
     int tabLen;
     const float4 *bankTab;          // [tabLen] (rise[2q], rise[2q+1], fall[2q], fall[2q+1]) per bin pair of an interval
@@ -98,8 +109,7 @@ template <int CT>
 __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_constant__ Params p) {
     extern __shared__ __align__(128) unsigned char smem[];
     float *span = reinterpret_cast<float *>(smem + p.offSpan);
-    float *scratchAll = reinterpret_cast<float *>(smem + p.offScratch);
-    float *sP = reinterpret_cast<float *>(smem + p.offP);                 // [kPairs][kPitchPairs][2]
+    float *sP = reinterpret_cast<float *>(smem + p.offP);                 // [2][kPairs][kPitchPairs][2]
     float2 *sWin = reinterpret_cast<float2 *>(smem + p.offWin);
     float2 *sTw = reinterpret_cast<float2 *>(smem + p.offTw);
     c64 *sSpec = reinterpret_cast<c64 *>(smem + p.offSpec);               // [2][32 n2][kSpecPitch]
@@ -109,10 +119,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     uint64_t *fullBar = reinterpret_cast<uint64_t *>(smem);               // [2] TMA landed (barriers at offset 0: fixed addresses)
     uint64_t *emptyBar = fullBar + 2;                                     // [2] frame warps took their samples
     uint64_t *specFull = fullBar + 4;                                     // [2] special columns of a tile stored
-    uint64_t *pFull = fullBar + 6;                                        // power-spectrum tile complete
-    uint64_t *pEmpty = fullBar + 7;                                       // bank done with it
-    uint64_t *lFull = fullBar + 8;                                        // [2] log-mel tile written by the bank warps
-    uint64_t *lEmpty = fullBar + 10;                                      // [2] ... consumed by the DCT warps
+    uint64_t *pFull = fullBar + 6;                                        // [2] power-spectrum tile complete
+    uint64_t *pEmpty = fullBar + 8;                                       // [2] bank done with it
+    uint64_t *cDone = fullBar + 10;                                       // [2] frame warps' transposes read out of it
+    uint64_t *lFull = fullBar + 12;                                       // [2] log-mel tile written by the bank warps
+    uint64_t *lEmpty = fullBar + 14;                                      // [2] ... consumed by the DCT warps
     float4 *sTab = reinterpret_cast<float4 *>(smem + p.offTab);           // interval-form bank weights
     unsigned *sDesc = reinterpret_cast<unsigned *>(smem + p.offDesc);
     unsigned short *sAssign = reinterpret_cast<unsigned short *>(smem + p.offAssign);
@@ -128,8 +139,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     for (int i = threadIdx.x; i < kMaxPieces; i += kThreads) sDesc[i] = p.pieceDesc[i];
     for (int i = threadIdx.x; i < kMaxNum + 4; i += kThreads) sPrefix[i] = p.piecePrefix[i];
     for (int i = threadIdx.x; i < kMaxPass * kEW * 32; i += kThreads) sAssign[i] = p.assign[i];
-    for (int i = threadIdx.x; i < kFW * kScratchFloats; i += kThreads) scratchAll[i] = 0.0f;
-    for (int i = threadIdx.x; i < kPairs * pitch * 2; i += kThreads) sP[i] = 0.0f;
+    for (int i = threadIdx.x; i < 2 * kTileFloats; i += kThreads) sP[i] = 0.0f;
     for (int i = threadIdx.x; i < 2 * 32 * kSpecPitch; i += kThreads) sSpec[i] = 0ull;
     for (int i = threadIdx.x; i < 2 * 16 * kLPitch; i += kThreads) sL[i] = 0.0f;
     if (!p.rawMel)
@@ -140,17 +150,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
             af_mbar_init(&fullBar[s], 1);
             af_mbar_init(&emptyBar[s], kFW);
             af_mbar_init(&specFull[s], kFW);
+            af_mbar_init(&pFull[s], kFW + 1);
+            af_mbar_init(&pEmpty[s], kBW);
+            af_mbar_init(&cDone[s], kFW);
+            af_mbar_init(&lFull[s], kBW);
+            af_mbar_init(&lEmpty[s], kDW);
         }
-        af_mbar_init(pFull, kFW + 1);
-        af_mbar_init(pEmpty, kBW);
-        for (int s = 0; s < 2; s++) { af_mbar_init(&lFull[s], kBW); af_mbar_init(&lEmpty[s], kDW); }
         af_fence_barrier_init();
     }
     __syncthreads();
 
     const int F = p.framesPerTile;
 
-    if (warp == kFW) {
+    if (warp == kProducerWarp) {
         // ================= producer (TMA) + special columns k1 = 0 / 32 of every frame of the tile =================
         const int S = p.stages;
         auto issue = [&](unsigned tile, int stage) {
@@ -194,9 +206,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 if (n2 >= 16 && kind) u[n2] = c_mul_mi(u[n2]);                        // W_64^16 = -i
             }
             af_fft32_fma(u);
-            af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);                   // bank done with the previous tile
+            af_mbar_wait(&cDone[sb], (uint32_t)(it >> 1) & 1u);          // the frames' transposes are out of these columns
             if (f < nf) {
-                float *dst = sP + 2 * f + (kind ? 32 * pitch : 0);                    // bin 64 k2 + 32 kind -> pair 32 k2 + 16 kind
+                float *dst = sP + sb * kTileFloats + 2 * f + (kind ? 32 * pitch : 0);   // bin 64 k2 + 32 kind -> pair 32 k2 + 16 kind
 #pragma unroll
                 for (int k2 = 0; k2 < 16; k2++) {
                     float pw = c_norm2_fma(u[AF_BR5(k2)]);
@@ -210,49 +222,47 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 }
             }
             __syncwarp();
-            if (lane == 0) af_mbar_arrive(pFull);
+            if (lane == 0) af_mbar_arrive(&pFull[sb]);
         }
         return;
     }
 
-    if (warp > kFW && warp <= kFW + kBW) {
+    if (bank_warp_index(warp) >= 0) {
         // ================= bank warps: interval-form filter bank over the whole tile =================
-        const int e = warp - (kFW + 1);
+        const int e = bank_warp_index(warp);
         const int rowFloats = p.num;
         int it = 0;
         for (unsigned tile = blockIdx.x; tile < p.totalTiles; tile += gridDim.x, ++it) {
-            const int lbuf = it & 1;
-            af_mbar_wait(pFull, (uint32_t)it & 1u);
+            const int lbuf = it & 1;                               // (power tile and log-mel tile alike)
+            float *P = sP + lbuf * kTileFloats;
+            af_mbar_wait(&pFull[lbuf], (uint32_t)(it >> 1) & 1u);
             if (!p.rawMel) af_mbar_wait(&lEmpty[lbuf], ((uint32_t)(it >> 1) & 1u) ^ 1u);    // DCT done with tile it - 2
             // ---- phase 1: ONE PIECE (<= Lmax bin pairs of one interval) PER LANE AND PASS, all frames of the tile in
             // registers: one LDS.128 of weights (rise of filter i, fall of filter i-1) and, per frame, one LDS.64 of the
             // power pair + two complex-pair FMAs -- kFW independent accumulator chains per lane.  Pass 0 walks the low rows of the
             // power tile, pass 1 the rest; once every helper warp is through a pass the rows it read are dead and take
             // the pieces' partial sums S[piece][frame] = (rise part, fall part), piece index = row index.
-            c64 *sS = reinterpret_cast<c64 *>(sP);
+            c64 *sS = reinterpret_cast<c64 *>(P);
             for (int ps = 0; ps < p.nPass; ps++) {
                 const unsigned piece = sAssign[(ps * kBW + e) * 32 + lane];
                 const bool have = piece != 0xffffu;
                 const unsigned d0 = sDesc[have ? piece : 0];
                 const int len = have ? (int)((d0 >> 16) & 15u) : 0;
                 const float4 *wt = sTab + (d0 & 0xffffu);
-                const c64 *q = reinterpret_cast<const c64 *>(sP) + (size_t)(d0 >> 20) * pitch;
+                const c64 *q = reinterpret_cast<const c64 *>(P) + (size_t)(d0 >> 20) * pitch;
                 c64 aR[kFW], aF[kFW];
 #pragma unroll
                 for (int f = 0; f < kFW; f++) { aR[f] = 0ull; aF[f] = 0ull; }
-                const int maxLen = p.passLen[ps];
-                for (int j = 0; j < maxLen; j++) {
-                    if (j < len) {
-                        const float4 w = wt[j];
-                        const c64 wr = c_pack(w.x, w.y), wf = c_pack(w.z, w.w);
+                for (int j = 0; j < len; j++) {
+                    const float4 w = wt[j];
+                    const c64 wr = c_pack(w.x, w.y), wf = c_pack(w.z, w.w);
 #pragma unroll
-                        for (int f = 0; f < kFW; f++) {
-                            const c64 v = q[f];
-                            aR[f] = v_fma(v, wr, aR[f]);
-                            aF[f] = v_fma(v, wf, aF[f]);
-                        }
-                        q += pitch;
+                    for (int f = 0; f < kFW; f++) {
+                        const c64 v = q[f];
+                        aR[f] = v_fma(v, wr, aR[f]);
+                        aF[f] = v_fma(v, wf, aF[f]);
                     }
+                    q += pitch;
                 }
                 named_bar_sync(3, kBW * 32);                   // every helper warp has read this pass's rows
                 if (have) {
@@ -295,7 +305,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
                 }
             }
             __syncwarp();
-            if (lane == 0) af_mbar_arrive(pEmpty);                 // frame warps may overwrite the power tile (and the sums in it)
+            if (lane == 0) af_mbar_arrive(&pEmpty[lbuf]);          // frame warps may overwrite the power tile (and the sums in it)
             if (m < p.num) {
 #pragma unroll
                 for (int f = 0; f < kFW; f++) {
@@ -325,10 +335,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         return;
     }
 
-    if (warp > kFW + kBW) {
+    if (dct_warp_index(warp) >= 0) {
         // ================= DCT warps: ortho DCT-II of the log-mel tile on the tensor cores, then the tile leaves =================
         if (p.rawMel) return;
-        const int d = warp - (kFW + 1 + kBW);
+        const int d = dct_warp_index(warp);
         const int g = lane >> 2, t = lane & 3;
         constexpr int kNB = (CT + kDW - 1) / kDW;                  // n-blocks of the DCT per warp
         float *stage = sStage;
@@ -414,13 +424,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
     }
 
     // ================= frame warps: warp w transforms frame f0 + w of every tile =================
-    float *scratch = scratchAll + (size_t)warp * kScratchFloats;
     const c64 *sWinC = reinterpret_cast<const c64 *>(sWin);
     const c64 *sTwC = reinterpret_cast<const c64 *>(sTw);
-    // power-tile addresses (floats): bin = lane + 64 k2 (k2 < 16) and 64 (32 - k2) - lane (k2 >= 16)
+    // addresses (floats) in this frame's column: power of bin = lane + 64 k2 (k2 < 16) and 64 (32 - k2) - lane (k2 >= 16);
+    // transposes: lane n2 writes pair n2 / 2 of every row, lane k1 reads row k1 - 1 (lane 0 has no column: it reads
+    // row 0 with lane 1, and its spectrum is never stored)
     const int strideK2 = 64 * pitch;
-    const int offLo = (lane >> 1) * (2 * pitch) + 2 * warp + (lane & 1);
-    const int offHi = -((lane + 1) >> 1) * (2 * pitch) + 2 * warp + (lane & 1);
+    const int offLo = (lane >> 1) * (2 * pitch) + (lane & 1);
+    const int offHi = -((lane + 1) >> 1) * (2 * pitch) + (lane & 1);
+    const int trWrite = (lane >> 1) * (kTrRows * 2 * pitch) + (lane & 1);
+    const int trRead = (lane ? lane - 1 : 0) * pitch;
 
     int it = 0, stage = 0;
     uint32_t stagePhase = 0;
@@ -433,7 +446,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         if (tIn >= (unsigned)p.tilesPerClip) tIn -= (unsigned)p.tilesPerClip;
         const int nf = min(F, p.timeLength - f0);
         const bool active = warp < nf;
-        const int sb = it & 1;
+        const int sb = it & 1;                                     // spectrum buffer and power tile of this tile
+        float *col = sP + sb * kTileFloats + 2 * warp;              // this frame's column of the power tile
 
         af_mbar_wait(&fullBar[stage], stagePhase);
 
@@ -448,10 +462,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         if (lane == 0) af_mbar_arrive(&emptyBar[stage]);           // span slot may be refilled
         if (++stage == p.stages) { stage = 0; stagePhase ^= 1u; }
         if (!active) {
-            // keep the tile protocols in step (one arrival per warp per tile and barrier)
-            if (lane == 0) af_mbar_arrive(&specFull[sb]);
-            af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);
-            if (lane == 0) af_mbar_arrive(pFull);
+            // keep the tile protocols in step (one arrival per warp per tile and barrier, after the release of tile it - 2)
+            af_mbar_wait(&pEmpty[sb], ((uint32_t)(it >> 1) & 1u) ^ 1u);
+            if (lane == 0) {
+                af_mbar_arrive(&specFull[sb]);
+                af_mbar_arrive(&cDone[sb]);
+                af_mbar_arrive(&pFull[sb]);
+            }
             continue;
         }
 
@@ -459,59 +476,61 @@ __global__ void __launch_bounds__(kThreads, 1) k_mfcc_fused2(const __grid_consta
         af_fft32_fma_win(z, sWinC + lane);                         // Z[k] at AF_BR5(k)
         // R[k] = (Z[k] + conj Z[32-k]) - i W_64^k (Z[k] - conj Z[32-k]) at AF_BR5(k), (R[0], R[32]) in z[0]
         af_rfft64_post_fma(z);
+        // the bank is done with tile it - 2, so the producer has read that tile's special columns out of this spectrum
+        // buffer, and this frame's column of the power tile is free
+        af_mbar_wait(&pEmpty[sb], ((uint32_t)(it >> 1) & 1u) ^ 1u);
         sSpec[((size_t)sb * 32 + lane) * kSpecPitch + warp] = z[0];
         __syncwarp();
         if (lane == 0) af_mbar_arrive(&specFull[sb]);
 
-        // ---- C: columns k1 = 1..31, 32 x 32 transpose (real plane, then imaginary plane).  Row k1 - 1 of a plane holds
-        // column k1 at pitch kTrPitch: the writers' 32-bit stores are one wavefront, and lane k1 reads its row as 16
-        // float2 (n2, n2 + 1) -- rows 2 apart in banks, so each half-warp's 64-bit loads are one wavefront.  Lane 0 has no
-        // column; it reads row 0 with lane 1 (same addresses) and its spectrum is never stored. ----
+        // ---- C: columns k1 = 1..31, 32 x 32 transpose (real plane, then imaginary plane) through this frame's column
+        // of the power tile (slot map at kTrRows): 32-bit stores, lane k1 reads its row as 16 float2 (n2, n2 + 1). ----
         {
             float yr[32], yi[32];
-            const float2 *row = reinterpret_cast<const float2 *>(scratch + (lane ? lane - 1 : 0) * kTrPitch);
+            float *tw = col + trWrite;
+            const float2 *row = reinterpret_cast<const float2 *>(col) + trRead;
 #pragma unroll
             for (int k1 = 1; k1 < 32; k1++) c_unpack(z[AF_BR5(k1)], yr[k1], yi[k1]);
 #pragma unroll
-            for (int k1 = 1; k1 < 32; k1++) scratch[(k1 - 1) * kTrPitch + lane] = yr[k1];
+            for (int k1 = 1; k1 < 32; k1++) tw[(k1 - 1) * 2 * pitch] = yr[k1];
             __syncwarp();
 #pragma unroll
-            for (int j = 0; j < 16; j++) { const float2 v = row[j]; yr[2 * j] = v.x; yr[2 * j + 1] = v.y; }
+            for (int j = 0; j < 16; j++) { const float2 v = row[j * kTrRows * pitch]; yr[2 * j] = v.x; yr[2 * j + 1] = v.y; }
             __syncwarp();
 #pragma unroll
-            for (int k1 = 1; k1 < 32; k1++) scratch[(k1 - 1) * kTrPitch + lane] = yi[k1];
+            for (int k1 = 1; k1 < 32; k1++) tw[(k1 - 1) * 2 * pitch] = yi[k1];
             __syncwarp();
 #pragma unroll
             for (int j = 0; j < 16; j++) {
-                const float2 v = row[j];
+                const float2 v = row[j * kTrRows * pitch];
                 z[2 * j] = c_pack(yr[2 * j], v.x);
                 z[2 * j + 1] = c_pack(yr[2 * j + 1], v.y);
             }
             __syncwarp();
+            if (lane == 0) af_mbar_arrive(&cDone[sb]);             // the producer may store the special bins
         }
         // ---- D: 32-point DFT over n2 of the column times W_2048^(n2 k1), in lane k1: bins k1 + 64 k2 and, mirrored,
         // 64 (32 - k2) - k1.  The twiddle is applied as (1 - i t) and a gain g inside the first butterflies. ----
         af_fft32_fma_tw(z, sTwC + lane);
-        af_mbar_wait(pEmpty, ((uint32_t)it & 1u) ^ 1u);      // bank done with the previous tile's spectra
         if (lane) {
             if (p.dataType == SpectralData_Mag) {                  // (uniform branch: no sqrt sequence in the power path)
 #pragma unroll
                 for (int k2 = 0; k2 < 32; k2++) {
                     const float pw = sqrtf(c_norm2_fma(z[AF_BR5(k2)]));
-                    if (k2 < 16) sP[offLo + k2 * strideK2] = pw;
-                    else sP[offHi + (32 - k2) * strideK2] = pw;
+                    if (k2 < 16) col[offLo + k2 * strideK2] = pw;
+                    else col[offHi + (32 - k2) * strideK2] = pw;
                 }
             } else {
 #pragma unroll
                 for (int k2 = 0; k2 < 32; k2++) {
                     const float pw = c_norm2_fma(z[AF_BR5(k2)]);
-                    if (k2 < 16) sP[offLo + k2 * strideK2] = pw;
-                    else sP[offHi + (32 - k2) * strideK2] = pw;
+                    if (k2 < 16) col[offLo + k2 * strideK2] = pw;
+                    else col[offHi + (32 - k2) * strideK2] = pw;
                 }
             }
         }
         __syncwarp();
-        if (lane == 0) af_mbar_arrive(pFull);
+        if (lane == 0) af_mbar_arrive(&pFull[sb]);
     }
 }
 
@@ -657,6 +676,38 @@ int plan_pieces(int num, const unsigned *desc /* num + 2 */, PiecePlan *pp) {
     return -1;
 }
 
+constexpr int kSmemBudget = 227 * 1024;
+
+// Shared-memory carve-up: as many frames per tile as fit (<= kFW), two TMA stages when they fit, else one.  Fills the
+// offsets, framesPerTile, stages, spanFloats and stageBytes of *pp (dctPitch must be set); returns the bytes, or -1
+// when not even one frame fits.
+int carve_smem(Params *pp, int timeLength, int hop, int num, int ccNum, int tabLen, int rawMel) {
+    int F = kFW < timeLength ? kFW : timeLength, stages = 2;
+    for (;;) {
+        int o = kBarBytes;                                      // the mbarriers come first
+        const int spanFloats = (F - 1) * hop + kN;
+        pp->offSpan = o;    o += stages * spanFloats * 4;
+        pp->offP = o;       o += (2 * kTileFloats * 4 + 15) & ~15;
+        pp->offWin = o;     o += 32 * 32 * 8;
+        pp->offTw = o;      o += kTwRows * 32 * 8;
+        pp->offSpec = o;    o += 2 * 32 * kSpecPitch * 8;
+        pp->offDct = o;     o += rawMel ? 0 : kMaxNum * pp->dctPitch * 4;
+        pp->offL = o;       o += 2 * 16 * kLPitch * 4;
+        pp->stageBytes = rawMel ? 2 * ((F * (num + 4) * 4 + 15) & ~15) : ((F * ccNum * 4 + 15) & ~15);
+        pp->offStage = o;   o += pp->stageBytes;
+        pp->offTab = o;     o += tabLen * 16;
+        pp->offDesc = o;    o += kMaxPieces * 4;
+        pp->offAssign = o;  o += (kMaxPass * kEW * 32 * 2 + 15) & ~15;
+        pp->offPrefix = o;  o += ((kMaxNum + 4) * 2 + 15) & ~15;
+        pp->spanFloats = spanFloats;
+        pp->framesPerTile = F; pp->stages = stages;
+        if (o <= kSmemBudget) return o;
+        if (stages == 2) { stages = 1; continue; }
+        stages = 2;
+        if (--F < 1) return -1;
+    }
+}
+
 }  // namespace
 
 int af_mfcc2_supported(int fftLength, int num, int ccNum, const float *bank) {
@@ -708,7 +759,6 @@ int af_mfcc2_plan_build(void **planOut, int fftLength, int num, int ccNum, const
         PiecePlan *pc = static_cast<PiecePlan *>(malloc(sizeof(PiecePlan)));
         if (!pc || plan_pieces(num, pl->ivDesc, pc) <= 0) { free(pc); free_plan(pl); return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC v2 plan: no piece plan"); }
         pl->nPass = pc->nPass; pl->nPieces = pc->nPieces; pl->lmax = pc->lmax; pl->firstPass2 = pc->firstPass2;
-        memcpy(pl->passLen, pc->passLen, sizeof(pl->passLen));
         memcpy(pl->pieceDesc, pc->pieceDesc, sizeof(pl->pieceDesc));
         memcpy(pl->piecePrefix, pc->prefix, sizeof(pl->piecePrefix));
         memcpy(pl->assign, pc->assign, sizeof(pl->assign));
@@ -737,38 +787,12 @@ int af_mfcc2_launch(void *plan, const float *data, int dataLength, int batch, in
     pp->nPeer = nPeer;
     for (int d = 0; d < nPeer; d++) pp->peerOut[d] = peerOut[d];
     pp->nPass = pl->nPass; pp->assign = pl->dAssign;
-    for (int i = 0; i < kMaxPass; i++) pp->passLen[i] = pl->passLen[i];
     pp->bankTab = pl->dTab; pp->pieceDesc = pl->dDesc; pp->piecePrefix = pl->dPrefix; pp->tabLen = pl->tabLen;
     pp->bulkStore = af_mfcc_bulk_store_ok(rawMel ? pl->num : pl->ccNum, out, nPeer, peerOut);
 
-    // shared-memory carve-up: as many frames per tile as fit (<= kFW), two TMA stages when they fit, else one
-    const int budget = 227 * 1024;
-    int F = kFW < timeLength ? kFW : timeLength, stages = 2, total = 0;
-    for (;;) {
-        int o = kBarBytes;                                      // the mbarriers come first
-        const int spanFloats = (F - 1) * slideLength + kN;
-        pp->offSpan = o;    o += stages * spanFloats * 4;
-        pp->offScratch = o; o += kFW * kScratchFloats * 4;
-        pp->offP = o;       o += (kPairs * kPitchPairs * 8 + 15) & ~15;
-        pp->offWin = o;     o += 32 * 32 * 8;
-        pp->offTw = o;      o += kTwRows * 32 * 8;
-        pp->offSpec = o;    o += 2 * 32 * kSpecPitch * 8;
-        pp->offDct = o;     o += rawMel ? 0 : kMaxNum * pp->dctPitch * 4;
-        pp->offL = o;       o += 2 * 16 * kLPitch * 4;
-        pp->stageBytes = rawMel ? 2 * ((F * (pl->num + 4) * 4 + 15) & ~15) : ((F * pl->ccNum * 4 + 15) & ~15);
-        pp->offStage = o;   o += pp->stageBytes;
-        pp->offTab = o;     o += pl->tabLen * 16;
-        pp->offDesc = o;    o += kMaxPieces * 4;
-        pp->offAssign = o;  o += (kMaxPass * kEW * 32 * 2 + 15) & ~15;
-        pp->offPrefix = o;  o += ((kMaxNum + 4) * 2 + 15) & ~15;
-        total = o;
-        pp->spanFloats = spanFloats;
-        if (total <= budget) break;
-        if (stages == 2) { stages = 1; continue; }
-        stages = 2;
-        if (--F < 1) { free(pp); return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC: slideLength %d too large for shared memory", slideLength); }
-    }
-    pp->framesPerTile = F; pp->stages = stages;
+    const int total = carve_smem(pp, timeLength, slideLength, pl->num, pl->ccNum, pl->tabLen, rawMel);
+    if (total < 0) { free(pp); return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC: slideLength %d too large for shared memory", slideLength); }
+    const int F = pp->framesPerTile;
     pp->tilesPerClip = (timeLength + F - 1) / F;
     if ((long long)pp->tilesPerClip * batch >= (1ll << 31)) { free(pp); return af_fail(AF_ERR_UNSUPPORTED, "fused MFCC: more than 2^31 tiles in one launch"); }
     pp->totalTiles = (unsigned)((long long)pp->tilesPerClip * batch);
@@ -776,6 +800,24 @@ int af_mfcc2_launch(void *plan, const float *data, int dataLength, int batch, in
     const int launched = af_mfcc_launch_ct(kernels, "k_mfcc_fused2", pl->ct, (long long)pp->totalTiles, kThreads, total, stream, *pp);
     free(pp);
     return launched;
+}
+
+// Test hook (host only): the shared-memory carve-up af_mfcc2_launch makes for a clip of timeLength frames at hop `hop`,
+// a bank of `num` bands with tabLen table entries and ccNum coefficients (rawMel: the filter-bank output instead).
+// Returns the bytes (-1: no frame fits); info = {frames per tile, TMA stages, offSpan, offP, offWin, offTw, offSpec,
+// offDct, offL, offStage, offTab, offDesc, offAssign, offPrefix, stageBytes, spanFloats}.
+extern "C" int afb200_mfccCarve2(int timeLength, int hop, int num, int ccNum, int tabLen, int rawMel, int *info /* 16 */) {
+    if (timeLength < 1 || hop < 1 || num < 1 || num > kMaxNum || ccNum < 1 || ccNum > 64 || tabLen < 0 || tabLen > kMaxTab) return -1;
+    Params pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.dctPitch = af_mfcc_dct_pitch(af_mfcc_ct(ccNum));
+    const int total = carve_smem(&pp, timeLength, hop, num, ccNum, tabLen, rawMel);
+    if (info) {
+        const int v[16] = {pp.framesPerTile, pp.stages, pp.offSpan, pp.offP, pp.offWin, pp.offTw, pp.offSpec, pp.offDct, pp.offL,
+                           pp.offStage, pp.offTab, pp.offDesc, pp.offAssign, pp.offPrefix, pp.stageBytes, pp.spanFloats};
+        memcpy(info, v, sizeof(v));
+    }
+    return total;
 }
 
 // Diagnostic / test hook (host only): the interval form the planner derives from a bank [num][1025], its cut into pieces

@@ -139,6 +139,13 @@ int afb200_decimatorTaps(float *left32, float *right31);
 int afb200_mfccBankPlan2(const float *bank, int num, int *owner /* 1025 */, unsigned *desc /* num + 2 */,
                          float *table /* 4 x 1408 */, unsigned *pieceDesc /* 256 */, unsigned short *prefix /* num + 2 */,
                          unsigned short *assign /* passes x helper lanes */, int *info /* 16 */);
+/* shared-memory carve-up of the second-generation fused kernel (host only, what its launcher computes): frames per tile
+ * and TMA stages for a clip of timeLength frames at hop `hop`, a bank of num bands with tabLen table entries and ccNum
+ * coefficients (rawMel != 0: filter-bank output).  Returns the bytes of shared memory, or -1 when not one frame fits.
+ * info = {frames per tile, stages, byte offsets of the TMA span, the two power tiles, window, twiddles, special columns,
+ * DCT matrix, log-mel tiles, staging, bank table, piece descriptors, lane assignment, piece prefix; staging bytes,
+ * span floats}. */
+int afb200_mfccCarve2(int timeLength, int hop, int num, int ccNum, int tabLen, int rawMel, int *info /* 16 */);
 /* cepstral deconvolution of rows x num constant-Q magnitudes (cqtObj_cqhc / cqtObj_deconv for any number of rows) */
 int cqtObj_cqhcBatch(CQTObj cqtObj, const float *in, int rows, int hcNum, float *out /* rows x hcNum */, int memKind, void *stream);
 int cqtObj_deconvBatch(CQTObj cqtObj, const float *in, int rows, float *timbre, float *pitch /* rows x num each */,

@@ -3,8 +3,10 @@
  * Three STFTs of the clip -- window h, its wrapped central difference dh and the ramp-weighted t.h -- give per cell the
  * reassigned frequency f - Im(S_dh / S_h) sr / 2 pi and time t + Re(S_th / S_h) / sr; cells are rounded to the grid and
  * the sign-alternated S_h is scatter-added.  Cell indices are integer outcomes of float32 divides: a cell within an ulp
- * of a rounding boundary may land one bin apart from the reference, so parity of the reassigned planes is stated
- * statistically (tests/test_gpu_reassign.py), while S_h itself meets the usual 1e-4. */
+ * of a rounding boundary may land one bin apart between two pipelines whose spectra differ in the last bits, so parity
+ * with the reference's output is stated statistically (tests/test_gpu_reassign.py), while S_h itself meets the usual
+ * 1e-4.  On the GPU's own three spectra every cell of the output is checked bit for bit
+ * (tests/test_gpu_scatter_cells.py). */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -7,7 +7,8 @@
 // t.h) are kernels/stft_generic.cu.
 //   * k_reassign_index: one thread per (clip, frame, bin), float32 operation by operation in the reference's order
 //     (explicit _rn intrinsics: no FMA contraction, the roundf outcome is an integer);
-//   * k_reassign_order: the row-local index iteration of order > 1, one CTA per (clip, frame), row in shared memory;
+//   * k_reassign_order: the row-local index iteration of order > 1, one CTA per (clip, frame); the row's scratch lives in
+//     global memory (the accumulator planes, not yet in use), so any row length works;
 //   * scatter: the reference adds the cells in (frame, bin) order into float planes; on the GPU the additions are made
 //     order-independent instead: every cell is scaled by a per-clip power of two (max |S_h| -> [2^35, 2^36)) and added
 //     as a 64-bit integer (atomicAdd on unsigned long long is associative), so the result is bit-stable for any
@@ -76,11 +77,9 @@ __global__ void __launch_bounds__(256) k_reassign_index(const float *__restrict_
 
 // order > 1: tmp[j] = fIdx[fIdx[j]] where the index stays in the row; tmp keeps its previous value elsewhere (it starts
 // at zero and is NOT cleared between iterations, reassign_algorithm.c:325-343)
-__global__ void __launch_bounds__(256) k_reassign_order(int *__restrict__ fIdx, int W, int order) {
-    extern __shared__ int sm[];
-    int *cur = sm, *tmp = sm + W;
-    int *row = fIdx + (size_t)blockIdx.x * W;
-    for (int j = threadIdx.x; j < W; j += blockDim.x) { cur[j] = row[j]; tmp[j] = 0; }
+__global__ void __launch_bounds__(256) k_reassign_order(int *fIdx, int *scratch, int W, int order) {
+    int *cur = fIdx + (size_t)blockIdx.x * W, *tmp = scratch + (size_t)blockIdx.x * W;
+    for (int j = threadIdx.x; j < W; j += blockDim.x) tmp[j] = 0;
     __syncthreads();
     for (int k = 0; k < order - 1; k++) {
         for (int j = threadIdx.x; j < W; j += blockDim.x) {
@@ -91,7 +90,6 @@ __global__ void __launch_bounds__(256) k_reassign_order(int *__restrict__ fIdx, 
         for (int j = threadIdx.x; j < W; j += blockDim.x) cur[j] = tmp[j];
         __syncthreads();
     }
-    for (int j = threadIdx.x; j < W; j += blockDim.x) row[j] = cur[j];
 }
 
 // per-clip maximum of |re|, |im| of S_h as float bits (non-negative floats order like unsigned integers)
@@ -178,7 +176,7 @@ extern "C" int af_launch_reassign(const AfReassignArgs *a, const float *r1, cons
     k_reassign_index<<<blocks, 256, 0, st>>>(r1, i1, r2, i2, r3, i3, p, tIdx, fIdx);
     AF_LAUNCH_CHECK("k_reassign_index");
     if (a->order > 1) {
-        k_reassign_order<<<(unsigned)((long long)a->batch * a->timeLength), 256, sizeof(int) * 2 * (size_t)W, st>>>(fIdx, W, a->order);
+        k_reassign_order<<<(unsigned)((long long)a->batch * a->timeLength), 256, 0, st>>>(fIdx, (int *)accRe, W, a->order);
         AF_LAUNCH_CHECK("k_reassign_order");
     }
     cudaError_t e = cudaMemsetAsync(maxBits, 0, sizeof(unsigned) * (size_t)a->batch, st);

@@ -3,7 +3,11 @@
 // Replaces the tail of wsstObj_wsst (src/wsst_algorithm.c:246-341: complex divide W'/W, / 2 pi, frequency -> row index,
 // scatter-add of W into the indexed rows) and of synsqObj_synsq (src/synsq_algorithm.c:147-300: atan2f phase, unwrap
 // along time, first difference, / 2 pi, the same index and scatter).  The transforms themselves are kernels/cwt.cu.
-//   * index: one thread per (row, time) cell, float32 operation by operation as the reference evaluates it;
+//   * index: one thread per (row, time) cell, float32 operation by operation as the reference evaluates it (explicit
+//     _rn intrinsics: nvcc would otherwise contract c*c + d*d, b*c - a*d and the |W|^2 threshold test into FMAs, and
+//     an FMA can move a cell to another row or across the threshold); log2f and atan2f are the CUDA Math API's, so
+//     the Octave / Log index and the synsq phase may differ from glibc's where those round differently.  The index
+//     and scatter are checked cell by cell on the GPU's own planes by tests/test_gpu_scatter_cells.py;
 //   * unwrap (synsq): the reference's sequential rule adds a multiple of 2 pi chosen from the distance to the previous
 //     UNWRAPPED sample; with wrapped phases in (-pi, pi] that is a running count K_i of +-1 jumps (jump when the raw
 //     difference leaves [-pi, pi]) and u_i = fl(p_i + 2 pi K_i) -- a prefix sum, done per row by one CTA;
@@ -28,9 +32,9 @@ struct IndexParams {
 
 __device__ __forceinline__ int fre_index(const IndexParams &p, float f) {
     if (p.scaleType == SpectralFilterBankScale_Octave || p.scaleType == SpectralFilterBankScale_Log)
-        return c_float_to_int(roundf((log2f(fabsf(f)) - p.l2min) * (float)p.num / p.l2den));
+        return c_float_to_int(roundf(__fdiv_rn(__fmul_rn(__fsub_rn(log2f(fabsf(f)), p.l2min), (float)p.num), p.l2den)));
     if (p.scaleType == SpectralFilterBankScale_Linear || p.scaleType == SpectralFilterBankScale_Linspace)
-        return c_float_to_int(roundf(fabsf(f - p.fmin) * (float)p.num / (p.fmax - p.fmin)));
+        return c_float_to_int(roundf(__fdiv_rn(__fmul_rn(fabsf(__fsub_rn(f, p.fmin)), (float)p.num), __fsub_rn(p.fmax, p.fmin))));
     // mel / bark / erb: __arr_roundIndex -- the band whose normalised frequency is nearest, -1 outside [arr[0], arr[num-1])
     const float a = fabsf(f);
     if (!(a >= p.norm[0]) || !(a < p.norm[p.num - 1])) return -1;
@@ -45,9 +49,14 @@ __global__ void k_wsst_index(const float *wr, const float *wi, const float *dr, 
     if (i >= (long long)p.num * p.n) return;
     const float a = dr[i], b = di[i], c = wr[i], d = wi[i];
     // __complexDiv (src/vector/flux_complex.c): (a + ib) / (c + id), imaginary part (b c - a d) / (c^2 + d^2)
-    const float den = c * c + d * d;
-    const float im = (b * c - a * d) / den;
-    idx[i] = fre_index(p, im / 6.283185307179586f);
+    const float den = __fadd_rn(__fmul_rn(c, c), __fmul_rn(d, d));
+    const float im = __fdiv_rn(__fsub_rn(__fmul_rn(b, c), __fmul_rn(a, d)), den);
+    idx[i] = fre_index(p, __fdiv_rn(im, 6.283185307179586f));
+}
+
+// u = fl(p + 2 pi K): the correction K * 2 pi rounded to double, then the sum (the reference's C expression; no DFMA)
+__device__ __forceinline__ float unwrapped(float ph, int K) {
+    return (float)__dadd_rn((double)ph, __dmul_rn(6.283185307179586, (double)K));
 }
 
 // synsq step 1-3: phase = atan2f(re, im) (the reference's argument order), unwrap along the row, first difference
@@ -60,13 +69,12 @@ __global__ void __launch_bounds__(kUwThreads) k_synsq_index(const float *re, con
     int *out = idx + (size_t)row * n;
     const int per = (n + kUwThreads - 1) / kUwThreads;             // consecutive samples per thread
     const int i0 = threadIdx.x * per, i1 = min(n, i0 + per);
-    const double kTwoPi = 6.283185307179586;
     // pass 1: jumps inside the thread's run (relative to its first sample's predecessor)
     int local = 0;
     float prev = i0 > 0 && i0 < n ? atan2f(r[i0 - 1], q[i0 - 1]) : 0.0f;
     for (int i = i0; i < i1; i++) {
         const float ph = atan2f(r[i], q[i]);
-        if (i > 0) { const float dlt = ph - prev; if (dlt > 3.14159265358979f) local--; else if (dlt < -3.14159265358979f) local++; }
+        if (i > 0) { const float dlt = __fsub_rn(ph, prev); if (dlt > 3.14159265358979f) local--; else if (dlt < -3.14159265358979f) local++; }
         prev = ph;
     }
     // block-wide exclusive scan of the per-thread jump counts
@@ -87,15 +95,15 @@ __global__ void __launch_bounds__(kUwThreads) k_synsq_index(const float *re, con
 
     // pass 2: unwrapped phase u = fl(p + 2 pi K), difference, index
     float uprev = 0.0f;
-    if (i0 > 0 && i0 < n) uprev = (float)((double)atan2f(r[i0 - 1], q[i0 - 1]) + kTwoPi * (double)K);
+    if (i0 > 0 && i0 < n) uprev = unwrapped(atan2f(r[i0 - 1], q[i0 - 1]), K);
     prev = i0 > 0 && i0 < n ? atan2f(r[i0 - 1], q[i0 - 1]) : 0.0f;
     for (int i = i0; i < i1; i++) {
         const float ph = atan2f(r[i], q[i]);
-        if (i > 0) { const float dlt = ph - prev; if (dlt > 3.14159265358979f) K--; else if (dlt < -3.14159265358979f) K++; }
-        const float u = (float)((double)ph + kTwoPi * (double)K);
-        const float dif = i > 0 ? u - uprev : 0.0f;
-        if (i < n - 1 || n == 1) out[i] = fre_index(p, dif / 6.283185307179586f);
-        if (i == n - 2) out[n - 1] = fre_index(p, dif / 6.283185307179586f);      // last column repeats column n - 2
+        if (i > 0) { const float dlt = __fsub_rn(ph, prev); if (dlt > 3.14159265358979f) K--; else if (dlt < -3.14159265358979f) K++; }
+        const float u = unwrapped(ph, K);
+        const float f = __fdiv_rn(i > 0 ? __fsub_rn(u, uprev) : 0.0f, 6.283185307179586f);
+        if (i < n - 1 || n == 1) out[i] = fre_index(p, f);
+        if (i == n - 2) out[n - 1] = fre_index(p, f);      // last column repeats column n - 2
         prev = ph; uprev = u;
     }
 }
@@ -109,7 +117,7 @@ __global__ void k_squeeze_scatter(const float *re, const float *im, const int *i
         const size_t k = (size_t)i * n + j;
         const int t = idx[k];
         const float v1 = re[k], v2 = im[k];
-        if (t >= 0 && t < num && v1 * v1 + v2 * v2 > thresh2) {
+        if (t >= 0 && t < num && __fadd_rn(__fmul_rn(v1, v1), __fmul_rn(v2, v2)) > thresh2) {
             outRe[(size_t)t * n + j] += v1;
             outIm[(size_t)t * n + j] += v2;
         }

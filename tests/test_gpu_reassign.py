@@ -1,7 +1,9 @@
 """Reassignment on the GPU (reassignObj_reassign / reassignObj_reassignBatch, kernels/reassign.cu) against the numpy
 oracle and the reference build.  Parity bar as in tests/test_reassign_cpu.py (indices are roundf() of float32 divides):
 >= 99.5 % of the cells identical to 1e-5 of the maximum and relative Frobenius error <= 5e-3 for the reassigned planes,
-1e-4 for the plain half spectrum; the GPU scatter is bit-stable across runs (64-bit fixed-point accumulation)."""
+1e-4 for the plain half spectrum; the GPU scatter is bit-stable across runs (64-bit fixed-point accumulation).
+This bar compares two different float32 pipelines.  On the GPU's own spectra every reassigned cell is checked bit for
+bit in tests/test_gpu_scatter_cells.py."""
 import numpy as np
 import pytest
 

@@ -6,7 +6,9 @@ round(log2f(|f_inst|) ...), an INTEGER outcome of float32 transcendental math --
 of a rounding boundary lands one row up or down depending on the libm / GPU rounding of log2f, atan2f and the divide.
 Between the numpy oracle and the reference build itself 0.02 % (wsst) / 0.2 % (synsq) of the time columns differ.  The
 test therefore demands (i) >= 98 % of the time columns identical to 1e-5 relative, (ii) a relative Frobenius error
-<= 1e-2 of the whole matrix, (iii) the plain CWT planes returned beside it within the usual 1e-4."""
+<= 1e-2 of the whole matrix, (iii) the plain CWT planes returned beside it within the usual 1e-4.
+This bar compares two different float32 pipelines.  The index and scatter kernels themselves are checked cell by cell on
+the GPU's own planes in tests/test_gpu_scatter_cells.py."""
 import numpy as np
 import pytest
 

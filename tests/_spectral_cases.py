@@ -65,6 +65,9 @@ def apply_edge(lib, obj, mode, num):
     return idx
 
 
+TWO_OUTPUTS = ("max", "mean", "var")        # features whose call returns (value, fre)
+
+
 def call_c(lib, name, x, fre, mode="full", phase=None, **kw):
     """one reference-signature call on a fresh object; x [T, num] -> [T] (or (value, fre) for max / mean / var)"""
     x = np.ascontiguousarray(x, np.float32)
@@ -102,12 +105,12 @@ def call_c(lib, name, x, fre, mode="full", phase=None, **kw):
         fn(obj, X, kw.get("threshold", 0), O1)
     elif name == "novelty":
         fn(obj, X, kw.get("step", 1), kw.get("threshold", 0.), ib(kw.get("method_type", 0)), ib(kw.get("data_type", 0)), O1)
-    elif name in ("max", "mean", "var"):
+    elif name in TWO_OUTPUTS:
         fn(obj, X, O1, O2)
     else:
         fn(obj, X, O1)
     lib.spectralObj_free(obj)
-    return (o1, o2) if name in ("max", "mean", "var") else o1
+    return (o1, o2) if name in TWO_OUTPUTS else o1
 
 
 def oracle(name, x, fre, mode="full", phase=None, **kw):

@@ -3,30 +3,15 @@ tests/golden/cepstrogram.npz), cepstrogramObj_new statuses and calTimeLength of 
 refusals (which need no device), the exported and bound symbols of include/afb200_cepstrogram.h and afb200_ext.h, and
 the Python class's argument checks."""
 import os
-import re
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
 import _cepstrogram_oracle as CO
+from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
-GOLD = os.path.join(GOLDEN, "cepstrogram.npz")
 ORACLE_TOL = 5e-5          # per frame, of max|log S|; worst seen: 1.6e-5 (details at 2^14, the reference's float32 FFTs)
 GOLDEN_MAX_CELLS = 1600    # cases with at most this many T x (N/2+1) cells go to the golden file (about 250 KB)
-
-
-def reference_outputs(names=None):
-    """{name: [cep, env, det] stacked} from the reference build when present, else the stored golden file"""
-    from oracle import ref_lib as R
-    if not R.available():
-        if not os.path.exists(GOLD):
-            pytest.skip("no reference build and no tests/golden/cepstrogram.npz")
-        g = np.load(GOLD)
-        return {k: g[k] for k in g.files}
-    lib = R.get_ref_lib()
-    return {name: np.stack(CO.c_case(lib, kw, CO.case_signal(name, kw)))
-            for name, kw in CO.cases() if names is None or name in names}
 
 
 def golden_names():
@@ -38,12 +23,20 @@ def golden_names():
     return out
 
 
+def _live(names):
+    """{name: [cep, env, det] stacked}"""
+    lib = ref_lib_or_none()
+    return {name: np.stack(CO.c_case(lib, kw, CO.case_signal(name, kw))) for name, kw in CO.cases() if name in names}
+
+
+GOLD = GoldenStore("cepstrogram.npz", _live, golden_names)
+
+
 @pytest.mark.parametrize("name,kw", CO.cases(), ids=[c[0] for c in CO.cases()])
 def test_oracle_matches_reference(name, kw):
-    from oracle import ref_lib as R
-    if not R.available() and name not in golden_names():
+    if ref_lib_or_none() is None and name not in golden_names():
         pytest.skip("case not in tests/golden/cepstrogram.npz and no reference build")
-    got = reference_outputs({name})[name]
+    got = GOLD.outputs({name})[name]
     *want, logs = CO.oracle_case(name, kw)
     for k in range(3):
         assert got[k].shape == want[k].shape, (name, k)
@@ -53,20 +46,13 @@ def test_oracle_matches_reference(name, kw):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/cepstrogram.npz")
-    g = np.load(GOLD)
-    assert sorted(g.files) == sorted(golden_names())
-    live = reference_outputs(set(g.files))
-    for k in g.files:
-        assert np.array_equal(live[k], g[k]), k
+    GOLD.check_file()
 
 
 def test_golden_file_covers_the_rules():
     names = golden_names()
     assert {"r1_c1", "r8_c128", "r8_c127", "r8_t0", "r8_t1", "r8_silent", "r9_slide512", "r9_slide700"} <= names
-    assert os.path.getsize(GOLD) < 400 * 1024
+    assert os.path.getsize(GOLD.path) < 400 * 1024
 
 
 def _grid():
@@ -146,27 +132,10 @@ def test_refusals_leave_outputs_untouched(product_lib):
     product_lib.cepstrogramObj_free(o)
 
 
-def _symbols(header):
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b(cepstrogramObj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
 def test_cepstrogram_symbols_exported_and_bound(product_lib):
     from audioflux_b200 import capi
-    names, ext = _symbols("afb200_cepstrogram.h"), _symbols("afb200_ext.h")
-    assert len(names) == 6 and ext == {"cepstrogramObj_cepstrogramBatch", "cepstrogramObj_cepstrogram2Batch"}
-    declared = set()
-    for h in os.listdir(os.path.join(ROOT, "include")):
-        declared |= _symbols(h)
-    assert declared == names | ext
-    assert set(capi.CEPSTROGRAM_API) == names | ext
-    for n in names | ext:
-        assert hasattr(product_lib, n), n
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        for n in names:
-            assert hasattr(lib, n), n
+    check_symbols(product_lib, "afb200_cepstrogram.h", "cepstrogramObj_", capi.CEPSTROGRAM_API, 6,
+                  {"cepstrogramObj_cepstrogramBatch", "cepstrogramObj_cepstrogram2Batch"})
 
 
 def test_python_class_checks(product_lib):

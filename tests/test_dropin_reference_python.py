@@ -2,29 +2,15 @@
 python/audioflux, byte-compiled into oracle/_ref/pyref by `make -C oracle`): after
 `audioflux.fftlib.set_fft_lib(lib_ext='b200')` (python/audioflux/fftlib.py:96-124) its BFT / XXCC / CQT / CWT /
 MelSpectrogram classes run on libaudioflux_b200.so and return what the reference build returns."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT, noise, tones, rel_max
+from conftest import noise, tones, rel_max
+from _parity_kit import raf  # noqa: F401  (a fixture)
 
 from oracle import af_oracle as O
-from oracle import ref_lib as R
-from oracle import ref_python as RP
 
 TOL = 1e-4
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    """the reference package, default library = the reference build, lib_ext 'b200' = the product"""
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def _use(raf, which):

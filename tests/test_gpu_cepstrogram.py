@@ -5,25 +5,18 @@ and half STFT planes and on a non-Hermitian plane, the launch count, the refusal
 class running on libaudioflux_b200.so."""
 import ctypes as C
 import itertools
-import os
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
 import _cepstrogram_oracle as CO
+from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 TOL = 1e-4          # per frame, of the frame's max |log S|; and per tensor, of max |want|
 LOG_CLAMP = float(np.log(np.float32(1e-16)))
-
-
-def _ref():
-    from oracle import ref_lib as R
-    return R.get_ref_lib() if R.available() else None
 
 
 def _check(got, want, logs, what):
@@ -46,7 +39,7 @@ def test_legacy_matches_oracle_and_reference(product_lib, cuda_device, name, kw)
     *want, logs = CO.oracle_case(name, kw)
     for k in range(3):
         _check(got[k], want[k], logs, (name, k, "oracle"))
-    ref = _ref()
+    ref = ref_lib_or_none()
     if ref is not None:
         for k, r in enumerate(CO.c_case(ref, kw, x)):
             _check(got[k], r.astype(np.float64), logs, (name, k, "reference"))
@@ -81,15 +74,6 @@ def test_silent_frames_hit_the_clamp(product_lib, cuda_device):
             assert abs(cep[t, 0] - LOG_CLAMP) <= 1e-6 * abs(LOG_CLAMP), (name, t, cep[t, 0])
             assert not cep[t, 1:].any() and not det[t].any(), (name, t)
             assert (env[t] == cep[t, 0]).all(), (name, t)
-
-
-def _stream():
-    import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _dptr(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def test_batches_bit_identical_to_legacy(product_lib, cuda_device):
@@ -156,11 +140,11 @@ def test_cepstrogram2_full_and_half_planes(product_lib, cuda_device):
         xd = torch.from_numpy(x).cuda()
         hre = torch.empty((T, n // 2 + 1), device="cuda")
         him = torch.empty_like(hre)
-        assert product_lib.stftObj_stftBatch(sobj, _dptr(xd), x.size, 1, _dptr(hre), _dptr(him), 1, _stream()) == 0
+        assert product_lib.stftObj_stftBatch(sobj, dptr(xd), x.size, 1, dptr(hre), dptr(him), 1, stream()) == 0
         outs = [torch.full((T, n // 2 + 1), 7.0, device="cuda") for _ in range(3)]
         h0 = (hre.clone(), him.clone())
-        assert product_lib.cepstrogramObj_cepstrogram2Batch(obj, c, _dptr(hre), _dptr(him), T, n // 2 + 1,
-                                                            *map(_dptr, outs), 1, _stream()) == 0
+        assert product_lib.cepstrogramObj_cepstrogram2Batch(obj, c, dptr(hre), dptr(him), T, n // 2 + 1,
+                                                            *map(dptr, outs), 1, stream()) == 0
         torch.cuda.synchronize()
         assert torch.equal(hre, h0[0]) and torch.equal(him, h0[1])
         for k in range(3):
@@ -206,29 +190,19 @@ def test_cepstrogram2_batch_spans_chunks(product_lib, cuda_device):
             assert np.array_equal(dev[k][b].cpu().numpy(), legacy[k][0]), (b, k, "device")
 
 
-def _launches(product_lib, fn):
-    import torch
-    fn()
-    torch.cuda.synchronize()
-    n0 = product_lib.afb200_kernelLaunchCount()
-    fn()
-    torch.cuda.synchronize()
-    return product_lib.afb200_kernelLaunchCount() - n0
-
-
 def test_one_launch_per_chunk(product_lib, cuda_device):
     import torch
     t = af.Cepstrogram(radix2_exp=12, window_type=af.WindowType.HANN, slide_length=1024)
     x = np.stack([CO.signal(s, 160000) for s in range(40)])
     xd = torch.from_numpy(x).cuda()
-    assert _launches(product_lib, lambda: t.cepstrogram_batch(xd, 4)) == 1
-    assert _launches(product_lib, lambda: t.cepstrogram_batch(xd, 4, env=False)) == 1
-    assert _launches(product_lib, lambda: t.cepstrogram_batch(x, 4)) == 3          # 16 + 16 + 8 clips
-    assert _launches(product_lib, lambda: t.cepstrogram_batch(x[:1], 4)) == 1
+    assert count_launches(product_lib, lambda: t.cepstrogram_batch(xd, 4), warm=True) == 1
+    assert count_launches(product_lib, lambda: t.cepstrogram_batch(xd, 4, env=False), warm=True) == 1
+    assert count_launches(product_lib, lambda: t.cepstrogram_batch(x, 4), warm=True) == 3          # 16 + 16 + 8 clips
+    assert count_launches(product_lib, lambda: t.cepstrogram_batch(x[:1], 4), warm=True) == 1
     for r in (1, 8, 14):
         u = af.Cepstrogram(radix2_exp=r)
         xr = torch.from_numpy(CO.signal(r, 5 * (1 << r))).cuda()
-        assert _launches(product_lib, lambda: u.cepstrogram_batch(xr, 1)) == 1, r
+        assert count_launches(product_lib, lambda: u.cepstrogram_batch(xr, 1), warm=True) == 1, r
 
 
 def test_refusals_on_the_device(product_lib, cuda_device):
@@ -239,25 +213,14 @@ def test_refusals_on_the_device(product_lib, cuda_device):
     T = t.cal_time_length(5000)
     outs = [torch.full((T, n // 2 + 1), 7.0, device="cuda") for _ in range(3)]
     for c in (0, n // 2 + 1):
-        st = product_lib.cepstrogramObj_cepstrogramBatch(t._obj, c, _dptr(xd), 5000, 1, *map(_dptr, outs), 1, _stream())
+        st = product_lib.cepstrogramObj_cepstrogramBatch(t._obj, c, dptr(xd), 5000, 1, *map(dptr, outs), 1, stream())
         assert st != 0 and f"cepNum={c}".encode() in product_lib.afb200_lastError()
         torch.cuda.synchronize()
         assert all((o == 7.0).all() for o in outs)
     # the largest legal cepNum runs, and its details are exactly 0
-    st = product_lib.cepstrogramObj_cepstrogramBatch(t._obj, n // 2, _dptr(xd), 5000, 1, *map(_dptr, outs), 1, _stream())
+    st = product_lib.cepstrogramObj_cepstrogramBatch(t._obj, n // 2, dptr(xd), 5000, 1, *map(dptr, outs), 1, stream())
     torch.cuda.synchronize()
     assert st == 0 and not outs[2].any() and (outs[0] != 7.0).all()
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_class_on_b200(raf, cuda_device):

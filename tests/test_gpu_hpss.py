@@ -3,41 +3,23 @@ buffers, H only, P only) against the float64 oracle and the reference build; the
 into zeroed buffers with host and device pointers, across staging chunks and workspace groups, with neighbouring clips
 of very different levels; the launch count; device calls queued back to back on one object; and the reference's own
 HPSS class running on libaudioflux_b200.so."""
-import ctypes as C
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 import _hpss_oracle as HO
+from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 TOL = 1e-4          # per output: max|got - want| <= TOL * max|want| where the normaliser is >= 1e-2, 1e-2 elsewhere
 CASES = dict(HO.cases())
-
-
-def _ref():
-    from oracle import ref_lib as R
-    return R.get_ref_lib() if R.available() else None
 
 
 def _check(got, want, kw, what):
     assert got.shape == want.shape, (what, got.shape, want.shape)
     err, ill = HO.errors(got, want, kw)
     assert err <= TOL and ill <= 1e-2, (what, err, ill)
-
-
-def _dptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _batch(lib, o, x, device, outputs="hp"):
@@ -49,8 +31,8 @@ def _batch(lib, o, x, device, outputs="hp"):
         import torch
         xd = torch.from_numpy(x).cuda()
         outs = [torch.full((b, m), 7.0, device="cuda") if c in outputs else None for c in "hp"]
-        ptrs = [None if t is None else _dptr(t) for t in outs]
-        assert lib.hpssObj_hpssBatch(o, _dptr(xd), n, b, *ptrs, 1, _stream()) == 0, lib.afb200_lastError()
+        ptrs = [None if t is None else dptr(t) for t in outs]
+        assert lib.hpssObj_hpssBatch(o, dptr(xd), n, b, *ptrs, 1, stream()) == 0, lib.afb200_lastError()
         torch.cuda.synchronize()
         return [None if t is None else t.cpu().numpy() for t in outs]
     outs = [np.full((b, m), 7.0, np.float32) if c in outputs else None for c in "hp"]
@@ -78,7 +60,7 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     got = HO.c_case(product_lib, name, kw)
     assert product_lib.afb200_lastError() in (b"", None)
     want = HO.oracle_case(name, kw)
-    ref = _ref()
+    ref = ref_lib_or_none()
     refs = HO.c_case(ref, name, kw) if ref is not None else None
     for k in range(2):
         assert (got[k] is None) == (want[k] is None), (name, k)
@@ -108,28 +90,20 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     product_lib.hpssObj_free(o)
 
 
-def _launches(lib, fn):
-    import torch
-    torch.cuda.synchronize()
-    n0 = lib.afb200_kernelLaunchCount()
-    fn()
-    torch.cuda.synchronize()
-    return lib.afb200_kernelLaunchCount() - n0
-
-
 def test_launch_count(product_lib, cuda_device):
     """per workspace group, up to fftLength 2^14: one STFT, one mask, two per inverse STFT (frames, overlap-add)"""
     import torch
     h = af.HPSS(radix2_exp=11)
     x = (0.1 * np.random.default_rng(1).standard_normal((8, 40000))).astype(np.float32)
     xd = torch.from_numpy(x).cuda()
-    assert _launches(product_lib, lambda: h.hpss_batch(xd)) == 6
-    assert _launches(product_lib, lambda: h.hpss(x)) == 6
+    assert count_launches(product_lib, lambda: h.hpss_batch(xd), warm=False) == 6
+    assert count_launches(product_lib, lambda: h.hpss(x), warm=False) == 6
     o = h._obj
     m = h.cal_data_length(40000)
     out = torch.empty((8, m), device="cuda")
-    for ptrs in ((_dptr(out), None), (None, _dptr(out))):
-        assert _launches(product_lib, lambda: product_lib.hpssObj_hpssBatch(o, _dptr(xd), 40000, 8, *ptrs, 1, _stream())) == 4
+    for ptrs in ((dptr(out), None), (None, dptr(out))):
+        call = lambda: product_lib.hpssObj_hpssBatch(o, dptr(xd), 40000, 8, *ptrs, 1, stream())  # noqa: E731
+        assert count_launches(product_lib, call, warm=False) == 4
 
 
 def test_batch_across_chunks_and_groups(product_lib, cuda_device):
@@ -144,11 +118,11 @@ def test_batch_across_chunks_and_groups(product_lib, cuda_device):
         x[k] = HO.case_signal(f"clip{k % 7}", dict(length=n)) * (1000.0 if k % 2 else 0.001)
         x[k] += (0.01 * rng.standard_normal(n)).astype(np.float32)
     host = {}
-    launches = _launches(product_lib, lambda: host.setdefault("o", h.hpss_batch(x)))
+    launches = count_launches(product_lib, lambda: host.setdefault("o", h.hpss_batch(x)), warm=False)
     assert launches == 6 * 5, launches
     xd = torch.from_numpy(x).cuda()
     dev = {}
-    launches = _launches(product_lib, lambda: dev.setdefault("o", h.hpss_batch(xd)))
+    launches = count_launches(product_lib, lambda: dev.setdefault("o", h.hpss_batch(xd)), warm=False)
     assert launches % 6 == 0 and launches >= 12, launches                 # several workspace groups
     for k in range(2):
         assert np.array_equal(dev["o"][k].cpu().numpy(), host["o"][k]), k
@@ -181,26 +155,15 @@ def test_refusals_on_the_device(product_lib, cuda_device):
     xd = torch.from_numpy(HO.case_signal("ref", dict(length=5000))).cuda()
     out = torch.full((8192,), 7.0, device="cuda")
     st, o = HO.c_new(product_lib, 13)
-    assert product_lib.hpssObj_hpssBatch(o, _dptr(xd), 5000, 1, _dptr(out), None, 1, _stream()) != 0
+    assert product_lib.hpssObj_hpssBatch(o, dptr(xd), 5000, 1, dptr(out), None, 1, stream()) != 0
     assert b"shorter than one frame" in product_lib.afb200_lastError()
     product_lib.hpssObj_free(o)
     st, o = HO.c_new(product_lib, 10, None, None, 21, 401)
-    assert product_lib.hpssObj_hpssBatch(o, _dptr(xd), 5000, 1, None, _dptr(out), 1, _stream()) != 0
+    assert product_lib.hpssObj_hpssBatch(o, dptr(xd), 5000, 1, None, dptr(out), 1, stream()) != 0
     assert b"orders up to" in product_lib.afb200_lastError()
     product_lib.hpssObj_free(o)
     torch.cuda.synchronize()
     assert (out == 7.0).all()
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_classes_on_b200(raf, cuda_device):

@@ -1,25 +1,18 @@
 """NSGT on the GPU: the reference's entry points against the oracle and the reference build, the batched entry point
 (host and device pointers, any batch size), the matrix as a gather of the cells, the launch count, the direct path of
 the widest bands, setMinLength, and the reference's own NSGT class running on libaudioflux_b200.so."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT, rel_max
+from conftest import rel_max
 import _nsgt_oracle as NO
+from _parity_kit import count_launches, raf, ref_lib_or_none  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 from oracle import af_oracle as O
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 TOL = 1e-4
-
-
-def _ref():
-    from oracle import ref_lib as R
-    return R.get_ref_lib() if R.available() else None
 
 
 def _cell_gather(cr, ci, lens, cmap):
@@ -30,7 +23,7 @@ def _cell_gather(cr, ci, lens, cmap):
 
 @pytest.mark.parametrize("name,kw", NO.cases(), ids=[c[0] for c in NO.cases()])
 def test_legacy_matches_oracle_and_reference(product_lib, cuda_device, name, kw):
-    ref = _ref()
+    ref = ref_lib_or_none()
     _, p = NO.params(**kw)
     x = NO.case_signal(7, p["fft_length"], p["samplate"])
     st, obj = NO.c_new(product_lib, **kw)
@@ -80,28 +73,19 @@ def test_batch_host_device_bit_identical_to_legacy(product_lib, cuda_device):
             assert np.array_equal(re[b], legacy[b][0]) and np.array_equal(im[b], legacy[b][1])
 
 
-def _launches(product_lib, t, xd):
-    import torch
-    t.nsgt_batch(xd)
-    torch.cuda.synchronize()
-    n0 = product_lib.afb200_kernelLaunchCount()
-    t.nsgt_batch(xd)
-    n = product_lib.afb200_kernelLaunchCount() - n0
-    torch.cuda.synchronize()
-    return n
-
-
 def test_launch_count(product_lib, cuda_device):
     """af_launch_stft's launches (one up to 2^14 points), one Bluestein launch, one direct launch when a band is wider
     than 4096"""
     import torch
     x12 = torch.zeros((3, 1 << 12), device="cuda")
-    assert _launches(product_lib, af.NSGT(num=84, radix2_exp=12), x12) == 2
+    t = af.NSGT(num=84, radix2_exp=12)
+    assert count_launches(product_lib, lambda: t.nsgt_batch(x12), warm=True) == 2
     x19 = torch.zeros((2, 1 << 19), device="cuda")
     wide = af.NSGT(num=84, radix2_exp=19, samplate=44100)             # widest band 5587: direct path
     narrow = af.NSGT(num=84, radix2_exp=19, samplate=196000)          # same FFT, every band <= 4096
     assert wide.get_time_length_arr().max() > 4096 >= narrow.get_time_length_arr().max()
-    assert _launches(product_lib, wide, x19) == _launches(product_lib, narrow, x19) + 1
+    assert (count_launches(product_lib, lambda: wide.nsgt_batch(x19), warm=True) ==
+            count_launches(product_lib, lambda: narrow.nsgt_batch(x19), warm=True) + 1)
 
 
 def _oracle_check(t, x, kw):
@@ -149,17 +133,6 @@ def test_refusals(product_lib):
         st, obj = NO.c_new(product_lib, **kw)
         assert st == -2 and not obj.value, kw
         assert product_lib.afb200_lastError()
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_nsgt_class_on_b200(raf, cuda_device):

@@ -3,26 +3,17 @@ chunk by chunk) and the batch against the float64 oracle and the reference build
 call into zeroed buffers with host and device pointers, across staging chunks, for ratios down to 2^-nbit and for
 upsampling by 6; a clip longer than 2^24 samples; device calls at different ratios queued back to back; the launch
 count; the refusals; and the reference's own Resample / WindowResample classes running on libaudioflux_b200.so."""
-import ctypes as C
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 import _resample_oracle as RO
+from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 TOL = 1e-4          # per tensor: max|got - want| <= TOL * max|want|
 CASES = dict(RO.cases())
-
-
-def _ref():
-    from oracle import ref_lib as R
-    return R.get_ref_lib() if R.available() else None
 
 
 def _check(got, want, what):
@@ -30,15 +21,6 @@ def _check(got, want, what):
     if got.size:
         err = np.abs(np.asarray(got, np.float64) - want).max() / max(np.abs(want).max(), 1e-30)
         assert err <= TOL, (what, err)
-
-
-def _dptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _batch(lib, o, x, device):
@@ -50,7 +32,7 @@ def _batch(lib, o, x, device):
         import torch
         xd = torch.from_numpy(x).cuda()
         out = torch.full((b, m), 7.0, device="cuda")
-        assert lib.resampleObj_resampleBatch(o, _dptr(xd), n, b, _dptr(out), 1, _stream()) == 0, lib.afb200_lastError()
+        assert lib.resampleObj_resampleBatch(o, dptr(xd), n, b, dptr(out), 1, stream()) == 0, lib.afb200_lastError()
         torch.cuda.synchronize()
         return out.cpu().numpy()
     out = np.full((b, m), 7.0, np.float32)
@@ -72,7 +54,7 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     got = RO.c_case(product_lib, name, kw)
     assert product_lib.afb200_lastError() in (b"", None)
     want = RO.oracle_case(name, kw)
-    ref = _ref()
+    ref = ref_lib_or_none()
     refs = RO.c_case(ref, name, kw) if ref is not None else None
     for k, (g, w) in enumerate(zip(got, want)):
         _check(g, w, (name, k, "oracle"))
@@ -100,22 +82,13 @@ def test_clip_beyond_2_24_samples(product_lib, cuda_device):
     got = RO.c_case(product_lib, name, kw)[0]
     assert got.size == int(np.floor(np.float32(RO.BIG) * np.float32(1 / 3)))
     _check(got, RO.oracle_case(name, kw)[0], "oracle")
-    ref = _ref()
+    ref = ref_lib_or_none()
     if ref is not None:
         _check(got, RO.c_case(ref, name, kw)[0].astype(np.float64), "reference")
     st, o = RO.c_new(product_lib, 2)
     RO.c_apply(product_lib, o, kw["ops"])
     assert np.array_equal(_batch(product_lib, o, RO.case_signal(name, kw)[None], True)[0], got)
     product_lib.resampleObj_free(o)
-
-
-def _launches(lib, fn):
-    import torch
-    torch.cuda.synchronize()
-    n0 = lib.afb200_kernelLaunchCount()
-    fn()
-    torch.cuda.synchronize()
-    return lib.afb200_kernelLaunchCount() - n0
 
 
 def test_batch_across_staging_chunks_and_launch_count(product_lib, cuda_device):
@@ -125,15 +98,15 @@ def test_batch_across_staging_chunks_and_launch_count(product_lib, cuda_device):
     rng = np.random.default_rng(3)
     x = (0.1 * rng.standard_normal((20, 1_200_000))).astype(np.float32)      # 4.8 MB clips: 13 per 64 MB chunk
     host = {}
-    assert _launches(product_lib, lambda: host.setdefault("o", r.resample_batch(x))) == 2
+    assert count_launches(product_lib, lambda: host.setdefault("o", r.resample_batch(x)), warm=False) == 2
     xd = torch.from_numpy(x).cuda()
     dev = {}
-    assert _launches(product_lib, lambda: dev.setdefault("o", r.resample_batch(xd))) == 1
+    assert count_launches(product_lib, lambda: dev.setdefault("o", r.resample_batch(xd)), warm=False) == 1
     assert np.array_equal(dev["o"].cpu().numpy(), host["o"])
     for k in (0, 12, 13, 19):
         n, buf = RO.c_resample(product_lib, r._obj, x[k])
         assert np.array_equal(host["o"][k], buf[:n]), k
-    assert _launches(product_lib, lambda: r.resample(x[:1, :5000])) == 1
+    assert count_launches(product_lib, lambda: r.resample(x[:1, :5000]), warm=False) == 1
 
 
 @pytest.mark.parametrize("qual", [0, 2])
@@ -195,25 +168,14 @@ def test_refusals_on_the_device(product_lib, cuda_device):
     st, o = RO.c_new(product_lib, 0)
     product_lib.resampleObj_setSamplateRatio(o, 0.0019)                      # 0.0019 * 512 < 1
     out = torch.full((64,), 7.0, device="cuda")
-    assert product_lib.resampleObj_resampleBatch(o, _dptr(xd), 5000, 1, _dptr(out), 1, _stream()) != 0
+    assert product_lib.resampleObj_resampleBatch(o, dptr(xd), 5000, 1, dptr(out), 1, stream()) != 0
     assert b"below 1" in product_lib.afb200_lastError()
     product_lib.resampleObj_setSamplate(o, 16000, 48000)
     product_lib.resampleObj_enableContinue(o, 1)                             # q = 1
-    assert product_lib.resampleObj_resampleBatch(o, _dptr(xd), 5000, 1, _dptr(out), 1, _stream()) != 0
+    assert product_lib.resampleObj_resampleBatch(o, dptr(xd), 5000, 1, dptr(out), 1, stream()) != 0
     torch.cuda.synchronize()
     assert (out == 7.0).all()
     product_lib.resampleObj_free(o)
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_classes_on_b200(raf, cuda_device):

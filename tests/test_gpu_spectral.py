@@ -1,19 +1,16 @@
 """Spectral descriptors on the GPU: the reference's entry points against the oracle and the reference build, the batched
 entry point (host and device pointers, one launch, clip boundaries), the documented differences (stateless objects,
 step >= timeLength) and the reference's own Spectral class running on libaudioflux_b200.so."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 import _spectral_cases as SC
+from _parity_kit import count_launches, raf, ref_lib_or_none  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 from audioflux_b200 import spectral as SP
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 
 
 def _parts(v):
@@ -21,8 +18,7 @@ def _parts(v):
 
 
 def test_legacy_entry_points_match_oracle_and_reference(product_lib, cuda_device):
-    from oracle import ref_lib as R
-    ref = R.get_ref_lib() if R.available() else None
+    ref = ref_lib_or_none()
     bad = []
     for setname, x, ph, fre in SC.spectrogram_sets(seed=3):
         for mode in ("full", "range", "list"):
@@ -96,12 +92,9 @@ def test_one_launch_per_device_call(product_lib, cuda_device):
     s = af.Spectral(x.shape[-1], fre)
     xd, pd = torch.from_numpy(x).cuda(), torch.from_numpy(ph).cuda()
     s.spectral_batch(xd, ["centroid"])
-    torch.cuda.synchronize()
+    # the first call with phase planes, and the first with every feature, each launch one kernel
     for feats in (["centroid"], _all_features()):
-        n0 = product_lib.afb200_kernelLaunchCount()
-        s.spectral_batch(xd, feats, phase=pd)
-        assert product_lib.afb200_kernelLaunchCount() - n0 == 1
-    torch.cuda.synchronize()
+        assert count_launches(product_lib, lambda: s.spectral_batch(xd, feats, phase=pd), warm=False) == 1
 
 
 def test_step_at_least_time_length_is_clamped(product_lib, cuda_device):
@@ -147,17 +140,6 @@ def test_stateless_repeated_and_multichannel(product_lib, cuda_device):
         for k in range(3):
             for g, w in zip(_parts(multi), _parts(SC.SO.compute(name, x[k], idx, fre))):
                 assert SC.agree(g[k], w, exact=name == "rolloff") is None, (name, k)
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_spectral_class_on_b200(raf, cuda_device):

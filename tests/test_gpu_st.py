@@ -2,25 +2,17 @@
 (both shared-memory paths of k_st_rows), FST rows as the exact expansion of their partition segment, the batched entry
 points (host and device pointers, batches that span several staging chunks) bit-identical to the legacy calls, the
 launch count, and the reference's own ST / FST classes running on libaudioflux_b200.so."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 import _st_oracle as SO
+from _parity_kit import count_launches, raf, ref_lib_or_none  # noqa: F401  (raf: a fixture)
 
 import audioflux_b200 as af
 
 pytestmark = pytest.mark.gpu
-B200 = os.path.join(ROOT, "audioflux_b200", "lib", "libaudioflux_b200.so")
 TOL = 1e-4          # per row, of the row's own max |want| (DESIGN section 2)
 ZERO_TOL = 1e-20    # rows that are exactly zero in the want
-
-
-def _ref():
-    from oracle import ref_lib as R
-    return R.get_ref_lib() if R.available() else None
 
 
 def _check_rows(re, im, want, what):
@@ -42,7 +34,7 @@ def test_st_legacy_matches_oracle_and_reference(product_lib, cuda_device, name, 
     _check_rows(re, im, SO.oracle_st_case(kw, x), (name, "oracle"))
     bins = SO.st_rows(kw)
     assert all(not im[r].any() for r, b in enumerate(bins) if b == 0)          # bin 0: an imaginary row of 0
-    ref = _ref()
+    ref = ref_lib_or_none()
     if ref is not None and kw["radix2_exp"] >= 3:
         rre, rim = SO.c_st_case(ref, kw, x)
         _check_rows(re, im, rre.astype(np.float64) + 1j * rim, (name, "reference"))
@@ -54,7 +46,7 @@ def test_fst_legacy_matches_oracle_and_reference(product_lib, cuda_device, name,
     re, im = SO.c_fst_case(product_lib, kw, x)
     assert product_lib.afb200_lastError() in (b"", None)
     _check_rows(re, im, SO.fst(x, kw["min_index"], kw["max_index"]), (name, "oracle"))
-    ref = _ref()
+    ref = ref_lib_or_none()
     if ref is not None:
         rre, rim = SO.c_fst_case(ref, kw, x)
         _check_rows(re, im, rre.astype(np.float64) + 1j * rim, (name, "reference"))
@@ -110,17 +102,6 @@ def test_batches_bit_identical_to_legacy(product_lib, cuda_device):
         assert np.array_equal(re.reshape(6, 100, 256)[b], lr) and np.array_equal(im.reshape(6, 100, 256)[b], li)
 
 
-def _launches(product_lib, fn, xd):
-    import torch
-    fn(xd)
-    torch.cuda.synchronize()
-    n0 = product_lib.afb200_kernelLaunchCount()
-    fn(xd)
-    n = product_lib.afb200_kernelLaunchCount() - n0
-    torch.cuda.synchronize()
-    return n
-
-
 def test_launch_count_independent_of_rows(product_lib, cuda_device):
     """ST: the forward FFT and k_st_rows; FST: the forward FFT, k_fst_segments and k_fst_expand"""
     import torch
@@ -128,8 +109,10 @@ def test_launch_count_independent_of_rows(product_lib, cuda_device):
         xd = torch.zeros((3, 1 << r), device="cuda")
         hi = (1 << (r - 1)) - 1
         for rows in ((1, 2), (1, hi), (hi - 3, hi)):
-            assert _launches(product_lib, af.ST(radix2_exp=r, min_index=rows[0], max_index=rows[1]).st_batch, xd) == 2
-            assert _launches(product_lib, af.FST(radix2_exp=r, min_index=rows[0], max_index=rows[1]).fst_batch, xd) == 3
+            st = af.ST(radix2_exp=r, min_index=rows[0], max_index=rows[1])
+            fst = af.FST(radix2_exp=r, min_index=rows[0], max_index=rows[1])
+            assert count_launches(product_lib, lambda: st.st_batch(xd), warm=True) == 2
+            assert count_launches(product_lib, lambda: fst.fst_batch(xd), warm=True) == 3
 
 
 def test_set_value_and_bin_list_follow_the_object(product_lib, cuda_device):
@@ -141,17 +124,6 @@ def test_set_value_and_bin_list_follow_the_object(product_lib, cuda_device):
     got = t.st(x)
     want = SO.st(x, [300, 0, 7, 7, 512], 2.5, 0.7)
     _check_rows(got.real.astype(np.float32), got.imag.astype(np.float32), want, "set_value + use_bin_arr")
-
-
-@pytest.fixture(scope="module")
-def raf(product_lib):
-    from oracle import ref_lib as R
-    from oracle import ref_python as RP
-    if not (RP.available() and R.available()):
-        pytest.skip("oracle/_ref/pyref or oracle/_ref/libaudioflux_ref.so not built (make -C oracle REF=<audioFlux tree>)")
-    mod = RP.load(R.REF_PATH, B200)
-    yield mod
-    mod.fftlib.set_fft_lib(None)
 
 
 def test_reference_classes_on_b200(raf, cuda_device):

@@ -4,46 +4,50 @@ refusals (which need no device), the exported and bound symbols of include/afb20
 Python class's argument checks."""
 import itertools
 import os
-import re
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
 import _hpss_oracle as HO
+from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
-GOLD = os.path.join(GOLDEN, "hpss.npz")
 ORACLE_TOL = 2e-5          # of max|reference output| where the normaliser is >= 1e-2 (elsewhere 1e-2); worst seen: 2e-6
 GOLDEN_MAX_LEN = 5000      # cases with outputs up to this many samples go to the golden file
+CASES = dict(HO.cases())
 
 
 def _key(name, k):
     return f"{name}__{k}"
 
 
-def reference_outputs(names):
-    """{name: [h, p]} (None for a skipped output) from the reference build when present, else the golden file"""
-    from oracle import ref_lib as R
-    cases = dict(HO.cases())
-    if R.available():
-        lib = R.get_ref_lib()
-        return {n: HO.c_case(lib, n, cases[n]) for n in names}
-    if not os.path.exists(GOLD):
-        pytest.skip("no reference build and no tests/golden/hpss.npz")
-    g = np.load(GOLD)
-    return {n: [g[_key(n, k)] if _key(n, k) in g.files else None for k in range(2)] for n in names}
-
-
 def golden_names():
     return {name for name, kw in HO.cases() if HO.data_length(kw["length"], 1 << kw["radix2_exp"]) <= GOLDEN_MAX_LEN}
 
 
+def _golden_keys():
+    """h is output 0 and p output 1; a skipped output has no key"""
+    return {_key(n, k) for n in golden_names() for k, c in enumerate("hp") if c in CASES[n].get("outputs", "hp")}
+
+
+def _live(keys):
+    lib = ref_lib_or_none()
+    out = {}
+    for n in sorted({k.split("__")[0] for k in keys}):
+        for k, o in enumerate(HO.c_case(lib, n, CASES[n])):
+            if o is not None and _key(n, k) in keys:
+                out[_key(n, k)] = o
+    return out
+
+
+GOLD = GoldenStore("hpss.npz", _live, _golden_keys)
+
+
 @pytest.mark.parametrize("name,kw", HO.cases(), ids=[c[0] for c in HO.cases()])
 def test_oracle_matches_reference(name, kw):
-    from oracle import ref_lib as R
-    if not R.available() and name not in golden_names():
+    if ref_lib_or_none() is None and name not in golden_names():
         pytest.skip("case not in tests/golden/hpss.npz and no reference build")
-    got = reference_outputs([name])[name]
+    out = GOLD.outputs({_key(name, k) for k in range(2)})
+    got = [out.get(_key(name, k)) for k in range(2)]
     want = HO.oracle_case(name, kw)
     for k, (g, w) in enumerate(zip(got, want)):
         assert (g is None) == (w is None), (name, k)
@@ -55,16 +59,7 @@ def test_oracle_matches_reference(name, kw):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/hpss.npz")
-    g = np.load(GOLD)
-    assert {k.split("__")[0] for k in g.files} == golden_names()
-    for n, outs in reference_outputs(sorted(golden_names())).items():
-        for k, o in enumerate(outs):
-            assert (o is None) == (_key(n, k) not in g.files), (n, k)
-            if o is not None:
-                assert np.array_equal(g[_key(n, k)], o), (n, k)
+    GOLD.check_file()
 
 
 def test_golden_file_covers_the_rules():
@@ -72,7 +67,7 @@ def test_golden_file_covers_the_rules():
     assert {"hamm_n10_defaults", "hann_n9", "rect_n9", "hamm_n6", "hamm_n6_orders_121_45", "h_order_1", "p_order_1",
             "orders_1_1", "orders_even_zero", "orders_negative_even", "t1", "t1_tail", "h_only", "p_only",
             "init_buffers"} <= names
-    assert os.path.getsize(GOLD) < 300 * 1024
+    assert os.path.getsize(GOLD.path) < 300 * 1024
 
 
 ORDERS = [None, -3, 0, 1, 2, 3, 20, 21, 31, 255, 383, 385, 1001]
@@ -146,28 +141,11 @@ def test_refusals(product_lib):
     L.hpssObj_free(None)
 
 
-def _symbols(header):
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b(hpssObj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
 def test_hpss_symbols_exported_and_bound(product_lib):
     from audioflux_b200 import capi
-    names, ext = _symbols("afb200_hpss.h"), _symbols("afb200_ext.h")
-    assert names == {"hpssObj_new", "hpssObj_calDataLength", "hpssObj_hpss", "hpssObj_free", "hpssObj_debug"}
-    assert ext == {"hpssObj_hpssBatch"}
-    declared = set()
-    for h in os.listdir(os.path.join(ROOT, "include")):
-        declared |= _symbols(h)
-    assert declared == names | ext
-    assert set(capi.HPSS_API) == names | ext
-    for n in names | ext:
-        assert hasattr(product_lib, n), n
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        for n in names:
-            assert hasattr(lib, n), n
+    check_symbols(product_lib, "afb200_hpss.h", "hpssObj_", capi.HPSS_API,
+                  {"hpssObj_new", "hpssObj_calDataLength", "hpssObj_hpss", "hpssObj_free", "hpssObj_debug"},
+                  {"hpssObj_hpssBatch"})
 
 
 def test_python_class_checks(product_lib):

@@ -1,17 +1,15 @@
 """NSGT without a GPU: the numpy oracle against the reference build (or its stored outputs in tests/golden/nsgt.npz),
 the column map on the reference's own outputs, and nsgtObj_new of libaudioflux_b200.so (status codes, getters, lengths,
 its -2 refusals) against the reference over the same sweep."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import GOLDEN
 import _nsgt_oracle as NO
+from _parity_kit import GoldenStore, ref_lib_or_none
 
 from oracle import af_oracle as O
 
-GOLD = os.path.join(GOLDEN, "nsgt.npz")
+KINDS = ("lens", "bins", "fre", "offs", "win", "cells", "matrix")
 # the golden file keeps every case's tables, but windows, cells and matrices only of the 2^8 cases (all styles, both
 # banks) and the cells of the docs example; where the reference build exists everything is compared
 GOLDEN_BULKY = ("win", "cells", "matrix")
@@ -21,18 +19,13 @@ def _signal(kw):
     return NO.case_signal(7, 1 << kw["radix2_exp"], kw["samplate"])
 
 
-def reference_outputs():
-    """{key: array} for every case: tables, windows, cells and (small) matrices -- from the reference build when present,
-    else the stored golden file"""
-    from oracle import ref_lib as R
-    if not R.available():
-        if not os.path.exists(GOLD):
-            pytest.skip("no reference build and no tests/golden/nsgt.npz")
-        g = np.load(GOLD)
-        return {k: g[k] for k in g.files}
-    lib = R.get_ref_lib()
+def _live(keys):
+    """{"<case>/<kind>": array}: tables, windows, cells and matrices"""
+    lib = ref_lib_or_none()
     res = {}
     for name, kw in NO.cases():
+        if not any(f"{name}/{kind}" in keys for kind in KINDS):
+            continue
         st, obj = NO.c_new(lib, **kw)
         assert st == 0, name
         _, p = NO.params(**kw)
@@ -40,31 +33,25 @@ def reference_outputs():
         fb = NO.c_filterbank(lib, p)
         re, im, cr, ci = NO.c_nsgt(lib, obj, _signal(kw), kw["num"])
         lib.nsgtObj_free(obj)
-        res[f"{name}/lens"] = t["lens"].astype(np.int32)
-        res[f"{name}/bins"] = t["bins"].astype(np.int32)
-        res[f"{name}/fre"] = t["fre"]
-        res[f"{name}/offs"] = fb["offs"].astype(np.int32)
-        res[f"{name}/win"] = fb["win"][:fb["total_len"]]
-        res[f"{name}/cells"] = np.stack([cr, ci])
-        res[f"{name}/matrix"] = np.stack([re, im])
+        case = dict(lens=t["lens"].astype(np.int32), bins=t["bins"].astype(np.int32), fre=t["fre"],
+                    offs=fb["offs"].astype(np.int32), win=fb["win"][:fb["total_len"]], cells=np.stack([cr, ci]),
+                    matrix=np.stack([re, im]))
+        res.update((f"{name}/{kind}", case[kind]) for kind in KINDS if f"{name}/{kind}" in keys)
     return res
 
 
-def golden_subset(res):
-    """what tests/golden/nsgt.npz keeps of reference_outputs()"""
-    radix = {name: kw["radix2_exp"] for name, kw in NO.cases()}
-    out = {}
-    for k, v in res.items():
-        name, kind = k.split("/")
-        if kind in GOLDEN_BULKY and radix[name] != 8 and (name, kind) != ("docs84", "cells"):
-            continue
-        out[k] = v
-    return out
+def _golden_keys():
+    """what tests/golden/nsgt.npz keeps"""
+    return {f"{name}/{kind}" for name, kw in NO.cases() for kind in KINDS
+            if kind not in GOLDEN_BULKY or kw["radix2_exp"] == 8 or (name, kind) == ("docs84", "cells")}
+
+
+GOLD = GoldenStore("nsgt.npz", _live, _golden_keys)
 
 
 @pytest.fixture(scope="module")
 def ref_out():
-    return reference_outputs()
+    return GOLD.outputs({f"{name}/{kind}" for name, _ in NO.cases() for kind in KINDS})
 
 
 @pytest.mark.parametrize("name,kw", NO.cases(), ids=[c[0] for c in NO.cases()])
@@ -106,14 +93,7 @@ def test_column_map_on_reference_outputs(ref_lib, name, kw):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/nsgt.npz")
-    g = np.load(GOLD)
-    live = golden_subset(reference_outputs())
-    assert sorted(g.files) == sorted(live)
-    for k in g.files:
-        assert np.array_equal(live[k], g[k]), k
+    GOLD.check_file()
 
 
 def _sweep():

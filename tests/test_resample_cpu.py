@@ -4,50 +4,44 @@ rate settings, the refusals (which need no device), the exported and bound symbo
 afb200_ext.h, and the Python classes' argument checks."""
 import itertools
 import os
-import re
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
 import _resample_oracle as RO
+from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
-GOLD = os.path.join(GOLDEN, "resample.npz")
 ORACLE_TOL = 1e-5          # of max|reference output|; worst seen: 1.3e-6 (the reference's float32 sums)
 GOLDEN_MAX_LEN = 20000     # cases with inputs up to this many samples go to the golden file
+CASES = dict(RO.cases())
 
 
-def _key(name, k):
-    return f"{name}__{k}"
-
-
-def reference_outputs(names):
-    """{name: [outputs]} from the reference build when present, else the stored golden file"""
-    from oracle import ref_lib as R
-    cases = dict(RO.cases())
-    if R.available():
-        lib = R.get_ref_lib()
-        return {n: RO.c_case(lib, n, cases[n]) for n in names}
-    if not os.path.exists(GOLD):
-        pytest.skip("no reference build and no tests/golden/resample.npz")
-    g = np.load(GOLD)
-    out = {}
-    for n in names:
-        ks = sorted((int(k.split("__")[1]), k) for k in g.files if k.split("__")[0] == n)
-        out[n] = [g[k] for _, k in ks]
-    return out
+def _keys(name):
+    """one key per call of the case: one, or one per chunk in continue mode"""
+    return [f"{name}__{k}" for k in range(len(CASES[name].get("chunks", [None])))]
 
 
 def golden_names():
     return {name for name, kw in RO.cases() if RO.case_signal(name, kw).size <= GOLDEN_MAX_LEN}
 
 
+def _live(keys):
+    lib = ref_lib_or_none()
+    out = {}
+    for n in sorted({k.split("__")[0] for k in keys}):
+        out.update((k, o) for k, o in zip(_keys(n), RO.c_case(lib, n, CASES[n])) if k in keys)
+    return out
+
+
+GOLD = GoldenStore("resample.npz", _live, lambda: {k for n in golden_names() for k in _keys(n)})
+
+
 @pytest.mark.parametrize("name,kw", RO.cases(), ids=[c[0] for c in RO.cases()])
 def test_oracle_matches_reference(name, kw):
-    from oracle import ref_lib as R
-    if not R.available() and name not in golden_names():
+    if ref_lib_or_none() is None and name not in golden_names():
         pytest.skip("case not in tests/golden/resample.npz and no reference build")
-    got = reference_outputs([name])[name]
+    out = GOLD.outputs(set(_keys(name)))
+    got = [out[k] for k in _keys(name)]
     want = RO.oracle_case(name, kw)
     assert len(got) == len(want), name
     for k, (g, w) in enumerate(zip(got, want)):
@@ -58,15 +52,7 @@ def test_oracle_matches_reference(name, kw):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/resample.npz")
-    g = np.load(GOLD)
-    assert {k.split("__")[0] for k in g.files} == golden_names()
-    live = reference_outputs(sorted(golden_names()))
-    for n, outs in live.items():
-        for k, o in enumerate(outs):
-            assert np.array_equal(g[_key(n, k)], o), (n, k)
+    GOLD.check_file()
 
 
 def test_golden_file_covers_the_rules():
@@ -75,7 +61,7 @@ def test_golden_file_covers_the_rules():
             "ratio_0.37", "ratio_2.5", "chain", "scale_up_init", "len1_down", "len2_up",
             "continue_48000_16000", "continue_44100_48000"} <= names
     assert all(f"win{w}_null" in names for w in range(1, 14))
-    assert os.path.getsize(GOLD) < 400 * 1024
+    assert os.path.getsize(GOLD.path) < 400 * 1024
 
 
 WINDOWS = [dict(), dict(zero_num=16, nbit=7, win_type=4, value=None, roll_off=None),
@@ -180,27 +166,9 @@ def test_refusals(product_lib):
     L.resampleObj_free(o)
 
 
-def _symbols(header):
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b(resampleObj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
 def test_resample_symbols_exported_and_bound(product_lib):
     from audioflux_b200 import capi
-    names, ext = _symbols("afb200_resample.h"), _symbols("afb200_ext.h")
-    assert len(names) == 9 and ext == {"resampleObj_resampleBatch"}
-    declared = set()
-    for h in os.listdir(os.path.join(ROOT, "include")):
-        declared |= _symbols(h)
-    assert declared == names | ext
-    assert set(capi.RESAMPLE_API) == names | ext
-    for n in names | ext:
-        assert hasattr(product_lib, n), n
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        for n in names:
-            assert hasattr(lib, n), n
+    check_symbols(product_lib, "afb200_resample.h", "resampleObj_", capi.RESAMPLE_API, 9, {"resampleObj_resampleBatch"})
 
 
 def test_python_class_checks(product_lib):

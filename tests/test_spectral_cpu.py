@@ -7,13 +7,12 @@ import re
 import numpy as np
 import pytest
 
-from conftest import ROOT, GOLDEN
+from conftest import ROOT
 import _spectral_cases as SC
+from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
 import audioflux_b200 as af
 from audioflux_b200 import capi
-
-GOLD = os.path.join(GOLDEN, "spectral.npz")
 
 
 def _key(setname, mode, vi, part=0):
@@ -29,26 +28,28 @@ def _cases():
                 yield setname, x, ph, fre, mode, vi, name, kw
 
 
-def _reference_outputs():
-    """{key: reference output}: from the reference build when present, else the stored golden file"""
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        res = {}
-        for setname, x, ph, fre, mode, vi, name, kw in _cases():
-            out = SC.call_c(lib, name, x, fre, mode, ph, **kw)
-            for part, o in enumerate(out if isinstance(out, tuple) else (out,)):
+def _keys():
+    return {_key(setname, mode, vi, part) for setname, _, _, _, mode, vi, name, _ in _cases()
+            for part in range(2 if name in SC.TWO_OUTPUTS else 1)}
+
+
+def _live(keys):
+    lib = ref_lib_or_none()
+    res = {}
+    for setname, x, ph, fre, mode, vi, name, kw in _cases():
+        out = SC.call_c(lib, name, x, fre, mode, ph, **kw)
+        for part, o in enumerate(out if isinstance(out, tuple) else (out,)):
+            if _key(setname, mode, vi, part) in keys:
                 res[_key(setname, mode, vi, part)] = o
-        return res
-    if not os.path.exists(GOLD):
-        pytest.skip("no reference build and no tests/golden/spectral.npz")
-    g = np.load(GOLD)
-    return {k: g[k] for k in g.files}
+    return res
+
+
+GOLD = GoldenStore("spectral.npz", _live, _keys, equal=lambda a, b: SC.agree(a, b, exact=True) is None)
 
 
 @pytest.fixture(scope="module")
 def ref_out():
-    return _reference_outputs()
+    return GOLD.outputs(_keys())
 
 
 def test_oracle_matches_reference(ref_out):
@@ -64,14 +65,7 @@ def test_oracle_matches_reference(ref_out):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/spectral.npz")
-    g = np.load(GOLD)
-    live = _reference_outputs()
-    assert sorted(g.files) == sorted(live)
-    for k in g.files:
-        assert SC.agree(live[k], g[k], exact=True) is None, k
+    GOLD.check_file()
 
 
 def test_constructor_and_edge_rules(product_lib):
@@ -124,24 +118,9 @@ def test_batch_rejects_bad_requests(product_lib):
     lib.spectralObj_free(obj)
 
 
-def _spectral_declared():
-    src = open(os.path.join(ROOT, "include", "afb200_spectral.h")).read() + \
-        open(os.path.join(ROOT, "include", "afb200_ext.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b(spectralObj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
 def test_spectral_api_declared_and_exported(product_lib):
-    declared = _spectral_declared()
-    assert set(capi.SPECTRAL_API) == declared
-    for name in capi.SPECTRAL_API:
-        assert hasattr(product_lib, name), name
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        for name in capi.SPECTRAL_API:
-            if name != "spectralObj_spectralBatch":
-                assert hasattr(lib, name), name
+    check_symbols(product_lib, "afb200_spectral.h", "spectralObj_", capi.SPECTRAL_API, 35,
+                  {"spectralObj_spectralBatch"})
 
 
 def test_feature_ids_match_header():

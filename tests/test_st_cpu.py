@@ -1,17 +1,12 @@
 """ST / FST without a GPU: the numpy oracle against the reference build (or its stored outputs in tests/golden/st.npz),
 the constructor statuses of both libraries, the exported and bound symbols of include/afb200_st.h, and the Python
 classes' argument checks."""
-import ctypes as C
-import os
-import re
-
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
 import _st_oracle as SO
+from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
-GOLD = os.path.join(GOLDEN, "st.npz")
 ORACLE_TOL = 2e-5          # worst row seen: 5.4e-6 (the reference's float32 FFTs)
 # cases whose output has at most this many complex values go to the golden file.  FST rows repeat each value N/len
 # times and compress well; the limits keep the file near 200 KB while covering the bin-0, Nyquist, bin-list and
@@ -27,21 +22,14 @@ def _signal(kind, kw):
     return SO.case_signal(3 if kind == "st" else 4, 1 << kw["radix2_exp"])
 
 
-def reference_outputs(names=None):
-    """{name: [re, im]} from the reference build when present, else the stored golden file"""
-    from oracle import ref_lib as R
-    if not R.available():
-        if not os.path.exists(GOLD):
-            pytest.skip("no reference build and no tests/golden/st.npz")
-        g = np.load(GOLD)
-        return {k: g[k] for k in g.files}
-    lib = R.get_ref_lib()
+def _live(names):
+    """{name: [re, im] stacked}"""
+    lib = ref_lib_or_none()
     res = {}
     for kind, name, kw in _cases():
-        if names is not None and name not in names:
-            continue
-        x = _signal(kind, kw)
-        res[name] = np.stack(SO.c_st_case(lib, kw, x) if kind == "st" else SO.c_fst_case(lib, kw, x))
+        if name in names:
+            x = _signal(kind, kw)
+            res[name] = np.stack(SO.c_st_case(lib, kw, x) if kind == "st" else SO.c_fst_case(lib, kw, x))
     return res
 
 
@@ -55,12 +43,14 @@ def golden_names():
     return out
 
 
+GOLD = GoldenStore("st.npz", _live, golden_names)
+
+
 @pytest.mark.parametrize("kind,name,kw", _cases(), ids=[c[1] for c in _cases()])
 def test_oracle_matches_reference(kind, name, kw):
-    from oracle import ref_lib as R
-    if not R.available() and name not in golden_names():
+    if ref_lib_or_none() is None and name not in golden_names():
         pytest.skip("case not in tests/golden/st.npz and no reference build")
-    got = reference_outputs({name})[name]
+    got = GOLD.outputs({name})[name]
     x = _signal(kind, kw)
     want = SO.oracle_st_case(kw, x) if kind == "st" else SO.fst(x, kw["min_index"], kw["max_index"])
     assert got.shape[1:] == want.shape
@@ -69,14 +59,7 @@ def test_oracle_matches_reference(kind, name, kw):
 
 
 def test_golden_file_matches_reference_build():
-    from oracle import ref_lib as R
-    if not (R.available() and os.path.exists(GOLD)):
-        pytest.skip("needs both the reference build and tests/golden/st.npz")
-    g = np.load(GOLD)
-    assert sorted(g.files) == sorted(golden_names())
-    live = reference_outputs(set(g.files))
-    for k in g.files:
-        assert np.array_equal(live[k], g[k]), k
+    GOLD.check_file()
 
 
 def _st_sweep():
@@ -147,28 +130,10 @@ def test_refusals_above_2e14(product_lib):
         assert b"largest supported is 14" in product_lib.afb200_lastError()
 
 
-def _st_header_symbols():
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "afb200_st.h")).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b((?:st|fst)Obj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
-def _ext_st_symbols():
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "afb200_ext.h")).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"\b((?:st|fst)Obj_[A-Za-z0-9_]*)\s*\(", src)}
-
-
 def test_st_symbols_exported_and_bound(product_lib):
     from audioflux_b200 import capi
-    names, ext = _st_header_symbols(), _ext_st_symbols()
-    assert len(names) == 8 and ext == {"stObj_stBatch", "stObj_getBinLength", "fstObj_fstBatch"}
-    assert set(capi.ST_API) == names | ext
-    for n in names | ext:
-        assert hasattr(product_lib, n), n
-    from oracle import ref_lib as R
-    if R.available():
-        lib = R.get_ref_lib()
-        for n in names:
-            assert hasattr(lib, n), n
+    check_symbols(product_lib, "afb200_st.h", "stObj_|fstObj_", capi.ST_API, 8,
+                  {"stObj_stBatch", "stObj_getBinLength", "fstObj_fstBatch"})
 
 
 def test_python_class_checks(product_lib):

@@ -14,25 +14,19 @@ name, power limit and max SM clock; and where oracle/_ref exists the reference b
 Prints one JSON line per workload.
 
     python tools/bench_hpss.py [--steps 10] [--warmup 2] [--workloads n12_32k,...] [--out results.json]"""
-import argparse
-import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.realpath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.dirname(os.path.realpath(__file__)))
+import _bench_kit as K  # noqa: E402
 
 import torch  # noqa: E402
 
 import audioflux_b200 as af  # noqa: E402
 import _hpss_oracle as HO  # noqa: E402
 
-HBM = 3.35e12
 RUN = 32                     # outputs per median run of k_hpss_mask (its frame tile and its bin run)
 WORKLOADS = {
     "n12_32k": dict(clips=1024, seconds=5, sr=32000, r=12, h=21, p=31),
@@ -42,35 +36,6 @@ WORKLOADS = {
 KERNELS = ("k_hpss_mask", "k_stft_generic", "k_istft_frames", "k_istft_ola")
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return out[torch.cuda.current_device()] if out else torch.cuda.get_device_name()
-    except Exception:  # noqa: BLE001
-        return torch.cuda.get_device_name()
-
-
-def kernel_times(fn, calls=3):
-    """device ms per call of each kernel (all its launches in the call), from torch.profiler"""
-    from torch.profiler import profile, ProfilerActivity
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(calls):
-            fn()
-        torch.cuda.synchronize()
-    per = {}
-    for e in prof.key_averages():
-        us = getattr(e, "device_time_total", None)
-        if us is None:
-            us = e.cuda_time_total
-        if us <= 0 or e.key.startswith(("cuda",)):
-            continue
-        key = next((k for k in KERNELS if k in e.key), e.key[:60])
-        per[key] = per.get(key, 0) + us / 1e3 / calls
-    return per
-
-
 def median_visits(order):
     """window elements visited per output along one axis: a run's first window by rank counts (at most order^2), then
     one pass of order elements for each of the other RUN - 1 outputs; an order of 1 visits nothing"""
@@ -78,16 +43,13 @@ def median_visits(order):
 
 
 def reference_ms_per_clip(w, x, clips=1):
-    from oracle import ref_lib as R
-    if not R.available():
-        return None
-    lib = R.get_ref_lib()
-    t0 = time.perf_counter()
-    for i in range(clips):                 # construction included, as a user pays it
-        st, o = HO.c_new(lib, w["r"], None, None, w["h"], w["p"])
-        HO.c_hpss(lib, o, x[i])
-        lib.hpssObj_free(o)
-    return (time.perf_counter() - t0) * 1e3 / clips
+    def prepare(lib):
+        def clip(i):                       # construction included, as a user pays it
+            st, o = HO.c_new(lib, w["r"], None, None, w["h"], w["p"])
+            HO.c_hpss(lib, o, x[i])
+            lib.hpssObj_free(o)
+        return clip
+    return K.reference_ms_per_clip(prepare, clips)
 
 
 def run(name, steps, warmup):
@@ -103,66 +65,31 @@ def run(name, steps, warmup):
 
     def fn():
         return obj.hpss_batch(xd)
-    for _ in range(warmup):
-        out = fn()
-    del out
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    times = []
-    for _ in range(steps):
-        e0.record()
-        out = fn()
-        e1.record()
-        e1.synchronize()
-        times.append(e0.elapsed_time(e1))
-        if len(times) < steps:
-            del out
+    times, out = K.event_times(fn, steps, warmup)
     ms = float(np.median(times))
     want = HO.hpss(x[0], w["r"], w["h"], w["p"])
     kw = dict(radix2_exp=w["r"], length=length)
     err = max(max(HO.errors(out[k][0].cpu().numpy(), want[k], kw)) for k in range(2))
     del out
-    per = kernel_times(fn)
+    per = K.kernel_times(fn, KERNELS)
     bins = clips * T * W
     call_bytes = clips * (length + 2 * m) * 4
     mask_bytes = bins * 6 * 4
     res = dict(workload=name, clips=clips, samples=length, frames=T, bins_per_frame=W, fft_length=n,
-               orders=[w["h"], w["p"]], ms_per_call=round(ms, 3), ms_min=round(float(np.min(times)), 3),
-               ms_max=round(float(np.max(times)), 3), kernels_ms_per_call={k: round(v, 3) for k, v in per.items()},
+               orders=[w["h"], w["p"]], **K.ms_stats(times, 3),
+               kernels_ms_per_call={k: round(v, 3) for k, v in per.items()},
                call_compulsory_bytes=call_bytes, call_GBps=round(call_bytes / (ms * 1e-3) / 1e9, 1),
                median_visits_per_bin=round(median_visits(w["h"]) + median_visits(w["p"]), 1),
-               rank_count_per_bin=w["h"] ** 2 + w["p"] ** 2, parity_clip0=err, parity_ok=bool(err <= 1e-4), card=card())
+               rank_count_per_bin=w["h"] ** 2 + w["p"] ** 2, parity_clip0=err, parity_ok=bool(err <= 1e-4), card=K.card())
     k = per.get("k_hpss_mask")
     if k:
         res["mask_compulsory_bytes"] = mask_bytes
         res["mask_GBps"] = round(mask_bytes / (k * 1e-3) / 1e9, 1)
-        res["mask_hbm_share"] = round(mask_bytes / (k * 1e-3) / HBM, 4)
+        res["mask_hbm_share"] = round(mask_bytes / (k * 1e-3) / K.HBM, 4)
         res["stft_istft_ms_per_call"] = round(sum(v for kk, v in per.items() if kk in KERNELS[1:]), 3)
     res["reference_ms_per_clip_1core"] = reference_ms_per_clip(w, x)
     return res
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--workloads", default=",".join(WORKLOADS))
-    ap.add_argument("--out", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_hpss needs a CUDA device")
-    results = []
-    for wname in a.workloads.split(","):
-        results.append(run(wname, a.steps, a.warmup))
-        print(json.dumps(results[-1]), flush=True)
-        torch.cuda.empty_cache()
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(results, f, indent=1)
-    if not all(r["parity_ok"] for r in results):
-        sys.exit("parity gate failed")
-
-
 if __name__ == "__main__":
-    main()
+    K.main(run, ",".join(WORKLOADS), steps=10, warmup=2)

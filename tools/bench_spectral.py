@@ -6,33 +6,19 @@ oracle/_ref is built) and the GPU name and power limit read in the same run.
 
     python tools/bench_spectral.py [--clips 1024] [--steps 20] [--warmup 3]"""
 import argparse
-import ctypes as C
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
-import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.realpath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.dirname(os.path.realpath(__file__)))
+import _bench_kit as K  # noqa: E402
+
+import torch  # noqa: E402
+
 import audioflux_b200 as af  # noqa: E402
 from audioflux_b200 import spectral as SP  # noqa: E402
-
-HBM_TBS = 3.35
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-        name, power = [v.strip() for v in q.split(",")[:2]]
-        return name, power
-    except Exception:   # noqa: BLE001
-        return torch.cuda.get_device_name(0), "unknown"
 
 
 def timed(fn, steps, warmup):
@@ -80,24 +66,19 @@ def main():
         "one_call_per_feature_ms": {k: round(v, 3) for k, v in per.items()},
         "compulsory_GB": round((in_bytes + out_bytes) / 1e9, 3),
         "all_features_TBps": round((in_bytes + out_bytes) / all_ms / 1e9, 3),
-        "fraction_of_3.35TBps": round((in_bytes + out_bytes) / all_ms / 1e9 / HBM_TBS, 3),
+        "fraction_of_3.35TBps": round((in_bytes + out_bytes) / all_ms / 1e-3 / K.HBM, 3),
     }
-    gname, power = gpu_info()
-    res["gpu"], res["power_limit"] = gname, power
+    card = [v.strip() for v in K.card().split(",")]
+    res["gpu"], res["power_limit"] = card[0], card[1] if len(card) > 1 else "unknown"
 
-    ref_path = os.path.join(ROOT, "oracle", "_ref", "libaudioflux_ref.so")
-    if os.path.exists(ref_path) and a.ref_clips > 0:
-        from oracle import ref_lib as R
+    if a.ref_clips > 0:
         import _spectral_cases as SC
-        lib = R.get_ref_lib()
         xs = x[:a.ref_clips].cpu().numpy()
-        t0 = time.perf_counter()
-        for b in range(a.ref_clips):
-            for n, kw in feats:
-                SC.call_c(lib, n, xs[b], fre, "full", None, **kw)
-        dt = (time.perf_counter() - t0) / a.ref_clips
-        res["reference_cpu_ms_per_clip_all_features"] = round(dt * 1e3, 2)
-        res["reference_cpu_extrapolated_ms_for_workload"] = round(dt * 1e3 * B, 1)
+        ms = K.reference_ms_per_clip(
+            lambda lib: lambda b: [SC.call_c(lib, n, xs[b], fre, "full", None, **kw) for n, kw in feats], a.ref_clips)
+        if ms is not None:
+            res["reference_cpu_ms_per_clip_all_features"] = round(ms, 2)
+            res["reference_cpu_extrapolated_ms_for_workload"] = round(ms * B, 1)
     print(json.dumps(res))
 
 

@@ -37,22 +37,35 @@ def compile_cubin(src, nvcc, out_dir):
     return cubin, r.stderr
 
 
+def ptxas_entries(log):
+    """{entry function: (registers, stack frame bytes, spill store bytes, spill load bytes)} from a -Xptxas -v log."""
+    rep, entry, props = {}, None, None
+    for line in log.splitlines():
+        m = re.search(r"Compiling entry function '(\S+)'", line)
+        if m:
+            entry = m.group(1)
+            rep[entry] = [0, 0, 0, 0]
+            continue
+        m = re.search(r"Function properties for (\S+)", line)
+        if m:
+            props = m.group(1)
+            continue
+        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
+        if m and props in rep:
+            rep[props][1:] = [int(v) for v in m.groups()]
+        m = re.search(r"Used (\d+) registers", line)
+        if m and entry is not None:
+            rep[entry][0] = int(m.group(1))
+    return {k: tuple(v) for k, v in rep.items()}
+
+
 def ptxas_report(log, kernel="k_mfcc_fused2"):
     """{CT: (registers, spill store bytes, spill load bytes)} of kernel<CT> from the -Xptxas -v log."""
-    rep, ct = {}, None
-    for line in log.splitlines():
-        m = re.search(kernel + r"ILi(\d+)E", line)
-        if "Compiling entry function" in line:
-            ct = int(m.group(1)) if m else None
-            continue
-        if ct is None:
-            continue
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
+    rep = {}
+    for name, (regs, _, st, ld) in ptxas_entries(log).items():
+        m = re.search(kernel + r"ILi(\d+)E", name)
         if m:
-            rep.setdefault(ct, [0, 0, 0])[1:] = [int(m.group(1)), int(m.group(2))]
-        m = re.search(r"Used (\d+) registers", line)
-        if m:
-            rep.setdefault(ct, [0, 0, 0])[0] = int(m.group(1))
+            rep[int(m.group(1))] = (regs, st, ld)
     return rep
 
 

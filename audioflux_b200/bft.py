@@ -6,7 +6,7 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, BandAxis, FrameAxis, as_f32, np_ptr, split_batch, swap_last2
+from .base import MEM_DEVICE, Base, BandAxis, Batch, FrameAxis, as_f32, band_range, is_torch, np_ptr, per_clip, swap_last2
 from .capi import opt_int, opt_float
 from .lib import check
 from .types import (WindowType, SpectralFilterBankScaleType, SpectralFilterBankStyleType,
@@ -24,10 +24,7 @@ class BFT(BandAxis, FrameAxis, Base):
         self.fft_length = fft_length = 1 << radix2_exp
         if num > fft_length // 2 + 1:
             raise ValueError(f"num={num} is too large")
-        if low_fre is None:
-            low_fre = 32.703196 if enum_value(scale_type) in (5, 6) else 0.0
-        if high_fre is None:
-            high_fre = samplate / 2
+        low_fre, high_fre = band_range(low_fre, high_fre, scale_type, samplate)
         if slide_length is None:
             slide_length = fft_length // 4
         self.num, self.radix2_exp, self.samplate = num, radix2_exp, samplate
@@ -37,26 +34,20 @@ class BFT(BandAxis, FrameAxis, Base):
         self.data_type = data_type
         self.result_type = 0
         self.is_reassign, self.is_temporal = is_reassign, is_temporal
-        status = self._lib.bftObj_new(
-            C.byref(self._obj), num, radix2_exp, opt_int(samplate), opt_float(low_fre),
-            opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(window_type)),
-            opt_int(slide_length), opt_int(enum_value(scale_type)), opt_int(enum_value(style_type)),
-            opt_int(enum_value(normal_type)), opt_int(enum_value(data_type)),
-            opt_int(int(is_reassign)), opt_int(int(is_temporal)))
-        if status != 0 or not self._obj:
-            raise ValueError(f"bftObj_new failed with status {status}")
-        self._is_created = True
+        self._new("bftObj_new", "bftObj_free", num, radix2_exp, opt_int(samplate), opt_float(low_fre),
+                  opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(window_type)),
+                  opt_int(slide_length), opt_int(enum_value(scale_type)), opt_int(enum_value(style_type)),
+                  opt_int(enum_value(normal_type)), opt_int(enum_value(data_type)),
+                  opt_int(int(is_reassign)), opt_int(int(is_temporal)))
 
     def cal_time_length(self, data_length):
         return self._lib.bftObj_calTimeLength(self._obj, data_length)
 
     def get_fre_band_arr(self):
-        p = self._lib.bftObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.num,)).copy()
+        return self._floats("bftObj_getFreBandArr", self.num)
 
     def get_bin_band_arr(self):
-        p = self._lib.bftObj_getBinBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int)), shape=(self.num,)).copy()
+        return self._ints("bftObj_getBinBandArr", self.num)
 
     def get_filter_bank_arr(self):
         """Additive: dense bank [num, fft_length//2+1] the device kernels consume."""
@@ -100,49 +91,32 @@ class BFT(BandAxis, FrameAxis, Base):
         x = as_f32(data_arr)
         if x.shape[-1] < self.fft_length:
             raise ValueError(f"radix2_exp={self.radix2_exp} is too large for data length {x.shape[-1]}")
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, x.shape[-1])
-        outs = []
-        for i in range(x2.shape[0]):
-            re, im = self.bft_planes(x2[i], result_type)
-            outs.append(re if result_type else re + 1j * im)
-        out = np.stack(outs).reshape(*lead, -1, self.num)
-        return swap_last2(out)
+        re, im = per_clip(lambda clip: self.bft_planes(clip, result_type), x)
+        return swap_last2(re if result_type else re + 1j * im)
 
     # ---- additive batched / device-pointer entry points (include/afb200_ext.h) ----
     def bft_batch(self, data, result_type=1):
         """data [B, L] (numpy host | torch cuda) -> [B, T, num] real, or (re, im) for result_type 0."""
-        fn = self._require_ext("bftObj_bftBatch")
         if result_type != self.result_type:
             self.set_result_type(result_type)
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
-        re = alloc(B, T, self.num)
-        im = alloc(B, T, self.num) if result_type == 0 else None
-        check(fn(self._obj, ptr(x2), L, B, ptr(re), ptr(im) if im is not None else C.c_void_p(None),
-                 kind, stream), "bftObj_bftBatch")
-        re = re.reshape(*lead, T, self.num)
-        return re if result_type else (re, im.reshape(*lead, T, self.num))
+        b = Batch(data)
+        T = self.cal_time_length(b.n)
+        re = b.alloc(b.rows, T, self.num)
+        im = b.alloc(b.rows, T, self.num) if result_type == 0 else None
+        self._call("bftObj_bftBatch", b, b.x, b.n, b.rows, re, im)
+        return b.shaped(re) if result_type else (b.shaped(re), b.shaped(im))
 
     def mfcc_batch(self, data, cc_num=13, rectify_type=CepstralRectifyType.LOG, out=None):
         """Fused STFT -> |.|^2 (or |.|) -> bank -> log10/cbrt -> DCT-II(ortho) -> first cc_num.
         data [B, L] -> [B, T, cc_num].  Equals bft(result_type=1) followed by XXCC.xxcc.
         Host arrays go through the library's chunked copy-in / transform / copy-out pipeline; pass page-locked arrays
         (and a page-locked `out`) to run it at PCIe speed."""
-        fn = self._require_ext("bftObj_mfccBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
+        b = Batch(data)
+        T = self.cal_time_length(b.n)
         if out is None:
-            out = alloc(B, T, cc_num)
-        elif tuple(out.shape) != (B, T, cc_num) or not (out.flags["C_CONTIGUOUS"] if hasattr(out, "flags") else out.is_contiguous()):
-            raise ValueError(f"out must be a contiguous float32 array of shape {(B, T, cc_num)}")
-        check(fn(self._obj, ptr(x2), L, B, cc_num, enum_value(rectify_type), ptr(out), kind, stream),
-              "bftObj_mfccBatch")
-        return out.reshape(*lead, T, cc_num)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.bftObj_free(self._obj)
-            self._is_created = False
+            out = b.alloc(b.rows, T, cc_num)
+        elif (is_torch(out) != (b.kind == MEM_DEVICE) or tuple(out.shape) != (b.rows, T, cc_num)
+              or not (out.flags["C_CONTIGUOUS"] if hasattr(out, "flags") else out.is_contiguous())):
+            raise ValueError(f"out must be a contiguous float32 array of shape {(b.rows, T, cc_num)} in the memory of data")
+        self._call("bftObj_mfccBatch", b, b.x, b.n, b.rows, cc_num, enum_value(rectify_type), out)
+        return b.shaped(out)

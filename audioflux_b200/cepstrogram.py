@@ -12,8 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, FrameAxis, split_batch, swap_last2
-from .lib import check
+from .base import Base, Batch, FrameAxis, swap_last2
 from .types import WindowType, enum_value
 
 
@@ -23,12 +22,8 @@ class Cepstrogram(FrameAxis, Base):
         self.radix2_exp, self.samplate = radix2_exp, samplate
         self.window_type, self.slide_length = window_type, slide_length
         self.fft_length = 1 << radix2_exp
-        status = self._lib.cepstrogramObj_new(C.byref(self._obj), radix2_exp, C.byref(C.c_int(enum_value(window_type))),
-                                              C.byref(C.c_int(slide_length)))
-        if status != 0 or not self._obj:
-            msg = f": {self._lib.afb200_lastError().decode()}" if self._is_product and status == -2 else ""
-            raise ValueError(f"cepstrogramObj_new failed with status {status}{msg}")
-        self._is_created = True
+        self._new("cepstrogramObj_new", "cepstrogramObj_free", radix2_exp, C.byref(C.c_int(enum_value(window_type))),
+                  C.byref(C.c_int(slide_length)))
 
     def cal_time_length(self, data_length):
         return self._lib.cepstrogramObj_calTimeLength(self._obj, int(data_length))
@@ -40,13 +35,8 @@ class Cepstrogram(FrameAxis, Base):
         if not 1 <= cep_num <= self.fft_length // 2:
             raise ValueError(f"cep_num={cep_num} must be in 1 .. fft_length/2 = {self.fft_length // 2}")
 
-    def _outputs(self, alloc, lead, rows, want):
-        width = self.fft_length // 2 + 1
-        return [alloc(*lead, rows, width) if w else None for w in want]
-
-    def _call(self, name, args, out, ptr, kind, stream):
-        fn = self._require_ext(name)
-        check(fn(self._obj, *args, *[ptr(o) if o is not None else None for o in out], kind, stream), name)
+    def _outputs(self, b, shape, want):
+        return [b.alloc(*shape, self.fft_length // 2 + 1) if w else None for w in want]
 
     def cepstrogram_batch(self, data, cep_num=4, cep=True, env=True, det=True):
         """data [..., n] (numpy host | torch cuda) -> (cepstrums, envelope, details), each [..., time, fft_length/2+1]
@@ -54,13 +44,12 @@ class Cepstrogram(FrameAxis, Base):
         self._check_cep_num(cep_num)
         if not (cep or env or det):
             raise ValueError("request at least one of cep, env, det")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        batch, n = x2.shape
-        t = self.cal_time_length(n)
-        out = self._outputs(alloc, (batch,), t, (cep, env, det))
-        if batch and t:
-            self._call("cepstrogramObj_cepstrogramBatch", (cep_num, ptr(x2), n, batch), out, ptr, kind, stream)
-        return tuple(o.reshape(*lead, *o.shape[1:]) if o is not None else None for o in out)
+        b = Batch(data)
+        t = self.cal_time_length(b.n)
+        out = self._outputs(b, (b.rows, t), (cep, env, det))
+        if b.rows and t:
+            self._call("cepstrogramObj_cepstrogramBatch", b, cep_num, b.x, b.n, b.rows, *out)
+        return tuple(map(b.shaped, out))
 
     def cepstrogram2_batch(self, m_real, m_imag, cep_num=4, cep=True, env=True, det=True):
         """STFT planes [..., rows, width], width fft_length (the mirrored layout of the legacy STFT) or
@@ -69,19 +58,14 @@ class Cepstrogram(FrameAxis, Base):
         self._check_cep_num(cep_num)
         if not (cep or env or det):
             raise ValueError("request at least one of cep, env, det")
-        re2, lead, kind, ptr, stream, alloc = split_batch(m_real)
-        im2, _, kind2, _, _, _ = split_batch(m_imag)
-        if kind2 != kind or tuple(im2.shape) != tuple(re2.shape):
-            raise ValueError("m_real and m_imag must have the same shape and live in the same memory")
-        width = re2.shape[-1]
-        if width not in (self.fft_length, self.fft_length // 2 + 1):
-            raise ValueError(f"plane width {width} must be fft_length={self.fft_length} or fft_length/2+1")
-        rows = re2.shape[0]
-        out = self._outputs(alloc, (), rows, (cep, env, det))
-        if rows:
-            self._call("cepstrogramObj_cepstrogram2Batch", (cep_num, ptr(re2), ptr(im2), rows, width), out, ptr, kind,
-                       stream)
-        return tuple(o.reshape(*lead, o.shape[-1]) if o is not None else None for o in out)
+        b = Batch(m_real)
+        im = b.second(m_imag, "m_imag")
+        if b.n not in (self.fft_length, self.fft_length // 2 + 1):
+            raise ValueError(f"plane width {b.n} must be fft_length={self.fft_length} or fft_length/2+1")
+        out = self._outputs(b, (b.rows,), (cep, env, det))
+        if b.rows:
+            self._call("cepstrogramObj_cepstrogram2Batch", b, cep_num, b.x, im, b.rows, b.n, *out)
+        return tuple(map(b.shaped, out))
 
     def cepstrogram(self, data_arr, cep_num=4):
         """data_arr [..., n] -> (cepstrums, envelope, details), each [..., fft_length/2+1, time] float32"""
@@ -89,8 +73,3 @@ class Cepstrogram(FrameAxis, Base):
         if data_arr.ndim == 0:
             raise ValueError('Audio data must have at least one dimension')
         return tuple(swap_last2(o) for o in self.cepstrogram_batch(data_arr, cep_num))
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.cepstrogramObj_free(self._obj)
-            self._is_created = False

@@ -2,17 +2,13 @@
 C: src/cqt_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, BandAxis, FrameAxis, as_f32, np_ptr, split_batch, swap_last2
+from .base import C1_HZ, Base, BandAxis, Batch, FrameAxis, as_f32, np_ptr, per_clip, swap_last2
 from .capi import opt_int, opt_float
 from .lib import check
 from .types import (WindowType, SpectralFilterBankNormalType, SpectralDataType, ChromaDataNormalType,
                     CepstralRectifyType, enum_value)
-
-C1_HZ = 32.703196
 
 
 class CQT(BandAxis, FrameAxis, Base):
@@ -27,14 +23,10 @@ class CQT(BandAxis, FrameAxis, Base):
         self.bin_per_octave, self.factor, self.beta, self.thresh = bin_per_octave, factor, beta, thresh
         self.window_type, self.slide_length = window_type, slide_length
         self.normal_type, self.is_scale = normal_type, is_scale
-        status = self._lib.cqtObj_newWith(
-            C.byref(self._obj), num, opt_int(samplate), opt_float(low_fre), opt_int(bin_per_octave),
-            opt_float(factor), opt_float(beta), opt_float(thresh), opt_int(enum_value(window_type)),
-            opt_int(slide_length), opt_int(int(is_continue)), opt_int(enum_value(normal_type)), opt_int(int(is_scale)))
         self.is_continue = is_continue
-        if status != 0 or not self._obj:
-            raise ValueError(f"cqtObj_newWith failed with status {status}")
-        self._is_created = True
+        self._new("cqtObj_newWith", "cqtObj_free", num, opt_int(samplate), opt_float(low_fre), opt_int(bin_per_octave),
+                  opt_float(factor), opt_float(beta), opt_float(thresh), opt_int(enum_value(window_type)),
+                  opt_int(slide_length), opt_int(int(is_continue)), opt_int(enum_value(normal_type)), opt_int(int(is_scale)))
         self.fft_length = self.get_fft_length()
         if self.slide_length is None:
             self.slide_length = self.fft_length // 4
@@ -46,8 +38,7 @@ class CQT(BandAxis, FrameAxis, Base):
         return self._lib.cqtObj_getFFTLength(self._obj)
 
     def get_fre_band_arr(self):
-        p = self._lib.cqtObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.num,)).copy()
+        return self._floats("cqtObj_getFreBandArr", self.num)
 
     def set_scale(self, flag=True):
         self._lib.cqtObj_setScale(self._obj, int(flag))
@@ -85,26 +76,16 @@ class CQT(BandAxis, FrameAxis, Base):
 
     def cqt(self, data_arr):
         """-> complex [..., num, T] as cqt.py:107-150."""
-        x = as_f32(data_arr)
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, x.shape[-1])
-        outs = []
-        for i in range(x2.shape[0]):
-            re, im = self.cqt_planes(x2[i])
-            outs.append(re + 1j * im)
-        out = np.stack(outs).reshape(*lead, -1, self.num)
-        return swap_last2(out)
+        re, im = per_clip(self.cqt_planes, as_f32(data_arr))
+        return swap_last2(re + 1j * im)
 
     def cqt_batch(self, data):
         """Additive: data [B, L] (numpy host | torch cuda) -> (re, im) each [B, T, num]."""
-        fn = self._require_ext("cqtObj_cqtBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
-        re = alloc(B, T, self.num)
-        im = alloc(B, T, self.num)
-        check(fn(self._obj, ptr(x2), L, B, ptr(re), ptr(im), kind, stream), "cqtObj_cqtBatch")
-        return re.reshape(*lead, T, self.num), im.reshape(*lead, T, self.num)
+        b = Batch(data)
+        T = self.cal_time_length(b.n)
+        re, im = b.alloc(b.rows, T, self.num), b.alloc(b.rows, T, self.num)
+        self._call("cqtObj_cqtBatch", b, b.x, b.n, b.rows, re, im)
+        return b.shaped(re), b.shaped(im)
 
     def chroma_planes(self, re, im, chroma_num=12, data_type=SpectralDataType.POWER,
                       norm_type=ChromaDataNormalType.MAX):
@@ -128,13 +109,11 @@ class CQT(BandAxis, FrameAxis, Base):
     def chroma_batch(self, re, im, chroma_num=12, data_type=SpectralDataType.POWER,
                      norm_type=ChromaDataNormalType.MAX):
         """Additive: planes [..., T, num] (numpy host | torch cuda) -> [..., T, chroma_num]."""
-        fn = self._require_ext("cqtObj_chromaBatch")
-        r2, lead, kind, ptr, stream, alloc = split_batch(re)
-        i2 = split_batch(im)[0]
-        out = alloc(r2.shape[0], chroma_num)
-        check(fn(self._obj, ptr(r2), ptr(i2), r2.shape[0], chroma_num, enum_value(data_type), enum_value(norm_type),
-                 ptr(out), kind, stream), "cqtObj_chromaBatch")
-        return out.reshape(*lead, chroma_num)
+        b = Batch(re)
+        im = b.second(im, "im")
+        out = b.alloc(b.rows, chroma_num)
+        self._call("cqtObj_chromaBatch", b, b.x, im, b.rows, chroma_num, enum_value(data_type), enum_value(norm_type), out)
+        return b.shaped(out)
 
     def cqcc_planes(self, m_tn, cc_num=13, rectify_type=CepstralRectifyType.LOG):
         """Raw C layout: [T, num] of the LAST cqt call -> [T, cc_num] (cqtObj_cqcc, src/cqt_algorithm.c:602-660)."""
@@ -152,12 +131,10 @@ class CQT(BandAxis, FrameAxis, Base):
 
     def cqcc_batch(self, m_tn, cc_num=13, rectify_type=CepstralRectifyType.LOG):
         """Additive: [..., T, num] (numpy host | torch cuda) -> [..., T, cc_num]."""
-        fn = self._require_ext("cqtObj_cqccBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        out = alloc(x2.shape[0], cc_num)
-        check(fn(self._obj, ptr(x2), x2.shape[0], cc_num, enum_value(rectify_type), ptr(out), kind, stream),
-              "cqtObj_cqccBatch")
-        return out.reshape(*lead, cc_num)
+        b = Batch(m_tn)
+        out = b.alloc(b.rows, cc_num)
+        self._call("cqtObj_cqccBatch", b, b.x, b.rows, cc_num, enum_value(rectify_type), out)
+        return b.shaped(out)
 
     def cqhc_planes(self, m_tn, hc_num=20):
         """Raw C layout: [T, num] of the LAST cqt call -> [T, hc_num] (cqtObj_cqhc, src/cqt_algorithm.c:662-714)."""
@@ -190,21 +167,14 @@ class CQT(BandAxis, FrameAxis, Base):
 
     def cqhc_batch(self, m_tn, hc_num=20):
         """Additive: [..., T, num] (numpy host | torch cuda) -> [..., T, hc_num]."""
-        fn = self._require_ext("cqtObj_cqhcBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        out = alloc(x2.shape[0], hc_num)
-        check(fn(self._obj, ptr(x2), x2.shape[0], int(hc_num), ptr(out), kind, stream), "cqtObj_cqhcBatch")
-        return out.reshape(*lead, hc_num)
+        b = Batch(m_tn)
+        out = b.alloc(b.rows, hc_num)
+        self._call("cqtObj_cqhcBatch", b, b.x, b.rows, int(hc_num), out)
+        return b.shaped(out)
 
     def deconv_batch(self, m_tn):
         """Additive: [..., T, num] (numpy host | torch cuda) -> (timbre, pitch) each [..., T, num]."""
-        fn = self._require_ext("cqtObj_deconvBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        tone, pitch = alloc(*x2.shape), alloc(*x2.shape)
-        check(fn(self._obj, ptr(x2), x2.shape[0], ptr(tone), ptr(pitch), kind, stream), "cqtObj_deconvBatch")
-        return tone.reshape(*lead, x2.shape[-1]), pitch.reshape(*lead, x2.shape[-1])
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.cqtObj_free(self._obj)
-            self._is_created = False
+        b = Batch(m_tn)
+        tone, pitch = b.alloc(b.rows, b.n), b.alloc(b.rows, b.n)
+        self._call("cqtObj_deconvBatch", b, b.x, b.rows, tone, pitch)
+        return b.shaped(tone), b.shaped(pitch)

@@ -47,6 +47,7 @@ int bftObj_new(BFTObj *out, int num, int radix2Exp, int *samplate, float *lowFre
                SpectralFilterBankScaleType *scaleType, SpectralFilterBankStyleType *styleType,
                SpectralFilterBankNormalType *normalType, SpectralDataType *dataType,
                int *isReassign, int *isTemporal) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     int r = radix2Exp ? radix2Exp : 12;

@@ -16,6 +16,7 @@ struct OpaqueCepstrogram {
 };
 
 int cepstrogramObj_new(CepstrogramObj *cepstrogramObj, int radix2Exp, WindowType *windowType, int *slideLength) {
+    af_clear_error();
     if (!cepstrogramObj) return -1;
     *cepstrogramObj = NULL;
     if (radix2Exp < 1 || radix2Exp > 30) {                          /* :68-72 */

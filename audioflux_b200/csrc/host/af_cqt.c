@@ -33,6 +33,7 @@ struct OpaqueCQT {
 int cqtObj_newWith(CQTObj *out, int num, int *samplate, float *minFre, int *binPerOctave, float *factor,
                    float *beta, float *thresh, WindowType *windowType, int *slideLength, int *isContinue,
                    SpectralFilterBankNormalType *normalType, int *isScale) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     int bpo = 12;

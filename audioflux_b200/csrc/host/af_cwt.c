@@ -31,6 +31,7 @@ struct OpaqueCWT {
 int cwtObj_new(CWTObj *out, int num, int radix2Exp, int *samplate, float *lowFre, float *highFre,
                int *binPerOctave, WaveletContinueType *waveletType, SpectralFilterBankScaleType *scaleType,
                float *gamma, float *beta, int *isPad) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (radix2Exp < 1 || radix2Exp > 30) { printf("radix2Exp is error!\n"); return -100; }
@@ -215,6 +216,7 @@ struct OpaquePWT { struct OpaqueCWT c; };
 int pwtObj_new(PWTObj *out, int num, int radix2Exp, int *samplate, float *lowFre, float *highFre, int *binPerOctave,
                SpectralFilterBankScaleType *scaleType, SpectralFilterBankStyleType *styleType,
                SpectralFilterBankNormalType *normalType, int *isPadding) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (radix2Exp < 1 || radix2Exp > 30) { printf("radix2Exp is error!\n"); return -100; }

@@ -22,6 +22,7 @@ struct OpaqueHPSS {
 };
 
 int hpssObj_new(HPSSObj *hpssObj, int radix2Exp, WindowType *windowType, int *slideLength, int *hOrder, int *pOrder) {
+    af_clear_error();
     if (!hpssObj) return 0;
     *hpssObj = NULL;
     HPSSObj s = (HPSSObj)calloc(1, sizeof(struct OpaqueHPSS));

@@ -312,6 +312,7 @@ int nsgtObj_new(NSGTObj *nsgtObj, int num, int radix2Exp, int *samplate, float *
                 int *binPerOctave, int *minLength, NSGTFilterBankType *nsgtFilterBankType,
                 SpectralFilterBankScaleType *filterScaleType, SpectralFilterBankStyleType *filterStyleType,
                 SpectralFilterBankNormalType *filterNormalType) {
+    af_clear_error();
     int minLen = 3, sr = 32000, bpo = 12;
     int bank = NSGTFilterBank_Efficient, scale = SpectralFilterBankScale_Octave;
     int style = SpectralFilterBankStyle_Hann, norm = SpectralFilterBankNormal_BandWidth;

@@ -27,6 +27,7 @@ struct OpaqueReassign {
 
 int reassignObj_new(ReassignObj *out, int radix2Exp, int *samplate, WindowType *windowType, int *slideLength,
                     ReassignType *reType, float *thresh, int *isPadding, int *isContinue) {
+    af_clear_error();
     (void)isContinue;                /* read by nobody in the reference either (reassign_algorithm.c:100, 152) */
     if (!out) return -1;
     *out = NULL;

@@ -68,6 +68,7 @@ static void rs_set_ratio(ResampleObj s, float ratio) {
 
 int resampleObj_newWithWindow(ResampleObj *resampleObj, int *zeroNum, int *nbit, WindowType *winType, float *value,
                               float *rollOff, int *isScale, int *isContinue) {
+    af_clear_error();
     if (!resampleObj) return -1;
     *resampleObj = NULL;
     int z = 64, nb = 9;                                                /* :115-175 */

@@ -33,6 +33,7 @@ static int reads_out(int f) {
 static int planes_of(int f) { return f == AFB200_SPECTRAL_MAX || f == AFB200_SPECTRAL_MEAN || f == AFB200_SPECTRAL_VAR ? 2 : 1; }
 
 int spectralObj_new(SpectralObj *out, int num, float *freBandArr) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (num < 2) { printf("num is error!!!\n"); return -1; }

@@ -29,6 +29,7 @@ int spectrogramObj_new(SpectrogramObj *out, int num, int *samplate, float *lowFr
                        int *radix2Exp, WindowType *windowType, int *slideLength, int *isContinue,
                        SpectralDataType *dataType, SpectralFilterBankScaleType *filterScaleType,
                        SpectralFilterBankStyleType *filterStyleType, SpectralFilterBankNormalType *filterNormalType) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     int r = 12;

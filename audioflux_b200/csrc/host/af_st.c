@@ -50,6 +50,7 @@ static void st_fill_v(STObj s) {
 }
 
 int stObj_new(STObj *stObj, int radix2Exp, int minIndex, int maxIndex, float *factor, float *norm) {
+    af_clear_error();
     if (!stObj) return -1;
     if (radix2Exp < 1) { af_fail(-1, "stObj_new: radix2Exp=%d; at least 1 is needed", radix2Exp); return -1; }
     if (radix2Exp > AF_ST_MAX_EXP) { too_long("stObj_new", radix2Exp); return -2; }
@@ -146,6 +147,7 @@ void stObj_free(STObj s) {
 /* ---------------- FST (fst_algorithm.c) ---------------- */
 
 int fstObj_new(FSTObj *fstObj, int radix2Exp) {
+    af_clear_error();
     if (!fstObj) return -1;
     if (radix2Exp < 3) return -1;                                   /* :67-69 */
     if (radix2Exp > AF_ST_MAX_EXP) { too_long("fstObj_new", radix2Exp); return -2; }

@@ -27,6 +27,7 @@ struct OpaqueSTFT {
 };
 
 int stftObj_new(STFTObj *out, int radix2Exp, WindowType *windowType, int *slideLength, int *isContinue) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (radix2Exp < 1 || radix2Exp > 30) return -100;

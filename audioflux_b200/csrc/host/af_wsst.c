@@ -38,6 +38,7 @@ static int upload_norm(const float *fre, int num, int samplate, float **dNorm) {
 int wsstObj_new(WSSTObj *out, int num, int radix2Exp, int *samplate, float *lowFre, float *highFre, int *binPerOctave,
                 WaveletContinueType *waveletType, SpectralFilterBankScaleType *scaleType, float *gamma, float *beta,
                 float *thresh, int *isPadding) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     float th = 0.001f;
@@ -123,6 +124,7 @@ struct OpaqueSynsq {
 };
 
 int synsqObj_new(SynsqObj *out, int num, int radix2Exp, int *samplate, int *order, float *thresh) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (num < 1 || radix2Exp < 1 || radix2Exp > 30) return -1;

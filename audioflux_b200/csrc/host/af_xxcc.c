@@ -12,6 +12,7 @@ struct OpaqueXXCC {
 };
 
 int xxccObj_new(XXCCObj *out, int num) {
+    af_clear_error();
     if (!out) return -1;
     *out = NULL;
     if (num < 2) { printf("num is error!!!\n"); return -1; }

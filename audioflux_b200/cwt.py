@@ -2,11 +2,9 @@
 C: src/cwt_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, BandAxis, SampleAxis, as_f32, np_ptr, split_batch
+from .base import Base, BandAxis, SampleAxis, as_f32, band_range, fit_length, np_ptr, per_clip
 from .capi import opt_int, opt_float
 from .lib import check
 from .types import WaveletContinueType, SpectralFilterBankScaleType, enum_value
@@ -24,10 +22,7 @@ class CWT(BandAxis, SampleAxis, Base):
         self.fft_length = 1 << radix2_exp
         if num > self.fft_length // 2 + 1:
             raise ValueError(f"num={num} is too large")
-        if low_fre is None:
-            low_fre = 32.703196 if enum_value(scale_type) in (5, 6) else 0.0
-        if high_fre is None:
-            high_fre = samplate / 2
+        low_fre, high_fre = band_range(low_fre, high_fre, scale_type, samplate)
         g0, b0 = _DEFAULT_GAMMA_BETA[enum_value(wavelet_type)]
         gamma = g0 if gamma is None else gamma
         beta = b0 if beta is None else beta
@@ -35,21 +30,15 @@ class CWT(BandAxis, SampleAxis, Base):
         self.low_fre, self.high_fre, self.bin_per_octave = low_fre, high_fre, bin_per_octave
         self.wavelet_type, self.scale_type = wavelet_type, scale_type
         self.gamma, self.beta, self.is_padding = gamma, beta, is_padding
-        status = self._lib.cwtObj_new(
-            C.byref(self._obj), num, radix2_exp, opt_int(samplate), opt_float(low_fre),
-            opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(wavelet_type)),
-            opt_int(enum_value(scale_type)), opt_float(gamma), opt_float(beta), opt_int(int(is_padding)))
-        if status != 0 or not self._obj:
-            raise ValueError(f"cwtObj_new failed with status {status}")
-        self._is_created = True
+        self._new("cwtObj_new", "cwtObj_free", num, radix2_exp, opt_int(samplate), opt_float(low_fre),
+                  opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(wavelet_type)),
+                  opt_int(enum_value(scale_type)), opt_float(gamma), opt_float(beta), opt_int(int(is_padding)))
 
     def get_fre_band_arr(self):
-        p = self._lib.cwtObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.num,)).copy()
+        return self._floats("cwtObj_getFreBandArr", self.num)
 
     def get_bin_band_arr(self):
-        p = self._lib.cwtObj_getBinBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int)), shape=(self.num,)).copy()
+        return self._ints("cwtObj_getBinBandArr", self.num)
 
     def cwt_planes(self, data_arr):
         """Raw C layout: (re, im) each [num, N], row 0 = highest band."""
@@ -63,19 +52,8 @@ class CWT(BandAxis, SampleAxis, Base):
 
     def cwt(self, data_arr):
         """-> complex [..., num, N] low->high frequency rows, as cwt.py:236-278."""
-        x = as_f32(data_arr)
-        N = self.fft_length
-        if x.shape[-1] > N:
-            x = x[..., :N]
-        elif x.shape[-1] < N:
-            x = np.concatenate([x, np.zeros((*x.shape[:-1], N - x.shape[-1]), np.float32)], axis=-1)
-        lead = x.shape[:-1]
-        x2 = np.ascontiguousarray(x).reshape(-1, N)
-        outs = []
-        for i in range(x2.shape[0]):
-            re, im = self.cwt_planes(x2[i])
-            outs.append((re + 1j * im)[::-1])
-        return np.ascontiguousarray(np.stack(outs).reshape(*lead, self.num, N))
+        re, im = per_clip(self.cwt_planes, fit_length(data_arr, self.fft_length, warn=False))
+        return np.ascontiguousarray((re + 1j * im)[..., ::-1, :])
 
     def ccwt(self, data_arr):
         """Continuous CWT of long audio (reference: cwt.py:280-320): windows of 2**radix2_exp samples every half window, the
@@ -119,27 +97,11 @@ class CWT(BandAxis, SampleAxis, Base):
 
     def cwt_det_batch(self, data):
         """Additive: data [B, N] (numpy host | torch cuda) -> (re, im) each [B, num, N] of the derivative transform."""
-        fn = self._require_ext("cwtObj_cwtDetBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, N = x2.shape
-        if N != self.fft_length:
-            raise ValueError(f"data length must be 2**radix2_exp = {self.fft_length}")
-        re = alloc(B, self.num, N)
-        im = alloc(B, self.num, N)
-        check(fn(self._obj, ptr(x2), B, ptr(re), ptr(im), kind, stream), "cwtObj_cwtDetBatch")
-        return re.reshape(*lead, self.num, N), im.reshape(*lead, self.num, N)
+        return self._window_batch("cwtObj_cwtDetBatch", data)
 
     def cwt_batch(self, data):
         """Additive: data [B, N] (numpy host | torch cuda) -> (re, im) each [B, num, N] (C row order)."""
-        fn = self._require_ext("cwtObj_cwtBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, N = x2.shape
-        if N != self.fft_length:
-            raise ValueError(f"data length must be 2**radix2_exp = {self.fft_length}")
-        re = alloc(B, self.num, N)
-        im = alloc(B, self.num, N)
-        check(fn(self._obj, ptr(x2), B, ptr(re), ptr(im), kind, stream), "cwtObj_cwtBatch")
-        return re.reshape(*lead, self.num, N), im.reshape(*lead, self.num, N)
+        return self._window_batch("cwtObj_cwtBatch", data)
 
     def get_filter_bank_arr(self):
         fn = self._require_ext("cwtObj_getFilterBankArr")
@@ -148,8 +110,3 @@ class CWT(BandAxis, SampleAxis, Base):
         out = np.zeros((self.num, width), np.float32)
         check(fn(self._obj, np_ptr(out)), "cwtObj_getFilterBankArr")
         return out
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.cwtObj_free(self._obj)
-            self._is_created = False

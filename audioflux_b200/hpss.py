@@ -10,8 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, split_batch
-from .lib import check
+from .base import Base, Batch
 from .types import WindowType, enum_value
 
 __all__ = ["HPSS"]
@@ -28,12 +27,8 @@ class HPSS(Base):
         self.slide_length = slide_length
         self.h_order = h_order
         self.p_order = p_order
-        status = self._lib.hpssObj_new(C.byref(self._obj), int(radix2_exp), C.byref(C.c_int(enum_value(window_type))),
-                                       C.byref(C.c_int(int(slide_length))), C.byref(C.c_int(int(h_order))),
-                                       C.byref(C.c_int(int(p_order))))
-        if status != 0 or not self._obj:
-            raise ValueError(f"hpssObj_new failed with status {status}")
-        self._is_created = True
+        self._new("hpssObj_new", "hpssObj_free", int(radix2_exp), C.byref(C.c_int(enum_value(window_type))),
+                  C.byref(C.c_int(int(slide_length))), C.byref(C.c_int(int(h_order))), C.byref(C.c_int(int(p_order))))
 
     def cal_data_length(self, data_length):
         """samples of each output of hpss() for data_length input samples"""
@@ -42,14 +37,12 @@ class HPSS(Base):
     def hpss_batch(self, data):
         """data [..., n] (numpy host | torch cuda) -> (h, p), each [..., cal_data_length(n)] of the same kind.  One
         hpssObj_hpssBatch call for all channels; each is bit-identical to a legacy call into zeroed buffers."""
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        batch, n = x2.shape
-        m = self.cal_data_length(n)
-        h, p = alloc(batch, m), alloc(batch, m)
-        if batch:
-            fn = self._require_ext("hpssObj_hpssBatch")
-            check(fn(self._obj, ptr(x2), n, batch, ptr(h), ptr(p), kind, stream), "hpssObj_hpssBatch")
-        return h.reshape(*lead, m), p.reshape(*lead, m)
+        b = Batch(data)
+        m = self.cal_data_length(b.n)
+        h, p = b.alloc(b.rows, m), b.alloc(b.rows, m)
+        if b.rows:
+            self._call("hpssObj_hpssBatch", b, b.x, b.n, b.rows, h, p)
+        return b.shaped(h), b.shaped(p)
 
     def hpss(self, data_arr):
         """data_arr [..., n] -> (h_arr, p_arr), float32 [..., cal_data_length(n)] each"""
@@ -59,8 +52,3 @@ class HPSS(Base):
         if data_arr.shape[-1] == 0:
             raise ValueError('Audio data must not be empty')
         return self.hpss_batch(data_arr)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.hpssObj_free(self._obj)
-            self._is_created = False

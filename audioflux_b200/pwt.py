@@ -2,11 +2,9 @@
 (reference binding: python/audioflux/pwt.py:20-257; C: src/pwt_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, BandAxis, SampleAxis, as_f32, np_ptr, split_batch
+from .base import Base, BandAxis, SampleAxis, as_f32, band_range, fit_length, is_log_scale, np_ptr, per_clip
 from .capi import opt_int, opt_float
 from .lib import check
 from .types import (SpectralFilterBankScaleType, SpectralFilterBankStyleType, SpectralFilterBankNormalType, enum_value)
@@ -20,33 +18,23 @@ class PWT(BandAxis, SampleAxis, Base):
         self.fft_length = 1 << radix2_exp
         if num > self.fft_length // 2 + 1:
             raise ValueError(f"num={num} is too large")
-        log_like = enum_value(scale_type) in (5, 6)
-        if low_fre is None:
-            low_fre = 32.703196 if log_like else 0.0
-        if high_fre is None:
-            high_fre = samplate / 2
-        if log_like and low_fre < 32.703:
+        low_fre, high_fre = band_range(low_fre, high_fre, scale_type, samplate)
+        if is_log_scale(scale_type) and low_fre < 32.703:
             raise ValueError(f"low_fre={low_fre} must be greater than or equal to 32.703")
         if low_fre < 0:
             raise ValueError(f"low_fre={low_fre} must be a non-negative number")
         self.num, self.radix2_exp, self.samplate = num, radix2_exp, samplate
         self.low_fre, self.high_fre, self.bin_per_octave = low_fre, high_fre, bin_per_octave
         self.scale_type, self.style_type, self.normal_type, self.is_padding = scale_type, style_type, normal_type, is_padding
-        status = self._lib.pwtObj_new(C.byref(self._obj), num, radix2_exp, opt_int(samplate), opt_float(low_fre),
-                                      opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(scale_type)),
-                                      opt_int(enum_value(style_type)), opt_int(enum_value(normal_type)),
-                                      opt_int(int(is_padding)))
-        if status != 0 or not self._obj:
-            raise ValueError(f"pwtObj_new failed with status {status}")
-        self._is_created = True
+        self._new("pwtObj_new", "pwtObj_free", num, radix2_exp, opt_int(samplate), opt_float(low_fre),
+                  opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(scale_type)),
+                  opt_int(enum_value(style_type)), opt_int(enum_value(normal_type)), opt_int(int(is_padding)))
 
     def get_fre_band_arr(self):
-        p = self._lib.pwtObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.num,)).copy()
+        return self._floats("pwtObj_getFreBandArr", self.num)
 
     def get_bin_band_arr(self):
-        p = self._lib.pwtObj_getBinBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int)), shape=(self.num,)).copy()
+        return self._ints("pwtObj_getBinBandArr", self.num)
 
     def enable_det(self, flag=True):
         self._lib.pwtObj_enableDet(self._obj, int(flag))
@@ -72,37 +60,15 @@ class PWT(BandAxis, SampleAxis, Base):
 
     def pwt(self, data_arr):
         """-> complex [..., num, N] as pwt.py:190-257 (no row flip, unlike CWT)."""
-        x = as_f32(data_arr)
-        N = self.fft_length
-        if x.shape[-1] > N:
-            x = x[..., :N]
-        elif x.shape[-1] < N:
-            x = np.concatenate([x, np.zeros((*x.shape[:-1], N - x.shape[-1]), np.float32)], axis=-1)
-        lead = x.shape[:-1]
-        x2 = np.ascontiguousarray(x).reshape(-1, N)
-        outs = []
-        for i in range(x2.shape[0]):
-            re, im = self.pwt_planes(x2[i])
-            outs.append(re + 1j * im)
-        return np.ascontiguousarray(np.stack(outs).reshape(*lead, self.num, N))
-
-    def _batch(self, name, data):
-        fn = self._require_ext(name)
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, N = x2.shape
-        if N != self.fft_length:
-            raise ValueError(f"data length must be 2**radix2_exp = {self.fft_length}")
-        re = alloc(B, self.num, N)
-        im = alloc(B, self.num, N)
-        check(fn(self._obj, ptr(x2), B, ptr(re), ptr(im), kind, stream), name)
-        return re.reshape(*lead, self.num, N), im.reshape(*lead, self.num, N)
+        re, im = per_clip(self.pwt_planes, fit_length(data_arr, self.fft_length, warn=False))
+        return re + 1j * im
 
     def pwt_batch(self, data):
         """Additive: data [B, N] (numpy host | torch cuda) -> (re, im) each [B, num, N]."""
-        return self._batch("pwtObj_pwtBatch", data)
+        return self._window_batch("pwtObj_pwtBatch", data)
 
     def pwt_det_batch(self, data):
-        return self._batch("pwtObj_pwtDetBatch", data)
+        return self._window_batch("pwtObj_pwtDetBatch", data)
 
     def get_filter_bank_arr(self):
         fn = self._require_ext("pwtObj_getFilterBankArr")
@@ -111,8 +77,3 @@ class PWT(BandAxis, SampleAxis, Base):
         out = np.zeros((self.num, width), np.float32)
         check(fn(self._obj, np_ptr(out)), "pwtObj_getFilterBankArr")
         return out
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.pwtObj_free(self._obj)
-            self._is_created = False

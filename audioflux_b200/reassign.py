@@ -1,11 +1,9 @@
 """Time-frequency reassignment (reference binding: python/audioflux/reassign.py:94-282; C: src/reassign_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, as_f32, np_ptr, split_batch, swap_last2
+from .base import Base, Batch, as_f32, np_ptr, per_clip, swap_last2
 from .capi import opt_int, opt_float
 from .types import ReassignType, WindowType, enum_value
 
@@ -19,12 +17,9 @@ class Reassign(Base):
         self.slide_length = self.fft_length // 4 if slide_length is None else slide_length
         self.re_type, self.thresh, self.is_padding = re_type, thresh, is_padding
         self.is_continue, self.order, self.result_type = False, 1, 0
-        status = self._lib.reassignObj_new(
-            C.byref(self._obj), radix2_exp, opt_int(samplate), opt_int(enum_value(window_type)), opt_int(self.slide_length),
-            opt_int(enum_value(re_type)), opt_float(thresh), opt_int(int(is_padding)), opt_int(0))
-        if status != 0 or not self._obj:
-            raise ValueError(f"reassignObj_new failed with status {status}")
-        self._is_created = True
+        self._new("reassignObj_new", "reassignObj_free", radix2_exp, opt_int(samplate), opt_int(enum_value(window_type)),
+                  opt_int(self.slide_length), opt_int(enum_value(re_type)), opt_float(thresh), opt_int(int(is_padding)),
+                  opt_int(0))
 
     def cal_time_length(self, data_length):
         return self._lib.reassignObj_calTimeLength(self._obj, int(data_length))
@@ -49,32 +44,19 @@ class Reassign(Base):
 
     def reassign(self, data_arr, result_type=0):
         """-> (reassigned, stft): [..., fre, time]; complex (result_type 0) or amplitude (1) as reassign.py:177-246."""
-        x = as_f32(data_arr)
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, x.shape[-1])
-        a, b = [], []
-        for row in x2:
-            re, im, sr, si = self.reassign_planes(row, result_type)
-            a.append(re + 1j * im if result_type == 0 else re)
-            b.append(sr + 1j * si)
-        m1 = np.stack(a).reshape(*lead, *a[0].shape)
-        m2 = np.stack(b).reshape(*lead, *b[0].shape)
-        return swap_last2(m1), swap_last2(m2)
+        re, im, sr, si = per_clip(lambda clip: self.reassign_planes(clip, result_type), as_f32(data_arr))
+        return swap_last2(re + 1j * im if result_type == 0 else re), swap_last2(sr + 1j * si)
 
     def reassign_batch(self, data, result_type=0):
         """Additive batched form (numpy host arrays or CUDA torch tensors): -> (re, im, stft_re, stft_im), each
         [..., T, fft_length/2+1], one call for the whole batch."""
-        fn = self._require_ext("reassignObj_reassignBatch")
         if result_type != self.result_type:
             self.set_result_type(result_type)
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        T, W = self.cal_time_length(x2.shape[-1]), self.fft_length // 2 + 1
-        outs = [alloc(x2.shape[0], T, W) for _ in range(4)]
-        for o in outs[:2]:
-            o.fill(0) if isinstance(o, np.ndarray) else o.zero_()
-        from . import lib as _libmod
-        _libmod.check(fn(self._obj, ptr(x2), x2.shape[-1], x2.shape[0], *[ptr(o) for o in outs], kind, stream), "reassignObj_reassignBatch")
-        return tuple(o.reshape(*lead, T, W) for o in outs)
+        b = Batch(data)
+        T, W = self.cal_time_length(b.n), self.fft_length // 2 + 1
+        outs = [b.alloc(b.rows, T, W, zero=k < 2) for k in range(4)]      # the reassigned planes are scattered into
+        self._call("reassignObj_reassignBatch", b, b.x, b.n, b.rows, *outs)
+        return tuple(map(b.shaped, outs))
 
     def y_coords(self):
         return np.linspace(0, self.samplate / 2, self.fft_length // 2 + 1 + 1)
@@ -84,8 +66,3 @@ class Reassign(Base):
             raise ValueError(f"radix2_exp={self.radix2_exp}(fft_length={self.fft_length}) is too large for data_length={data_length}")
         x_coords = np.linspace(0, data_length / self.samplate, self.cal_time_length(data_length) + 1)
         return x_coords
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.reassignObj_free(self._obj)
-            self._is_created = False

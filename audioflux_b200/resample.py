@@ -12,8 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, split_batch
-from .lib import check
+from .base import Base, Batch
 from .types import ResampleQualityType, WindowType, enum_value
 
 __all__ = ["Resample", "WindowResample"]
@@ -39,12 +38,6 @@ class ResampleBase(Base):
         self.source_rate = None
         self.target_rate = None
 
-    def _created(self, status, who):
-        if status != 0 or not self._obj:
-            msg = f": {self._lib.afb200_lastError().decode()}" if self._is_product and status != 0 else ""
-            raise ValueError(f"{who} failed with status {status}{msg}")
-        self._is_created = True
-
     def set_samplate(self, source_rate, target_rate):
         self._lib.resampleObj_setSamplate(self._obj, int(source_rate), int(target_rate))
         self.source_rate = source_rate
@@ -57,14 +50,12 @@ class ResampleBase(Base):
     def resample_batch(self, data):
         """data [..., n] (numpy host | torch cuda) -> [..., cal_data_length(n)] of the same kind.  One
         resampleObj_resampleBatch call for all channels; each is bit-identical to a legacy call into a zeroed buffer."""
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        batch, n = x2.shape
-        m = self.cal_data_length(n)
-        out = alloc(batch, m)
-        if batch and m > 0:
-            fn = self._require_ext("resampleObj_resampleBatch")
-            check(fn(self._obj, ptr(x2), n, batch, ptr(out), kind, stream), "resampleObj_resampleBatch")
-        return out.reshape(*lead, m)
+        b = Batch(data)
+        m = self.cal_data_length(b.n)
+        out = b.alloc(b.rows, m)
+        if b.rows and m > 0:
+            self._call("resampleObj_resampleBatch", b, b.x, b.n, b.rows, out)
+        return b.shaped(out)
 
     def resample(self, data_arr):
         """data_arr [..., n] -> float32 [..., cal_data_length(n)]"""
@@ -75,11 +66,6 @@ class ResampleBase(Base):
             raise ValueError('Audio data must not be empty')
         return self.resample_batch(data_arr)
 
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.resampleObj_free(self._obj)
-            self._is_created = False
-
 
 class Resample(ResampleBase):
     """Resampling with one of the three Kaiser-windowed presets (ResampleQualityType or 'best' / 'mid' / 'fast')."""
@@ -89,9 +75,8 @@ class Resample(ResampleBase):
         self.qual_type = _get_quality_type(qual_type)
         self.is_scale = is_scale
         self.is_continue = False
-        status = self._lib.resampleObj_new(C.byref(self._obj), C.byref(C.c_int(self.qual_type.value)),
-                                           C.byref(C.c_int(int(is_scale))), C.byref(C.c_int(0)))
-        self._created(status, "resampleObj_new")
+        self._new("resampleObj_new", "resampleObj_free", C.byref(C.c_int(self.qual_type.value)),
+                  C.byref(C.c_int(int(is_scale))), C.byref(C.c_int(0)))
 
 
 class WindowResample(ResampleBase):
@@ -103,8 +88,7 @@ class WindowResample(ResampleBase):
         self.zero_num, self.nbit, self.win_type = zero_num, nbit, win_type
         self.value, self.roll_off, self.is_scale = value, roll_off, is_scale
         self.is_continue = False
-        status = self._lib.resampleObj_newWithWindow(
-            C.byref(self._obj), C.byref(C.c_int(int(zero_num))), C.byref(C.c_int(int(nbit))),
-            C.byref(C.c_int(enum_value(win_type))), None if value is None else C.byref(C.c_float(value)),
-            C.byref(C.c_float(roll_off)), C.byref(C.c_int(int(is_scale))), C.byref(C.c_int(0)))
-        self._created(status, "resampleObj_newWithWindow")
+        self._new("resampleObj_newWithWindow", "resampleObj_free", C.byref(C.c_int(int(zero_num))),
+                  C.byref(C.c_int(int(nbit))), C.byref(C.c_int(enum_value(win_type))),
+                  None if value is None else C.byref(C.c_float(value)), C.byref(C.c_float(roll_off)),
+                  C.byref(C.c_int(int(is_scale))), C.byref(C.c_int(0)))

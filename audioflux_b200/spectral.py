@@ -10,8 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, as_f32, np_ptr, is_torch, MEM_HOST, MEM_DEVICE
-from .lib import check
+from .base import Base, Batch, as_f32, np_ptr
 from .types import SpectralNoveltyMethodType, SpectralNoveltyDataType, enum_value
 
 # feature ids of include/afb200_ext.h (AFB200_SPECTRAL_*)
@@ -76,10 +75,7 @@ class Spectral(Base):
             raise ValueError(f"fre_band_arr holds {self.fre_band_arr.shape[0]} values, num={num}")
         self.time_length = 0
         fre = None if self.fre_band_arr is None else np_ptr(self.fre_band_arr)
-        status = self._lib.spectralObj_new(C.byref(self._obj), num, fre)
-        if status != 0 or not self._obj:
-            raise ValueError(f"spectralObj_new failed with status {status}")
-        self._is_created = True
+        self._new("spectralObj_new", "spectralObj_free", num, fre)
 
     def set_time_length(self, time_length):
         self._lib.spectralObj_setTimeLength(self._obj, int(time_length))
@@ -111,7 +107,6 @@ class Spectral(Base):
         """m_tn [..., T, num] time-major (numpy host | torch cuda), features [(name, kwargs), ...] ->
         {name: [..., T]} ((value, fre) for max / mean / var) from one spectralObj_spectralBatch call.
         `phase` (same shape and kind as m_tn) is needed by pd / wpd / nwpd / cd / rcd."""
-        fn = self._require_ext("spectralObj_spectralBatch")
         feats = [(f, {}) if isinstance(f, str) else (f[0], dict(f[1] or {})) for f in features]
         names = [f[0] for f in feats]
         if not feats or len(feats) > MAX_REQ:
@@ -126,26 +121,12 @@ class Spectral(Base):
             raise ValueError(f"last axis holds {m_tn.shape[-1]} bins, the object has num={self.num}")
         if any(n in PHASE_FEATURES for n in names) and phase is None:
             raise ValueError("pd / wpd / nwpd / cd / rcd need the phase planes")
-        lead, T = tuple(m_tn.shape[:-2]), int(m_tn.shape[-2])
-        batch = int(np.prod(lead)) if lead else 1
-        if is_torch(m_tn):
-            import torch
-            if not m_tn.is_cuda:
-                raise ValueError("torch inputs must live on a CUDA device; pass numpy arrays for host data")
-            x = m_tn.contiguous().float()
-            ph = None if phase is None else phase.to(x.device).contiguous().float()
-            out = torch.zeros((planes, batch, T), dtype=torch.float32, device=x.device)
-            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-            ptr, kind = (lambda t: C.c_void_p(t.data_ptr())), MEM_DEVICE
-        else:
-            x = as_f32(m_tn)
-            ph = None if phase is None else as_f32(phase)
-            out = np.zeros((planes, batch, T), np.float32)
-            stream, ptr, kind = C.c_void_p(None), np_ptr, MEM_HOST
-        if ph is not None and tuple(ph.shape) != tuple(x.shape):
-            raise ValueError("phase must have the shape of the spectrogram")
-        check(fn(self._obj, ptr(x), None if ph is None else ptr(ph), T, batch, len(enc), np_ptr(req), np_ptr(par),
-                 ptr(out), kind, stream), "spectralObj_spectralBatch")
+        b = Batch(m_tn)
+        lead, T = b.lead[:-1], b.lead[-1]
+        batch = int(np.prod(lead))
+        ph = None if phase is None else b.second(phase, "phase")
+        out = b.alloc(planes, batch, T, zero=True)
+        self._call("spectralObj_spectralBatch", b, b.x, ph, T, batch, len(enc), req, par, out)
         res, k = {}, 0
         for n in names:
             if n in TWO_PLANES:
@@ -257,8 +238,3 @@ class Spectral(Base):
 
     def var(self, m_data_arr):
         return self._run("var", m_data_arr)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.spectralObj_free(self._obj)
-            self._is_created = False

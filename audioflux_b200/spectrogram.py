@@ -7,13 +7,10 @@ import ctypes as C
 
 import numpy as np
 
-from .base import Base, BandAxis, as_f32, np_ptr, split_batch, swap_last2
+from .base import Base, BandAxis, Batch, as_f32, band_range, is_log_scale, np_ptr, per_clip, swap_last2
 from .capi import opt_int, opt_float
-from .lib import check
 from .types import (WindowType, SpectralFilterBankScaleType, SpectralFilterBankStyleType,
                     SpectralFilterBankNormalType, SpectralDataType, CepstralRectifyType, enum_value)
-
-_LOG_LIKE = (5, 6)
 
 
 class Spectrogram(BandAxis, Base):
@@ -29,13 +26,10 @@ class Spectrogram(BandAxis, Base):
                 raise ValueError(f"bin_per_octave={bin_per_octave} must be 12, 24 or 36")
             if num % bin_per_octave != 0:
                 raise ValueError(f"num={num} must be an integer multiple of bin_per_octave={bin_per_octave}")
-        if low_fre is None:
-            low_fre = 32.703196 if scale in _LOG_LIKE else 0.0
-        if high_fre is None:
-            high_fre = samplate / 2
+        low_fre, high_fre = band_range(low_fre, high_fre, scale, samplate)
         if window_type is None:
             window_type = WindowType.HANN
-        if scale in _LOG_LIKE and low_fre < 32.703:
+        if is_log_scale(scale) and low_fre < 32.703:
             raise ValueError(f"low_fre={low_fre} must be greater than or equal to 32.703")
         if low_fre < 0:
             raise ValueError(f"low_fre={low_fre} must be a non-negative number")
@@ -46,14 +40,10 @@ class Spectrogram(BandAxis, Base):
         self.bin_per_octave, self.radix2_exp, self.window_type = bin_per_octave, radix2_exp, window_type
         self.slide_length, self.is_continue, self.data_type = slide_length, is_continue, data_type
         self.filter_bank_type, self.style_type, self.normal_type = filter_bank_type, style_type, normal_type
-        status = self._lib.spectrogramObj_new(
-            C.byref(self._obj), int(num), opt_int(samplate), opt_float(low_fre), opt_float(high_fre),
-            opt_int(bin_per_octave), opt_int(radix2_exp), opt_int(enum_value(window_type)), opt_int(slide_length),
-            opt_int(int(is_continue)), opt_int(enum_value(data_type)), opt_int(scale),
-            opt_int(enum_value(style_type)), opt_int(enum_value(normal_type)))
-        if status != 0 or not self._obj:
-            raise ValueError(f"spectrogramObj_new failed with status {status}")
-        self._is_created = True
+        self._new("spectrogramObj_new", "spectrogramObj_free", int(num), opt_int(samplate), opt_float(low_fre),
+                  opt_float(high_fre), opt_int(bin_per_octave), opt_int(radix2_exp), opt_int(enum_value(window_type)),
+                  opt_int(slide_length), opt_int(int(is_continue)), opt_int(enum_value(data_type)), opt_int(scale),
+                  opt_int(enum_value(style_type)), opt_int(enum_value(normal_type)))
         self.num = self.get_band_num()
 
     def set_data_norm_value(self, norm_value):
@@ -69,12 +59,10 @@ class Spectrogram(BandAxis, Base):
         return self._lib.spectrogramObj_getBinBandLength(self._obj)
 
     def get_fre_band_arr(self):
-        p = self._lib.spectrogramObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.get_bin_band_length(),)).copy()
+        return self._floats("spectrogramObj_getFreBandArr", self.get_bin_band_length())
 
     def get_bin_band_arr(self):
-        p = self._lib.spectrogramObj_getBinBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int)), shape=(self.get_bin_band_length(),)).copy()
+        return self._ints("spectrogramObj_getBinBandArr", self.get_bin_band_length())
 
     def spectrogram_planes(self, data_arr, is_phase_arr=False):
         """Raw C layout: one clip -> [T, num] (and phase [T, num], Linear bank only)."""
@@ -91,38 +79,26 @@ class Spectrogram(BandAxis, Base):
         if is_phase_arr and enum_value(self.filter_bank_type) != 0:
             raise ValueError("Only LINEAR bank type has phase arr")
         x = as_f32(data_arr)
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, x.shape[-1])
-        res = [self.spectrogram_planes(x2[i], is_phase_arr) for i in range(x2.shape[0])]
         if is_phase_arr:
-            spec = np.stack([r[0] for r in res]).reshape(*lead, -1, self.num)
-            phase = np.stack([r[1] for r in res]).reshape(*lead, -1, self.num)
-            return swap_last2(spec), swap_last2(phase)
-        return swap_last2(np.stack(res).reshape(*lead, -1, self.num))
+            return tuple(map(swap_last2, per_clip(lambda clip: self.spectrogram_planes(clip, True), x)))
+        spec, = per_clip(lambda clip: (self.spectrogram_planes(clip),), x)
+        return swap_last2(spec)
 
     def spectrogram_batch(self, data, is_phase_arr=False):
         """Additive: data [B, L] (numpy host | torch cuda) -> [B, T, num] (time-major; + phase for LINEAR)."""
-        fn = self._require_ext("spectrogramObj_spectrogramBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
-        spec = alloc(B, T, self.num)
-        phase = alloc(B, T, self.num) if is_phase_arr else None
-        check(fn(self._obj, ptr(x2), L, B, ptr(spec), ptr(phase) if is_phase_arr else None, kind, stream),
-              "spectrogramObj_spectrogramBatch")
-        spec = spec.reshape(*lead, T, self.num)
-        return (spec, phase.reshape(*lead, T, self.num)) if is_phase_arr else spec
+        b = Batch(data)
+        T = self.cal_time_length(b.n)
+        spec = b.alloc(b.rows, T, self.num)
+        phase = b.alloc(b.rows, T, self.num) if is_phase_arr else None
+        self._call("spectrogramObj_spectrogramBatch", b, b.x, b.n, b.rows, spec, phase)
+        return (b.shaped(spec), b.shaped(phase)) if is_phase_arr else b.shaped(spec)
 
     def mfcc_batch(self, data, cc_num=13, rectify_type=CepstralRectifyType.LOG):
         """Additive: the fused STFT -> bank -> log -> DCT kernel. data [B, L] -> [B, T, cc_num]."""
-        fn = self._require_ext("spectrogramObj_mfccBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
-        out = alloc(B, T, cc_num)
-        check(fn(self._obj, ptr(x2), L, B, cc_num, enum_value(rectify_type), ptr(out), kind, stream),
-              "spectrogramObj_mfccBatch")
-        return out.reshape(*lead, T, cc_num)
+        b = Batch(data)
+        out = b.alloc(b.rows, self.cal_time_length(b.n), cc_num)
+        self._call("spectrogramObj_mfccBatch", b, b.x, b.n, b.rows, cc_num, enum_value(rectify_type), out)
+        return b.shaped(out)
 
     def _cc(self, fn_name, m_data_arr, cc_num, rectify_type=None):
         """[num, T] of the LAST spectrogram call -> [cc_num, T]."""
@@ -176,18 +152,12 @@ class Spectrogram(BandAxis, Base):
 
     def deconv_batch(self, m_tn):
         """Additive: [..., T, num] (numpy host | torch cuda, time-major as spectrogram_batch returns it) -> (tone, pitch)."""
-        fn = self._require_ext("spectrogramObj_deconvBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        if x2.shape[-1] != self.num:
+        b = Batch(m_tn)
+        if b.n != self.num:
             raise ValueError(f"last dimension must be num={self.num}")
-        tone, pitch = alloc(*x2.shape), alloc(*x2.shape)
-        check(fn(self._obj, ptr(x2), x2.shape[0], ptr(tone), ptr(pitch), kind, stream), "spectrogramObj_deconvBatch")
-        return tone.reshape(*lead, self.num), pitch.reshape(*lead, self.num)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.spectrogramObj_free(self._obj)
-            self._is_created = False
+        tone, pitch = b.alloc(b.rows, b.n), b.alloc(b.rows, b.n)
+        self._call("spectrogramObj_deconvBatch", b, b.x, b.rows, tone, pitch)
+        return b.shaped(tone), b.shaped(pitch)
 
 
 def _scaled(scale, default_num):

@@ -15,12 +15,10 @@ Two differences from the reference's ``ST``, both on purpose:
 from __future__ import annotations
 
 import ctypes as C
-import warnings
 
 import numpy as np
 
-from .base import Base, SampleAxis, as_f32, split_batch
-from .lib import check
+from .base import Base, SampleAxis, fit_length
 
 
 def _range_checks(fft_length, min_index, max_index):
@@ -32,43 +30,10 @@ def _range_checks(fft_length, min_index, max_index):
         raise ValueError(f'min_index={min_index} must be less than max_index={max_index}')
 
 
-def _fit_length(data_arr, fft_length):
-    """data [..., n] as float32, zero-padded or truncated to fft_length with the reference's warnings
-    (python/audioflux/utils/util.py:98-110)"""
-    data_arr = np.asarray(data_arr, dtype=np.float32, order='C')
-    if data_arr.ndim == 0:
-        raise ValueError('Audio data must have at least one dimension')
-    n = data_arr.shape[-1]
-    if n < fft_length:
-        pad = fft_length - n
-        warnings.warn(f'The audio length={n} is not enough for fft_length={fft_length}(2**radix2_exp), '
-                      f'and {pad} zeros are automatically filled after the audio')
-        data_arr = np.pad(data_arr, (*[(0, 0)] * (data_arr.ndim - 1), (0, pad)))
-    elif n > fft_length:
-        warnings.warn(f'fft_length={fft_length}(2**radix2_exp) is too small for data_arr length={n}, '
-                      f'only the first fft_length={fft_length} data are valid')
-        data_arr = data_arr[..., :fft_length].copy()
-    return as_f32(data_arr)
-
-
 class _Stockwell(Base, SampleAxis):
-    def _new_failed(self, name, status):
-        raise ValueError(f"{name} failed with status {status}"
-                         + (f": {self._lib.afb200_lastError().decode()}" if self._is_product and status == -2 else ""))
-
     def y_coords(self):
         fre = self.get_fre_band_arr()
         return np.insert(fre, 0, fre[0])
-
-    def _run(self, name, data, *args):
-        fn = self._require_ext(name)
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        if x2.shape[-1] != self.fft_length:
-            raise ValueError(f"data length must be 2**radix2_exp = {self.fft_length}")
-        batch = x2.shape[0]
-        re, im = alloc(batch, self.num, self.fft_length), alloc(batch, self.num, self.fft_length)
-        check(fn(self._obj, ptr(x2), batch, *args, ptr(re), ptr(im), kind, stream), name)
-        return re.reshape(*lead, self.num, self.fft_length), im.reshape(*lead, self.num, self.fft_length)
 
 
 class ST(_Stockwell):
@@ -81,11 +46,8 @@ class ST(_Stockwell):
         self.radix2_exp, self.samplate = radix2_exp, samplate
         self.min_index, self.max_index = min_index, max_index
         self.factor, self.norm = factor, norm
-        status = self._lib.stObj_new(C.byref(self._obj), radix2_exp, min_index, max_index,
-                                     C.byref(C.c_float(factor)), C.byref(C.c_float(norm)))
-        if status != 0 or not self._obj:
-            self._new_failed("stObj_new", status)
-        self._is_created = True
+        self._new("stObj_new", "stObj_free", radix2_exp, min_index, max_index, C.byref(C.c_float(factor)),
+                  C.byref(C.c_float(norm)))
         self._bins = np.arange(min_index, max_index + 1, dtype=np.int32)
         self.num = len(self._bins)
 
@@ -110,18 +72,13 @@ class ST(_Stockwell):
     def st_batch(self, data):
         """data [..., 2**radix2_exp] (numpy host | torch cuda) -> (re, im) each [..., num, 2**radix2_exp].
         One stObj_stBatch call."""
-        return self._run("stObj_stBatch", data)
+        return self._window_batch("stObj_stBatch", data)
 
     def st(self, data_arr):
         """data_arr [..., 2**radix2_exp] (padded / truncated with a warning, as the reference) -> complex
         [..., num, 2**radix2_exp]"""
-        re, im = self.st_batch(_fit_length(data_arr, self.fft_length))
+        re, im = self.st_batch(fit_length(data_arr, self.fft_length, warn=True))
         return re + im * 1j
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.stObj_free(self._obj)
-            self._is_created = False
 
 
 class FST(_Stockwell):
@@ -134,10 +91,7 @@ class FST(_Stockwell):
         self.radix2_exp, self.samplate = radix2_exp, samplate
         self.min_index, self.max_index = min_index, max_index
         self.num = max_index - min_index + 1
-        status = self._lib.fstObj_new(C.byref(self._obj), radix2_exp)
-        if status != 0 or not self._obj:
-            self._new_failed("fstObj_new", status)
-        self._is_created = True
+        self._new("fstObj_new", "fstObj_free", radix2_exp)
 
     def get_fre_band_arr(self):
         return np.arange(self.min_index, self.max_index + 1, dtype=np.float32) * self.samplate / self.fft_length
@@ -145,15 +99,10 @@ class FST(_Stockwell):
     def fst_batch(self, data):
         """data [..., 2**radix2_exp] (numpy host | torch cuda) -> (re, im) each [..., num, 2**radix2_exp], rows
         min_index .. max_index.  One fstObj_fstBatch call."""
-        return self._run("fstObj_fstBatch", data, self.min_index, self.max_index)
+        return self._window_batch("fstObj_fstBatch", data, self.min_index, self.max_index)
 
     def fst(self, data_arr):
         """data_arr [..., 2**radix2_exp] (padded / truncated with a warning, as the reference) -> complex
         [..., num, 2**radix2_exp]"""
-        re, im = self.fst_batch(_fit_length(data_arr, self.fft_length))
+        re, im = self.fst_batch(fit_length(data_arr, self.fft_length, warn=True))
         return re + im * 1j
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.fstObj_free(self._obj)
-            self._is_created = False

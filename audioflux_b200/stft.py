@@ -1,13 +1,10 @@
 """STFT object (reference binding: python/audioflux/stft.py:14-300; C: src/stft_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, as_f32, np_ptr, split_batch
+from .base import Base, Batch, as_f32, np_ptr, per_clip
 from .capi import opt_int, opt_float
-from .lib import check
 from .types import WindowType, PaddingPositionType, PaddingModeType, enum_value
 
 
@@ -18,12 +15,9 @@ class STFT(Base):
         self.fft_length = 1 << radix2_exp
         self.window_type = window_type
         self.slide_length = slide_length
-        status = self._lib.stftObj_new(C.byref(self._obj), radix2_exp, opt_int(enum_value(window_type)),
-                                       opt_int(slide_length), opt_int(int(is_continue)))
         self.is_continue = is_continue
-        if status != 0 or not self._obj:
-            raise ValueError(f"stftObj_new failed with status {status}")
-        self._is_created = True
+        self._new("stftObj_new", "stftObj_free", radix2_exp, opt_int(enum_value(window_type)), opt_int(slide_length),
+                  opt_int(int(is_continue)))
 
     def set_slide_length(self, slide_length):
         self._lib.stftObj_setSlideLength(self._obj, slide_length)
@@ -49,14 +43,10 @@ class STFT(Base):
         self._lib.stftObj_useWindowDataArr(self._obj, np_ptr(w))
 
     def get_window_data_arr(self):
-        p = self._lib.stftObj_getWindowDataArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.fft_length,)).copy()
+        return self._floats("stftObj_getWindowDataArr", self.fft_length)
 
     def cal_time_length(self, data_length):
         return self._lib.stftObj_calTimeLength(self._obj, data_length)
-
-    def cal_data_length(self, time_length):
-        return self._lib.stftObj_calDataLength(self._obj, time_length)
 
     def stft_planes(self, data_arr):
         """Raw C layout: (re, im) each [T, fft_length] (full mirrored spectrum), one clip."""
@@ -69,27 +59,17 @@ class STFT(Base):
 
     def stft(self, data_arr):
         """-> complex [..., fft_length//2+1, T] like the reference wrapper (stft.py:259-300)."""
-        x = as_f32(data_arr)
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, x.shape[-1])
-        outs = []
-        for i in range(x2.shape[0]):
-            re, im = self.stft_planes(x2[i])
-            outs.append((re + 1j * im).T[: self.fft_length // 2 + 1])
-        out = np.stack(outs).reshape(*lead, self.fft_length // 2 + 1, -1)
-        return np.ascontiguousarray(out)
+        re, im = per_clip(self.stft_planes, as_f32(data_arr))
+        return np.ascontiguousarray(np.swapaxes(re + 1j * im, -1, -2)[..., : self.fft_length // 2 + 1, :])
 
     def stft_batch(self, data):
         """Additive batched entry point: data [B, L] (numpy host or torch cuda) ->
         (re, im) each [B, T, fft_length//2+1]."""
-        fn = self._require_ext("stftObj_stftBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(data)
-        B, L = x2.shape
-        T = self.cal_time_length(L)
-        re = alloc(B, T, self.fft_length // 2 + 1)
-        im = alloc(B, T, self.fft_length // 2 + 1)
-        check(fn(self._obj, ptr(x2), L, B, ptr(re), ptr(im), kind, stream), "stftObj_stftBatch")
-        return re.reshape(*lead, T, -1), im.reshape(*lead, T, -1)
+        b = Batch(data)
+        T = self.cal_time_length(b.n)
+        re, im = b.alloc(b.rows, T, self.fft_length // 2 + 1), b.alloc(b.rows, T, self.fft_length // 2 + 1)
+        self._call("stftObj_stftBatch", b, b.x, b.n, b.rows, re, im)
+        return b.shaped(re), b.shaped(im)
 
     def cal_data_length(self, time_length):
         return self._lib.stftObj_calDataLength(self._obj, int(time_length))
@@ -120,30 +100,17 @@ class STFT(Base):
             raise ValueError("m_data_arr's dimensions must be greater than 1")
         mirror = np.conj(z[..., ::-1, :][..., 1:-1, :])
         full = np.swapaxes(np.concatenate([z, mirror], axis=-2), -1, -2)          # [..., T, fft_length]
-        lead = full.shape[:-2]
-        f2 = full.reshape((-1,) + full.shape[-2:])
-        outs = [self.istft_planes(f2[i].real, f2[i].imag, method_type) for i in range(f2.shape[0])]
-        return np.stack(outs).reshape(*lead, -1)
+        out, = per_clip(lambda clip: (self.istft_planes(clip.real, clip.imag, method_type),), full, clip_ndim=2)
+        return out
 
     def istft_batch(self, re, im, method_type=0):
         """Additive: planes [B, T, W] with W = fft_length//2+1 (as stft_batch returns them) or fft_length
         (numpy host | torch cuda) -> data [B, (T-1)*slide + fft_length]."""
-        fn = self._require_ext("stftObj_istftBatch")
-        r2, lead, kind, ptr, stream, alloc = split_batch(re)
-        i2 = split_batch(im)[0]
-        if len(lead) < 1:
+        b = Batch(re)
+        im = b.second(im, "im")
+        if len(b.lead) < 1:
             raise ValueError("planes must be [..., T, W]")
-        T, W = lead[-1], r2.shape[-1]
-        B = r2.shape[0] // T
-        out = alloc(B, self.cal_data_length(T))
-        if kind == 0:
-            out[...] = 0
-        else:
-            out.zero_()
-        check(fn(self._obj, ptr(r2), ptr(i2), T, B, W, int(method_type), ptr(out), kind, stream), "stftObj_istftBatch")
-        return out.reshape(*lead[:-1], -1)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.stftObj_free(self._obj)
-            self._is_created = False
+        T = b.lead[-1]
+        out = b.alloc(b.rows // T, self.cal_data_length(T), zero=True)
+        self._call("stftObj_istftBatch", b, b.x, im, T, b.rows // T, b.n, int(method_type), out)
+        return out.reshape(*b.lead[:-1], -1)

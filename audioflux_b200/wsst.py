@@ -2,11 +2,9 @@
 C: src/wsst_algorithm.c, src/synsq_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, BandAxis, SampleAxis, as_f32, np_ptr
+from .base import Base, BandAxis, SampleAxis, as_f32, band_range, fit_length, np_ptr, per_clip
 from .capi import opt_int, opt_float
 from .types import WaveletContinueType, SpectralFilterBankScaleType, enum_value
 from .cwt import _DEFAULT_GAMMA_BETA
@@ -17,10 +15,7 @@ class WSST(BandAxis, SampleAxis, Base):
                  wavelet_type=WaveletContinueType.MORLET, scale_type=SpectralFilterBankScaleType.OCTAVE,
                  gamma=None, beta=None, thresh=0.001, is_padding=True, _lib=None):
         super().__init__(_lib)
-        if low_fre is None:
-            low_fre = 32.703196 if enum_value(scale_type) in (5, 6) else 0.0
-        if high_fre is None:
-            high_fre = samplate / 2
+        low_fre, high_fre = band_range(low_fre, high_fre, scale_type, samplate)
         g0, b0 = _DEFAULT_GAMMA_BETA[enum_value(wavelet_type)]
         gamma = g0 if gamma is None else gamma
         beta = b0 if beta is None else beta
@@ -28,21 +23,16 @@ class WSST(BandAxis, SampleAxis, Base):
         self.low_fre, self.high_fre, self.bin_per_octave = low_fre, high_fre, bin_per_octave
         self.wavelet_type, self.scale_type, self.gamma, self.beta = wavelet_type, scale_type, gamma, beta
         self.thresh, self.is_padding, self.order = thresh, is_padding, 1
-        status = self._lib.wsstObj_new(
-            C.byref(self._obj), num, radix2_exp, opt_int(samplate), opt_float(low_fre), opt_float(high_fre),
-            opt_int(bin_per_octave), opt_int(enum_value(wavelet_type)), opt_int(enum_value(scale_type)),
-            opt_float(gamma), opt_float(beta), opt_float(thresh), opt_int(int(is_padding)))
-        if status != 0 or not self._obj:
-            raise ValueError(f"wsstObj_new failed with status {status}")
-        self._is_created = True
+        self._new("wsstObj_new", "wsstObj_free", num, radix2_exp, opt_int(samplate), opt_float(low_fre),
+                  opt_float(high_fre), opt_int(bin_per_octave), opt_int(enum_value(wavelet_type)),
+                  opt_int(enum_value(scale_type)), opt_float(gamma), opt_float(beta), opt_float(thresh),
+                  opt_int(int(is_padding)))
 
     def get_fre_band_arr(self):
-        p = self._lib.wsstObj_getFreBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(self.num,)).copy()
+        return self._floats("wsstObj_getFreBandArr", self.num)
 
     def get_bin_band_arr(self):
-        p = self._lib.wsstObj_getBinBandArr(self._obj)
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int)), shape=(self.num,)).copy()
+        return self._ints("wsstObj_getBinBandArr", self.num)
 
     def set_order(self, order):
         self._lib.wsstObj_setOrder(self._obj, int(order))
@@ -59,25 +49,8 @@ class WSST(BandAxis, SampleAxis, Base):
 
     def wsst(self, data_arr):
         """-> (wsst, cwt) complex [..., num, N] as wsst.py:258-330."""
-        x = as_f32(data_arr)
-        N = self.fft_length
-        if x.shape[-1] > N:
-            x = x[..., :N]
-        elif x.shape[-1] < N:
-            x = np.concatenate([x, np.zeros((*x.shape[:-1], N - x.shape[-1]), np.float32)], axis=-1)
-        lead = x.shape[:-1]
-        x2 = np.ascontiguousarray(x).reshape(-1, N)
-        a, b = [], []
-        for i in range(x2.shape[0]):
-            re, im, cr, ci = self.wsst_planes(x2[i])
-            a.append(re + 1j * im)
-            b.append(cr + 1j * ci)
-        return (np.stack(a).reshape(*lead, self.num, N), np.stack(b).reshape(*lead, self.num, N))
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.wsstObj_free(self._obj)
-            self._is_created = False
+        re, im, cr, ci = per_clip(self.wsst_planes, fit_length(data_arr, self.fft_length, warn=False))
+        return re + 1j * im, cr + 1j * ci
 
 
 class Synsq(Base):
@@ -85,10 +58,7 @@ class Synsq(Base):
         super().__init__(_lib)
         self.num, self.radix2_exp, self.samplate, self.order, self.thresh = num, radix2_exp, samplate, order, thresh
         self.fft_length = 1 << radix2_exp
-        status = self._lib.synsqObj_new(C.byref(self._obj), num, radix2_exp, opt_int(samplate), opt_int(order), opt_float(thresh))
-        if status != 0 or not self._obj:
-            raise ValueError(f"synsqObj_new failed with status {status}")
-        self._is_created = True
+        self._new("synsqObj_new", "synsqObj_free", num, radix2_exp, opt_int(samplate), opt_int(order), opt_float(thresh))
 
     def synsq_planes(self, fre_arr, scale_type, re, im):
         """Raw C layout: planes [num, N] -> squeezed (re, im) [num, N]."""
@@ -104,15 +74,5 @@ class Synsq(Base):
             raise ValueError(f"m_data_arr with dtype={z.dtype} is not of complex type")
         if z.ndim < 2:
             raise ValueError(f"m_data_arr.ndim=[{z.ndim}] should be greater than 1")
-        lead = z.shape[:-2]
-        z2 = z.reshape(-1, *z.shape[-2:])
-        outs = []
-        for i in range(z2.shape[0]):
-            r, m = self.synsq_planes(fre_arr, filter_bank_type, z2[i].real, z2[i].imag)
-            outs.append(r + 1j * m)
-        return np.stack(outs).reshape(*lead, *z.shape[-2:])
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.synsqObj_free(self._obj)
-            self._is_created = False
+        re, im = per_clip(lambda clip: self.synsq_planes(fre_arr, filter_bank_type, clip.real, clip.imag), z, clip_ndim=2)
+        return re + 1j * im

@@ -2,13 +2,10 @@
 (reference binding: python/audioflux/feature/xxcc.py:14-136; C: src/feature/xxcc_algorithm.c)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from .base import Base, as_f32, np_ptr, split_batch, swap_last2, is_torch
+from .base import Base, Batch, as_f32, np_ptr, per_clip, swap_last2
 from .capi import opt_int
-from .lib import check
 from .types import CepstralRectifyType, CepstralEnergyType, enum_value
 
 
@@ -19,10 +16,7 @@ class XXCC(Base):
             raise ValueError("num must be >= 2")
         self.num = num
         self.time_length = 0
-        status = self._lib.xxccObj_new(C.byref(self._obj), num)
-        if status != 0 or not self._obj:
-            raise ValueError(f"xxccObj_new failed with status {status}")
-        self._is_created = True
+        self._new("xxccObj_new", "xxccObj_free", num)
 
     def set_time_length(self, time_length):
         self._lib.xxccObj_setTimeLength(self._obj, int(time_length))
@@ -45,21 +39,15 @@ class XXCC(Base):
         m = as_f32(m)
         if cc_num > self.num:
             raise ValueError("cc_num must be <= num")
-        lead = m.shape[:-2]
-        m2 = np.ascontiguousarray(np.swapaxes(m, -1, -2)).reshape(-1, m.shape[-1], m.shape[-2])
-        outs = [self.xxcc_planes(m2[i], cc_num, rectify_type) for i in range(m2.shape[0])]
-        out = np.stack(outs).reshape(*lead, m.shape[-1], cc_num)
+        out, = per_clip(lambda clip: (self.xxcc_planes(clip, cc_num, rectify_type),), swap_last2(m), clip_ndim=2)
         return swap_last2(out)
 
     def xxcc_batch(self, m_tn, cc_num=13, rectify_type=CepstralRectifyType.LOG):
         """Additive: m_tn [..., T, num] time-major (numpy host | torch cuda) -> [..., T, cc_num]."""
-        fn = self._require_ext("xxccObj_xxccBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        rows = x2.shape[0]
-        out = alloc(rows, cc_num)
-        check(fn(self._obj, ptr(x2), rows, cc_num, enum_value(rectify_type), ptr(out), kind, stream),
-              "xxccObj_xxccBatch")
-        return out.reshape(*lead, cc_num)
+        b = Batch(m_tn)
+        out = b.alloc(b.rows, cc_num)
+        self._call("xxccObj_xxccBatch", b, b.x, b.rows, cc_num, enum_value(rectify_type), out)
+        return b.shaped(out)
 
     def xxcc_standard_planes(self, m_tn, energy, cc_num=13, delta_window_length=9,
                              energy_type=CepstralEnergyType.REPLACE, rectify_type=CepstralRectifyType.LOG):
@@ -79,35 +67,17 @@ class XXCC(Base):
     def xxcc_standard(self, m_data_arr, energy_arr, cc_num=13, delta_window_length=9,
                       energy_type=CepstralEnergyType.REPLACE, rectify_type=CepstralRectifyType.LOG):
         """m_data_arr [..., num, T], energy_arr [..., T] -> three arrays [..., W, T] as feature/xxcc.py:138-240."""
-        m = as_f32(m_data_arr)
-        e = as_f32(energy_arr)
-        lead = m.shape[:-2]
-        m2 = np.ascontiguousarray(np.swapaxes(m, -1, -2)).reshape(-1, m.shape[-1], m.shape[-2])
-        e2 = e.reshape(-1, e.shape[-1])
-        res = [self.xxcc_standard_planes(m2[i], e2[i], cc_num, delta_window_length, energy_type, rectify_type)
-               for i in range(m2.shape[0])]
-        return tuple(swap_last2(np.stack([r[k] for r in res]).reshape(*lead, m.shape[-1], -1)) for k in range(3))
+        outs = per_clip(lambda m, e: self.xxcc_standard_planes(m, e, cc_num, delta_window_length, energy_type, rectify_type),
+                        swap_last2(as_f32(m_data_arr)), clip_ndim=2, y=as_f32(energy_arr))
+        return tuple(map(swap_last2, outs))
 
     def xxcc_standard_batch(self, m_tn, energy, cc_num=13, delta_window_length=9,
                             energy_type=CepstralEnergyType.REPLACE, rectify_type=CepstralRectifyType.LOG):
         """Additive: m_tn [..., T, num], energy [..., T] (numpy host | torch cuda) -> three [..., T, W]."""
-        fn = self._require_ext("xxccObj_xxccStandardBatch")
-        x2, lead, kind, ptr, stream, alloc = split_batch(m_tn)
-        rows = x2.shape[0]
-        if is_torch(m_tn):
-            e = energy.contiguous().float().reshape(-1)
-        else:
-            e = as_f32(energy).reshape(-1)
-        if e.shape[0] != rows:
-            raise ValueError("energy must hold one value per frame")
+        b = Batch(m_tn)
+        e = b.second(energy, "energy (one value per frame)", (b.rows,))
         w = cc_num + (1 if enum_value(energy_type) == 1 else 0)
-        outs = [alloc(rows, w) for _ in range(3)]
-        check(fn(self._obj, ptr(x2), ptr(e), rows, cc_num, int(delta_window_length), enum_value(energy_type),
-                 enum_value(rectify_type), ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), kind, stream),
-              "xxccObj_xxccStandardBatch")
-        return tuple(o.reshape(*lead, w) for o in outs)
-
-    def __del__(self):
-        if getattr(self, "_is_created", False):
-            self._lib.xxccObj_free(self._obj)
-            self._is_created = False
+        outs = [b.alloc(b.rows, w) for _ in range(3)]
+        self._call("xxccObj_xxccStandardBatch", b, b.x, e, b.rows, cc_num, int(delta_window_length),
+                   enum_value(energy_type), enum_value(rectify_type), *outs)
+        return tuple(map(b.shaped, outs))

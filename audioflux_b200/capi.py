@@ -294,6 +294,16 @@ HPSS_API = {
     "hpssObj_hpssBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp]),
 }
 
+# onset detection (include/mir/onset_algorithm.h, include/afb200_onset.h) and the additive batched entry point
+# (include/afb200_ext.h)
+ONSET_API = {
+    "onsetObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, C.c_int, c_int_p, c_int_p, c_int_p]),
+    "onsetObj_onset": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, vp, vp]),
+    "onsetObj_free": (None, [vp]),
+    "onsetObj_debug": (None, [vp]),
+    "onsetObj_onsetBatch": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -308,7 +318,7 @@ REFERENCE_BUILDERS = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, ONSET_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

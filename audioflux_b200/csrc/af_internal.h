@@ -351,8 +351,22 @@ typedef struct {
     float meanFre;                /* float mean of fre over the bins, summed in list order (spectral_algorithm.c:1124-1130) */
     int req[AFB200_SPECTRAL_MAX_REQ], plane[AFB200_SPECTRAL_MAX_REQ];
     float par[4 * AFB200_SPECTRAL_MAX_REQ];
+    int fresh;                    /* onset (0 for spectralObj_*): frame 1 of PD / WPD / NWPD is written as 0 and BROADBAND
+                                     stores its counts, instead of leaving / adding to what `out` holds */
 } AfSpectralArgs;
 int af_launch_spectral(const AfSpectralArgs *a, void *stream);
+
+/* onset detection (kernels/onset.cu).  Max filter over bins: out[r][k] = max of in[r][k - order/2 .. k - 1 + order -
+ * order/2] clipped to [0, num), rows = clips x T.  Peak picking: one CTA per clip normalises evn [clips][T] in place
+ * and writes points [clips][T] (0 after the clip's count) and counts [clips]; postMax, postAvg >= 1. */
+int af_launch_onset_maxfilter(const float *in, long long rows, int num, int order, float *out, void *stream);
+typedef struct {
+    float *evn;
+    int *points, *counts;
+    int clips, T, preMax, postMax, preAvg, postAvg, wait;
+    float delta;
+} AfOnsetPickArgs;
+int af_launch_onset_pick(const AfOnsetPickArgs *a, void *stream);
 
 /* NSGT band transforms (kernels/nsgt.cu).  Bands with L <= AF_NSGT_BLUESTEIN_MAX run as Bluestein FFTs of size
  * M = 2^ceil(log2(2L-1)) (k_nsgt_bluestein, one CTA per (group of bands, clip)); longer bands, up to AF_NSGT_MAX_LEN,

@@ -322,11 +322,14 @@ __global__ void __launch_bounds__(WARPS * 32) k_spectral(const __grid_constant__
                     if (diff > thr) s += 1.f;
                 }
                 s = wsum(s);
-                if (lane == 0) a.out[(size_t)pl * BT + o] += s;      // counts into the caller's array
+                if (lane == 0) {
+                    if (a.fresh) a.out[(size_t)pl * BT + o] = s;
+                    else a.out[(size_t)pl * BT + o] += s;          // counts into the caller's array
+                }
             } break;
             case AFB200_SPECTRAL_PD: case AFB200_SPECTRAL_WPD: case AFB200_SPECTRAL_NWPD: {
                 if (t == 0) { put(pl, 0.f); break; }
-                if (t == 1) break;                                    // the reference never writes frame 1
+                if (t == 1) { if (a.fresh) put(pl, 0.f); break; }     // the reference never writes frame 1
                 const float *ph = pclip + (size_t)t * num;
                 const int weight = f != AFB200_SPECTRAL_PD, norm = f == AFB200_SPECTRAL_NWPD;
                 float s = 0.f, sx = 0.f;

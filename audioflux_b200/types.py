@@ -129,5 +129,20 @@ class ResampleQualityType(Enum):
     FAST = 2
 
 
+class NoveltyType(Enum):
+    """novelty function of an onset (include/mir/onset_algorithm.h:13-30)"""
+    FLUX = 0
+    HFC = 1
+    SD = 2
+    SF = 3
+    MKL = 4
+    PD = 5
+    WPD = 6
+    NWPD = 7
+    CD = 8
+    RCD = 9
+    BROADBAND = 10
+
+
 def enum_value(v):
     return int(v.value) if isinstance(v, Enum) else int(v)

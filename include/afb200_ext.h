@@ -28,6 +28,7 @@
 #include "afb200_cepstrogram.h"
 #include "afb200_resample.h"
 #include "afb200_hpss.h"
+#include "afb200_onset.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -224,6 +225,16 @@ int resampleObj_resampleBatch(ResampleObj resampleObj, const float *data, int da
  * two inverse STFT launches per requested output. */
 int hpssObj_hpssBatch(HPSSObj hpssObj, const float *data, int dataLength, int batch, float *h, float *p, int memKind,
                       void *stream);
+
+/* onset detection of a batch: spec (and phase, NULL unless the object's type is PD / WPD / NWPD / CD / RCD)
+ * batch x nLength x mLength -> evn batch x nLength, points batch x nLength (each clip's points first, 0 after them)
+ * and counts batch (points per clip).  param and indexArr are host memory (param NULL: the defaults of onsetObj_onset).
+ * Each clip's results are bit-identical to onsetObj_onset on that clip, whatever the batch.  Refused wherever
+ * onsetObj_onset refuses.  Per group of clips (the filtered matrix is a workspace bounded by grouping): the max filter
+ * when filterOrder >= 2, one novelty launch and one peak-picking launch. */
+int onsetObj_onsetBatch(OnsetObj onsetObj, const float *spec, const float *phase, int batch, const NoveltyParam *param,
+                        const int *indexArr, int indexLength, float *evn, int *points, int *counts, int memKind,
+                        void *stream);
 
 #ifdef __cplusplus
 }

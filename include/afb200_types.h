@@ -55,6 +55,21 @@ typedef enum { WaveletContinue_Morse = 0, WaveletContinue_Morlet, WaveletContinu
 /* src/reassign_algorithm.h:14-22 */
 typedef enum { Reassign_All = 0, Reassign_Fre, Reassign_Time, Reassign_None } ReassignType;
 
+/* include/mir/onset_algorithm.h:13-44: the novelty function of an onset and its parameters ("isPostive" is the
+ * reference's spelling) */
+typedef enum { Novelty_Flux = 0, Novelty_HFC, Novelty_SD, Novelty_SF, Novelty_MKL, Novelty_PD, Novelty_WPD,
+               Novelty_NWPD, Novelty_CD, Novelty_RCD, Novelty_Broadband } NoveltyType;
+typedef struct {
+    int step;          /* >= 1 */
+    float p;           /* != 0 */
+    int isPostive;
+    int isExp;
+    int type;          /* 0 sum, 1 mean */
+    float threshold;   /* >= 0 */
+    int isNorm;        /* 0 | 1 */
+    float gamma;
+} NoveltyParam;
+
 #ifdef __cplusplus
 }
 #endif

@@ -304,6 +304,16 @@ ONSET_API = {
     "onsetObj_onsetBatch": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, C.c_int, vp]),
 }
 
+# harmonic ratio (include/mir/harmonicRatio_algorithm.h, include/afb200_harmonic_ratio.h) and the additive batched entry
+# point (include/afb200_ext.h)
+HARMONIC_RATIO_API = {
+    "harmonicRatioObj_new": (C.c_int, [P(vp), c_int_p, c_float_p, c_int_p, c_int_p, c_int_p]),
+    "harmonicRatioObj_calTimeLength": (C.c_int, [vp, C.c_int]),
+    "harmonicRatioObj_harmonicRatio": (None, [vp, vp, C.c_int, vp]),
+    "harmonicRatioObj_free": (None, [vp]),
+    "harmonicRatioObj_harmonicRatioBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -318,7 +328,7 @@ REFERENCE_BUILDERS = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -455,6 +455,19 @@ typedef struct {
 } AfHpssArgs;
 int af_launch_hpss_mask(const AfHpssArgs *a, void *stream);
 
+/* Harmonic ratio (kernels/harmonic_ratio.cu), W = 2^log2w (1 .. AFB200_HARMONIC_RATIO_MAX_EXP), two launches per call:
+ * every frame t of every clip b (samples b * dataLength + t * hop .. + W-1, times `window`) gets its crossing index in
+ * minIdx[b * T + t] (-1 for none) and, when it has one, its value in value[b * T + t]; then the frames without one take
+ * the index of the last earlier frame of their clip that has one (0 when none) and get their value.
+ * 1 <= maxLength <= W-1. */
+typedef struct {
+    const float *data, *window;   /* device: clips batch x dataLength, window W floats */
+    float *value;                 /* device, batch x timeLength */
+    int *minIdx;                  /* device workspace, batch x timeLength */
+    int log2w, maxLength, dataLength, hop, timeLength, batch;
+} AfHarmonicRatioArgs;
+int af_launch_harmonic_ratio(const AfHarmonicRatioArgs *a, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

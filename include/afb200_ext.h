@@ -29,6 +29,7 @@
 #include "afb200_resample.h"
 #include "afb200_hpss.h"
 #include "afb200_onset.h"
+#include "afb200_harmonic_ratio.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -235,6 +236,13 @@ int hpssObj_hpssBatch(HPSSObj hpssObj, const float *data, int dataLength, int ba
 int onsetObj_onsetBatch(OnsetObj onsetObj, const float *spec, const float *phase, int batch, const NoveltyParam *param,
                         const int *indexArr, int indexLength, float *evn, int *points, int *counts, int memKind,
                         void *stream);
+
+/* harmonic ratio of a batch: data batch x dataLength -> value batch x T, T = harmonicRatioObj_calTimeLength(dataLength).
+ * The minIndex carry of a frame without a crossing starts afresh at every clip.  Each clip's row is bit-identical to
+ * harmonicRatioObj_harmonicRatio on that clip, whatever the batch.  Two kernel launches per staging chunk: every frame,
+ * then the frames without a crossing of their own. */
+int harmonicRatioObj_harmonicRatioBatch(HarmonicRatioObj harmonicRatioObj, const float *data, int dataLength, int batch,
+                                        float *value, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

@@ -327,8 +327,25 @@ REFERENCE_BUILDERS = {
 }
 
 
+WAVELET_API = {
+    "dwtObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, c_int_p, c_int_p, c_int_p]),
+    "dwtObj_dwt": (None, [vp, vp, vp, vp]),
+    "dwtObj_free": (None, [vp]),
+    "wptObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, c_int_p, c_int_p, c_int_p]),
+    "wptObj_wpt": (None, [vp, vp, vp, vp]),
+    "wptObj_free": (None, [vp]),
+    "swtObj_new": (C.c_int, [P(vp), C.c_int, C.c_int, c_int_p, c_int_p, c_int_p]),
+    "swtObj_swt": (None, [vp, vp, vp, vp]),
+    "swtObj_free": (None, [vp]),
+    "dwtObj_dwtBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_int, vp]),
+    "wptObj_wptBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_int, vp]),
+    "swtObj_swtBatch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_int, vp]),
+}
+
+
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API,
+                              REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -468,6 +468,25 @@ typedef struct {
 } AfHarmonicRatioArgs;
 int af_launch_harmonic_ratio(const AfHarmonicRatioArgs *a, void *stream);
 
+/* Discrete wavelet transforms (kernels/wavelet.cu).  One split level of DWT / WPT: node k (0 .. nodes-1) of L samples
+ * at in + b*inStride + k*L, periodically indexed, gives a[i] = sum_j loD[j] x[(2i + dec - dec/2 - j) mod L] and d[i]
+ * likewise with hiD, i < L/2; a goes to lo + b*loStride + k*L + i and d to hi + b*hiStride + k*L + L/2 + i, the two
+ * halves exchanged when wpt and the node's tree index nodeBase + k is even and non-zero.  L is a power of two. */
+typedef struct {
+    const float *in, *loD, *hiD;  /* device; filters dec floats */
+    float *lo, *hi;
+    long long inStride, loStride, hiStride;
+    int L, nodes, nodeBase, wpt, dec, batch;
+} AfWaveletLevel;
+int af_launch_wavelet_level(const AfWaveletLevel *a, void *stream);
+/* out[b][r][j] = coef[b][base(r) + (j >> shift(r))], r < rows, j < N = 2^log2n: DWT (wpt = 0) base = 2^(r+1),
+ * shift = log2n - r - 1; WPT base = r * N / rows, shift = log2(rows) */
+int af_launch_wavelet_expand(const float *coef, int log2n, int rows, int wpt, int batch, float *out, void *stream);
+/* One SWT level: out[b][t] = sum_j f[j] x[(t + off - j*s) mod n] for loD -> lo and hiD -> hi, x = in + b*inStride,
+ * t < n, s = dilation, off = dec*s/2 */
+int af_launch_swt_level(const float *in, long long inStride, const float *loD, const float *hiD, int dec, int n, int s,
+                        int batch, float *lo, float *hi, long long outStride, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

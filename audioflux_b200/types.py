@@ -122,6 +122,16 @@ class WaveletContinueType(Enum):
     RICKER = 7
 
 
+class WaveletDiscreteType(Enum):
+    HAAR = 0
+    DB = 1
+    SYM = 2
+    COIF = 3
+    FK = 4
+    BIOR = 5
+    DMEY = 6
+
+
 class ResampleQualityType(Enum):
     """src/dsp/resample_algorithm.h"""
     BEST = 0

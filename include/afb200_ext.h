@@ -30,6 +30,9 @@
 #include "afb200_hpss.h"
 #include "afb200_onset.h"
 #include "afb200_harmonic_ratio.h"
+#include "afb200_dwt.h"
+#include "afb200_wpt.h"
+#include "afb200_swt.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -243,6 +246,14 @@ int onsetObj_onsetBatch(OnsetObj onsetObj, const float *spec, const float *phase
  * then the frames without a crossing of their own. */
 int harmonicRatioObj_harmonicRatioBatch(HarmonicRatioObj harmonicRatioObj, const float *data, int dataLength, int batch,
                                         float *value, int memKind, void *stream);
+
+/* discrete wavelet transforms of a batch of clips (data batch x N): coef batch x N and mData batch x rows x N (rows =
+ * num for DWT, 2^num for WPT; NULL: not written); SWT: mData1, mData2 batch x num x fftLength.  One kernel launch per
+ * level per staging chunk (and one for mData); each clip's rows are bit-identical to the legacy call on that clip. */
+int dwtObj_dwtBatch(DWTObj dwtObj, const float *data, int batch, float *coef, float *mData, int memKind, void *stream);
+int wptObj_wptBatch(WPTObj wptObj, const float *data, int batch, float *coef, float *mData, int memKind, void *stream);
+int swtObj_swtBatch(SWTObj swtObj, const float *data, int batch, float *mData1, float *mData2, int memKind,
+                    void *stream);
 
 #ifdef __cplusplus
 }

@@ -302,7 +302,7 @@ def band_edges(num, n_fft, sr, low, high, scale, ref, is_edge, slaney_bins):
     pts = _linspace_f32(lo, hi, num + det)
     fre = np.array([_scale_to_fre(p, scale, ref) for p in pts], dtype=f32)
     if not slaney_bins:
-        bins = np.round((f32(n_fft) * fre).astype(f32) / f32(sr)).astype(np.int64)
+        bins = _roundf((f32(n_fft) * fre).astype(f32) / f32(sr)).astype(np.int64)     # roundf: an edge at x.5 goes up
     else:
         grid = _linspace_f32(0, f32(f32(sr) - f32(f32(sr) / f32(n_fft))), n_fft)
         bins = np.zeros(num + det, dtype=np.int64)

@@ -106,9 +106,16 @@ def column_map(lens, fft_length, samplate):
 
 def transform(x, p, b=None):
     """-> (cells [list of complex128 arrays], matrix complex128 [num, max_len])"""
+    X = np.fft.fft(np.asarray(x, np.float64))                # the reference's full complex FFT of the real clip
+    return transform_spectrum(X, p, b)
+
+
+def transform_spectrum(X, p, b=None):
+    """the band step of the transform from the clip's full complex spectrum X [fft_length]
+    -> (cells [list of complex128 arrays], matrix complex128 [num, max_len])"""
     b = bank(p) if b is None else b
     n = p["fft_length"]
-    X = np.fft.fft(np.asarray(x, np.float64))                # the reference's full complex FFT of the real clip
+    X = np.asarray(X, np.complex128)
     cells = []
     for ln, off, w in zip(b["lens"], b["offs"], b["windows"]):
         j = np.arange(ln)
@@ -121,6 +128,59 @@ def transform(x, p, b=None):
         ok = cmap[i] >= 0
         m[i, ok] = c[cmap[i, ok]]
     return cells, m
+
+
+# ---- per-band comparison of the band kernels (kernels/nsgt.cu) ----
+BLUESTEIN_MAX = 4096        # longest band of k_nsgt_bluestein; longer bands run k_nsgt_direct
+DIRECT_PASS = 1024 * 6      # outputs k_nsgt_direct computes per pass (1024 threads x 6)
+BAND_TOL = 1e-4
+
+
+def log2_m(ln):
+    """log2 of k_nsgt_bluestein's convolution size M = 2^ceil(log2(2L - 1))"""
+    return int(2 * ln - 2).bit_length()
+
+
+def band_path(ln):
+    """the kernel path of a band of length ln, e.g. "bluestein M=2^13" or "direct 3 passes" """
+    if ln <= BLUESTEIN_MAX:
+        return f"bluestein M=2^{log2_m(ln)}"
+    passes = -(-int(ln) // DIRECT_PASS)
+    return f"direct {passes} pass{'es' if passes > 1 else ''}"
+
+
+def full_spectrum(re, im):
+    """half-spectrum planes [..., N/2 + 1] -> the full complex128 spectrum [..., N] the band kernels read: bins above N/2
+    are the conjugate mirror X[k] = conj(X[N - k])"""
+    h = np.asarray(re, np.float64) + 1j * np.asarray(im, np.float64)
+    return np.concatenate([h, np.conj(h[..., -2:0:-1])], axis=-1)
+
+
+def split_cells(cr, ci, lens):
+    """one clip's cell planes [total_len] -> [complex128 array per band]"""
+    c = np.asarray(cr, np.float64) + 1j * np.asarray(ci, np.float64)
+    return np.split(c, np.cumsum(lens)[:-1])
+
+
+def check_bands(got, want, lens, tol=BAND_TOL, what=""):
+    """Per band: max |got - want| <= tol * max |want| of that band; a band whose want is exactly zero must be exactly
+    zero in got.  got, want: [complex array per band].  -> {band_path: worst relative error}.  AssertionError naming
+    every failing band (index, L, log2 M, path)."""
+    worst, bad = {}, []
+    for i, (g, w, ln) in enumerate(zip(got, want, lens)):
+        assert g.shape == w.shape == (ln,), (what, i, g.shape, w.shape, ln)
+        path = band_path(ln)
+        peak = np.abs(w).max()
+        if peak == 0:
+            err = 0.0 if not np.any(g) else np.inf
+        else:
+            err = float(np.abs(g - w).max() / peak)
+        worst[path] = max(worst.get(path, 0.0), err)
+        if not err <= tol:
+            bad.append(f"band {i} L={ln} log2M={log2_m(ln) if ln <= BLUESTEIN_MAX else '-'} {path}: "
+                       + ("want exactly 0, got max |.| %.3e" % np.abs(g).max() if peak == 0 else f"{err:.3e}"))
+    assert not bad, f"{what}: {len(bad)} of {len(lens)} bands above {tol:g} of their own max\n" + "\n".join(bad[:30])
+    return worst
 
 
 # ---- the C API (libaudioflux_b200.so or the reference build) ----

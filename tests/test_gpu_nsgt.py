@@ -1,6 +1,7 @@
 """NSGT on the GPU: the reference's entry points against the oracle and the reference build, the batched entry point
 (host and device pointers, any batch size), the matrix as a gather of the cells, the launch count, the direct path of
-the widest bands, setMinLength, and the reference's own NSGT class running on libaudioflux_b200.so."""
+the widest bands (end to end, and band by band on the GPU's own spectrum), setMinLength, and the reference's own NSGT
+class running on libaudioflux_b200.so.  test_gpu_nsgt_bands.py checks every band kernel path band by band."""
 import numpy as np
 import pytest
 
@@ -88,12 +89,26 @@ def test_launch_count(product_lib, cuda_device):
             count_launches(product_lib, lambda: narrow.nsgt_batch(x19), warm=True) + 1)
 
 
+def _gpu_spectrum(x):
+    """the clips' forward FFT exactly as nsgtObj_nsgtBatch computes it (af_launch_stft: rect window, one frame, half
+    planes), mirrored to the full complex128 spectrum [clips, N]"""
+    r = x.shape[-1].bit_length() - 1
+    re, im = af.STFT(r, af.WindowType.RECT, 1 << r).stft_batch(x)
+    return NO.full_spectrum(re[:, 0], im[:, 0])
+
+
 def _oracle_check(t, x, kw):
+    """end to end against the float64 FFT of each clip per tensor, and every band against the oracle's band step on the
+    GPU's own spectrum per band"""
     _, p = NO.params(**kw)
-    re, im = t.nsgt_batch(x)
-    for b in range(len(x)):
-        _, m = NO.transform(x[b], p)
-        assert rel_max(re[b], m.real) <= TOL and rel_max(im[b], m.imag) <= TOL, (kw, b)
+    b = NO.bank(p)
+    re, im, cr, ci = t.nsgt_batch(x, with_cells=True)
+    X = _gpu_spectrum(x)
+    for c in range(len(x)):
+        _, m = NO.transform(x[c], p, b)
+        assert rel_max(re[c], m.real) <= TOL and rel_max(im[c], m.imag) <= TOL, (kw, c)
+        want, _ = NO.transform_spectrum(X[c], p, b)
+        NO.check_bands(NO.split_cells(cr[c], ci[c], b["lens"]), want, b["lens"], what=(kw, c))
 
 
 def test_direct_path_octave84_2e19(product_lib, cuda_device):

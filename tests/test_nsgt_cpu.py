@@ -77,6 +77,38 @@ def test_oracle_matches_reference(ref_out, name, kw):
         assert np.abs(m.real - w[0]).max() <= 1e-5 * scale and np.abs(m.imag - w[1]).max() <= 1e-5 * scale
 
 
+def test_transform_spectrum_is_the_band_step_of_transform():
+    """the band step alone, from the float64 FFT of the clip, is the whole transform bit for bit; the mirrored half
+    spectrum is the full one"""
+    for name, kw in NO.cases():
+        _, p = NO.params(**kw)
+        x = _signal(kw)
+        X = np.fft.fft(x.astype(np.float64))
+        cells, m = NO.transform(x, p)
+        cells2, m2 = NO.transform_spectrum(X, p)
+        assert all(np.array_equal(a, b) for a, b in zip(cells, cells2)) and np.array_equal(m, m2), name
+        h = np.fft.rfft(x.astype(np.float64))
+        assert np.abs(NO.full_spectrum(h.real, h.imag) - X).max() <= 1e-12 * np.abs(X).max(), name
+
+
+def test_check_bands_holds_each_band_to_its_own_scale():
+    rng = np.random.default_rng(0)
+    lens = [1, 3, 4097, 2]
+    want = [rng.standard_normal(n) + 1j * rng.standard_normal(n) for n in lens]
+    want[1] *= 1e-6                                           # a quiet band
+    want[3][:] = 0                                            # an all-zero band
+    worst = NO.check_bands([w.copy() for w in want], want, lens)
+    assert set(worst) == {"bluestein M=2^0", "bluestein M=2^3", "direct 1 pass", "bluestein M=2^2"}
+    got = [w.copy() for w in want]
+    got[1][0] += 2e-4 * np.abs(want[1]).max()                 # far below the tensor's scale, 2e-4 of the band's own
+    with pytest.raises(AssertionError, match="band 1 L=3 log2M=3"):
+        NO.check_bands(got, want, lens)
+    got = [w.copy() for w in want]
+    got[3][1] = 1e-30
+    with pytest.raises(AssertionError, match="band 3 L=2 log2M=2 bluestein M=2\\^2: want exactly 0"):
+        NO.check_bands(got, want, lens)
+
+
 @pytest.mark.parametrize("name,kw", NO.cases(), ids=[c[0] for c in NO.cases()])
 def test_column_map_on_reference_outputs(ref_lib, name, kw):
     """the reference's matrix is its cells gathered with the oracle's column map, bit for bit"""

@@ -343,8 +343,17 @@ WAVELET_API = {
 }
 
 
+# non-negative matrix factorisation (include/classic/nmf.h, include/afb200_nmf.h) and the additive batched entry point
+# (include/afb200_ext.h)
+NMF_API = {
+    "nmf": (None, [vp, C.c_int, C.c_int, C.c_int, vp, vp, c_int_p, c_int_p, c_float_p, c_int_p]),
+    "nmfBatch": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, c_int_p, c_int_p, c_float_p, c_int_p, vp,
+                           C.c_int, vp]),
+}
+
+
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API,
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API, NMF_API,
                               REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""

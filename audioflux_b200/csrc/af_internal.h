@@ -487,6 +487,20 @@ int af_launch_wavelet_expand(const float *coef, int log2n, int rows, int wpt, in
 int af_launch_swt_level(const float *in, long long inStride, const float *loD, const float *hiD, int dec, int n, int s,
                         int batch, float *lo, float *hi, long long outStride, void *stream);
 
+/* Non-negative matrix factorisation (kernels/nmf.cu), 1 + 4 maxIter launches whatever the batch: for each matrix b of
+ * V [batch][n][m], W [batch][n][k] and H [batch][k][m] (in place) the iterations of src/classic/nmf.c, each matrix
+ * stopping on its own.  type 0 KL, 1 IS, 2 Euclidean (the caller maps every other type to 2); norm 1 | 2 column p-norm,
+ * other column max.  iters (device, batch ints, or NULL) receives the iterations each matrix ran.  The workspace (one
+ * n x m plane per matrix, two for IS, and the previous W and H) is allocated and freed in stream order on `stream`. */
+typedef struct {
+    const float *V;
+    float *W, *H;
+    int *iters;
+    int n, m, k, batch, maxIter, type, norm;
+    float thresh;
+} AfNmfArgs;
+int af_launch_nmf(const AfNmfArgs *a, void *stream);
+
 void af_count_launch(int n);
 
 #ifdef __cplusplus

@@ -33,6 +33,7 @@
 #include "afb200_dwt.h"
 #include "afb200_wpt.h"
 #include "afb200_swt.h"
+#include "afb200_nmf.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -254,6 +255,17 @@ int dwtObj_dwtBatch(DWTObj dwtObj, const float *data, int batch, float *coef, fl
 int wptObj_wptBatch(WPTObj wptObj, const float *data, int batch, float *coef, float *mData, int memKind, void *stream);
 int swtObj_swtBatch(SWTObj swtObj, const float *data, int batch, float *mData1, float *mData2, int memKind,
                     void *stream);
+
+/* non-negative matrix factorisation of a batch (afb200_nmf.h): V batch x n x m; W batch x n x k and H batch x k x m in/out,
+ * initialised by the caller; iters (batch ints, NULL: not written) receives the iterations each matrix ran.  maxIter,
+ * type, thresh and norm apply to every matrix, NULL giving nmf's defaults.  Each matrix stops on its own and gives the
+ * same bits as nmf on it, whatever the batch.  Returns -1 when n, m, k or batch is below 1 or an array is NULL.
+ * 1 + 4 maxIter kernel launches per staging chunk (per call with device pointers), however many matrices it holds; the
+ * host never waits between iterations.  The call allocates a device workspace for the matrices it runs at once (with
+ * device pointers the whole batch) of (P n m + n k + k m + k + 1) floats each, P = 2 for IS and 1 otherwise: 4096
+ * IS matrices of 513 x 431 need about 7.3 GB.  When that allocation fails the call returns an error and writes nothing. */
+int nmfBatch(const float *V, int batch, int n, int m, int k, float *W, float *H, const int *maxIter, const int *type,
+             const float *thresh, const int *norm, int *iters, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

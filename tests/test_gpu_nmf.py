@@ -1,0 +1,209 @@
+"""NMF on the GPU: every oracle case through nmf / nmfBatch against the oracle and the reference build (W and H within
+1e-4 of their max, the iteration counts equal modulo an undetermined stop); the batch bit-identical to per-matrix nmf
+calls, matrices that stop at different iterations included, with host pointers across staging chunks and with device
+pointers; the launch count independent of the batch; the reference's own audioflux nmf on libaudioflux_b200.so; and the
+register / spill budget of the four kernels (compile only, no GPU needed)."""
+import ctypes as C
+import importlib
+import os
+import shutil
+import subprocess
+import tempfile
+
+import numpy as np
+import pytest
+
+import _nmf_oracle as NO
+from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
+from test_nmf_cpu import TOL, check_against
+from test_register_budgets import CSRC, _ptxas_entries, makefile_nvcc_line
+
+import audioflux_b200 as af
+
+CASES = dict(NO.cases())
+gpu = pytest.mark.gpu
+
+
+def _reference(name, kw):
+    ref = ref_lib_or_none()
+    if ref is not None:
+        W, H = NO.c_nmf(ref, kw)
+        return W, H, NO.c_iters(ref, kw, W, H, NO.oracle_case(kw)[2])
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "nmf.npz"))
+    return g[f"{name}/W"], g[f"{name}/H"], int(g[f"{name}/iters"])
+
+
+def _batch(lib, V, k, kw, device, W=None, H=None):
+    """nmfBatch on V [b][n][m] with the case's C arguments -> (W, H, iters) as numpy"""
+    b, n, m = V.shape
+    W = np.broadcast_to(np.arange(1, n * k + 1, dtype=np.float32).reshape(n, k), (b, n, k)).copy() if W is None else W
+    H = np.broadcast_to(np.arange(1, k * m + 1, dtype=np.float32).reshape(k, m), (b, k, m)).copy() if H is None else H
+    it = np.full(b, -7, np.int32)
+    args = (NO._opt(C.c_int, kw["max_iter"]), NO._opt(C.c_int, kw["tp"]), NO._opt(C.c_float, kw["thresh"]),
+            NO._opt(C.c_int, kw["norm"]))
+    if device:
+        import torch
+        t = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in (V, W, H, it)]
+        rc = lib.nmfBatch(dptr(t[0]), b, n, m, k, dptr(t[1]), dptr(t[2]), *args, dptr(t[3]), 1, stream())
+        torch.cuda.synchronize()
+        W, H, it = (x.cpu().numpy() for x in t[1:])
+    else:
+        V = np.ascontiguousarray(V)
+        rc = lib.nmfBatch(V.ctypes.data, b, n, m, k, W.ctypes.data, H.ctypes.data, *args, it.ctypes.data, 0, None)
+    assert rc == 0, lib.afb200_lastError()
+    return W, H, it
+
+
+@gpu
+@pytest.mark.parametrize("name", list(CASES))
+def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
+    kw = CASES[name]
+    W, H = NO.c_nmf(product_lib, kw)
+    assert product_lib.afb200_lastError() in (b"", None)
+    V = NO.case_matrix(kw)[None]
+    Wb, Hb, it = _batch(product_lib, V, kw["k"], kw, False)
+    assert np.array_equal(Wb[0], W) and np.array_equal(Hb[0], H)
+    iters = int(it[0])
+    check_against(kw, W, H, iters, (name, "oracle"))
+    Wr, Hr, ir = _reference(name, kw)
+    _, _, _, stat = NO.oracle_case(kw, stop=False)
+    assert NO.counts_agree(iters, ir, stat, NO.resolved(kw)["thresh"]), (name, iters, ir)
+    if iters == ir:
+        for got, want, nm in ((W, Wr, "W"), (H, Hr, "H")):
+            err = np.abs(got.astype(np.float64) - want).max() / max(float(np.abs(want).max()), 1e-30)
+            assert err <= TOL, (name, nm, err)
+
+
+@gpu
+@pytest.mark.parametrize("name", ["tp0_norm0", "tp1_norm2", "tp2_norm1", "tp3_is_euclidean", "lowrank_stop_kl", "k16",
+                                  "iter0"])
+def test_batch_equals_single_calls(product_lib, cuda_device, name):
+    """three matrices (the case, a louder reversed copy, a low-rank one that stops early): each bit-identical to nmf on
+    it, with host and device pointers"""
+    kw = CASES[name]
+    n, m, k = kw["n"], kw["m"], kw["k"]
+    V0 = NO.case_matrix(kw)
+    Vs = np.stack([V0, 1000 * V0[::-1, ::-1], NO.matrix(5, n, m, "lowrank")]).astype(np.float32)
+    single = []
+    for v in Vs:
+        kwv = dict(kw)
+        W, H, it = _batch(product_lib, v[None], k, kwv, False)
+        single.append((W[0], H[0], it[0]))
+    assert single[0][2] >= 0
+    for device in (False, True):
+        W, H, it = _batch(product_lib, Vs, k, kw, device)
+        for i, (w, h, c) in enumerate(single):
+            assert np.array_equal(W[i], w) and np.array_equal(H[i], h) and it[i] == c, (name, device, i)
+
+
+@gpu
+def test_staging_chunks_and_stops(product_lib, cuda_device):
+    """700 matrices of 257 x 200 (three 64 MB staging chunks) with a mix of noise and low-rank matrices that stop at
+    different iterations: the matrices at the chunk edges equal single calls, host and device"""
+    n, m, k = 257, 200, 3
+    kw = dict(max_iter=40, tp=0, thresh=2e-2, norm=0)
+    Vs = np.stack([NO.matrix(i, n, m, "lowrank" if i % 3 else "noise") for i in range(700)])
+    Wh, Hh, ih = _batch(product_lib, Vs, k, kw, False)
+    Wd, Hd, idv = _batch(product_lib, Vs, k, kw, True)
+    assert np.array_equal(Wh, Wd) and np.array_equal(Hh, Hd) and np.array_equal(ih, idv)
+    assert len(set(ih.tolist())) >= 2 and ih.min() < 40, sorted(set(ih.tolist()))
+    for i in (0, 1, 319, 320, 321, 639, 640, 699):
+        W, H, it = _batch(product_lib, Vs[i:i + 1], k, kw, False)
+        assert np.array_equal(W[0], Wh[i]) and np.array_equal(H[0], Hh[i]) and it[0] == ih[i], i
+
+
+@gpu
+def test_launches_do_not_depend_on_batch(product_lib, cuda_device):
+    import torch
+    n, m, k, mi = 64, 48, 4, 7
+    for b in (1, 5, 64):
+        V = torch.from_numpy(np.stack([NO.matrix(i, n, m) for i in range(b)])).cuda()
+        W = torch.ones(b, n, k, device="cuda")
+        H = torch.ones(b, k, m, device="cuda")
+        fn = lambda: product_lib.nmfBatch(dptr(V), b, n, m, k, dptr(W), dptr(H), C.byref(C.c_int(mi)), None,  # noqa: E731
+                                          None, None, None, 1, stream())
+        assert count_launches(product_lib, fn, warm=True) == 1 + 4 * mi, b
+
+
+@gpu
+def test_python_functions(product_lib, cuda_device):
+    """nmf returns (h, w) like the reference binding; nmf_batch with numpy and with CUDA tensors, init arrays and counts"""
+    import torch
+    kw = CASES["tp0_norm0"]
+    V = NO.case_matrix(kw)
+    h, w = af.nmf(V, 4, max_iter=50, tp=0)
+    W, H = NO.c_nmf(product_lib, kw)
+    assert np.array_equal(h, H) and np.array_equal(w, W) and h.dtype == np.float32
+    X = np.stack([V, 2 * V]).reshape(2, 1, *V.shape)
+    hb, wb, it = af.nmf_batch(X, 4, max_iter=50, return_iters=True)
+    assert hb.shape == (2, 1, 4, V.shape[1]) and wb.shape == (2, 1, V.shape[0], 4) and it.shape == (2, 1)
+    assert np.array_equal(hb[0, 0], h) and np.array_equal(wb[0, 0], w)
+    ht, wt, itt = af.nmf_batch(torch.from_numpy(X).cuda(), 4, max_iter=50, return_iters=True)
+    assert ht.is_cuda and np.array_equal(ht.cpu().numpy(), hb) and np.array_equal(wt.cpu().numpy(), wb)
+    assert np.array_equal(itt.cpu().numpy(), it)
+    w0 = np.random.default_rng(0).random((2, 1, V.shape[0], 4)).astype(np.float32)
+    h0 = np.random.default_rng(1).random((2, 1, 4, V.shape[1])).astype(np.float32)
+    w0c, h0c = w0.copy(), h0.copy()
+    hb2, wb2 = af.nmf_batch(X, 4, max_iter=20, w_init=w0, h_init=h0)
+    assert np.array_equal(w0, w0c) and np.array_equal(h0, h0c)
+    Wo, Ho, _, _ = NO.run(X[1, 0], 4, max_iter=20, tp=0, W=w0[1, 0], H=h0[1, 0])
+    assert np.abs(wb2[1, 0] - Wo).max() <= TOL * np.abs(Wo).max()
+    assert np.abs(hb2[1, 0] - Ho).max() <= TOL * np.abs(Ho).max()
+
+
+@gpu
+def test_reference_nmf_on_b200(raf, cuda_device):
+    """the reference's own nmf (classic/nmf.py, tp=0 by default) on the reference build and on libaudioflux_b200.so"""
+    nmf = importlib.import_module(raf.__name__ + ".classic").nmf
+    V = NO.matrix(3, 129, 60)
+    res = {}
+    for which in ("ref", "b200"):
+        raf.fftlib.set_fft_lib(lib_ext="b200" if which == "b200" else None)
+        res[which] = nmf(V, 3, max_iter=100)
+    raf.fftlib.set_fft_lib(None)
+    own = af.nmf(V, 3, max_iter=100)
+    for a, b, c in zip(res["b200"], own, res["ref"]):
+        assert np.array_equal(a, b)
+        assert np.abs(a - c).max() <= TOL * np.abs(c).max()
+
+
+@gpu
+def test_stop_counts_match_oracle(product_lib, cuda_device):
+    """the stop test sums the squares in float in the reference's order, so the iteration counts equal the oracle's on
+    every case; at most two may differ, and only by an undetermined decision (a last-bit difference of W or H from the
+    order of the double sums)"""
+    differ = []
+    for name, kw in CASES.items():
+        _, _, it = _batch(product_lib, NO.case_matrix(kw)[None], kw["k"], kw, False)
+        want = NO.oracle_case(kw)[2]
+        if int(it[0]) != want:
+            _, _, _, stat = NO.oracle_case(kw, stop=False)
+            assert NO.counts_agree(int(it[0]), want, stat, NO.resolved(kw)["thresh"]), (name, int(it[0]), want)
+            differ.append((name, int(it[0]), want))
+    print(f"nmf: cases whose count differs from the oracle's by an undetermined stop: {differ}")
+    assert len(differ) <= 2, differ
+
+
+def test_kernel_budget():
+    """the four NMF kernels spill nothing and fit at least two 256-thread CTAs per SM, compiled with the Makefile's own
+    nvcc line"""
+    cmd = makefile_nvcc_line("nmf.cu")
+    nvcc = shutil.which(cmd[0])
+    if nvcc is None:
+        pytest.skip(f"nvcc not found: {cmd[0]}")
+    cmd[0] = nvcc
+    assert "-fmad=false" in cmd
+    with tempfile.TemporaryDirectory() as tmp:
+        o = cmd.index("-o")
+        cmd[o + 1] = os.path.join(tmp, "nmf.cu.o")
+        r = subprocess.run(cmd + ["-Xptxas", "-v"], cwd=CSRC, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    seen = {}
+    for entry, figures in _ptxas_entries()(r.stderr).items():
+        for name in ("k_nmf_d", "k_nmf_h", "k_nmf_w", "k_nmf_norm"):
+            if name + "E" in entry:
+                seen[name] = figures
+    assert set(seen) == {"k_nmf_d", "k_nmf_h", "k_nmf_w", "k_nmf_norm"}, r.stderr
+    for name, (regs, stack, st, ld) in seen.items():
+        assert st == 0 and ld == 0 and stack == 0, (name, regs, stack, st, ld)
+        assert regs <= 96, (name, regs)                  # 256-thread CTAs: two per SM at least

@@ -1,5 +1,5 @@
 // cwt.cu -- continuous wavelet transform: big forward FFT of the clip, then per scale
-// (wavelet(s*omega) * spectrum) -> inverse FFT, for N = 2^12 .. 2^22 points.
+// (wavelet(s*omega) * spectrum) -> inverse FFT, for N = 2^1 .. 2^24 points.
 //
 // Replaces `__cwtObj_cwt` (src/cwt_algorithm.c:361-483): reflect pad (:404-414), fftObj_fft (:417-422),
 // the num x N filter-bank multiply (:426-437), num inverse FFTs fftObj_ifft (:440-459) and the crop
@@ -11,7 +11,7 @@
 //                    so global accesses are contiguous runs;
 //   rows kernel    : N1 contiguous length-N2 transforms, `rows` adjacent rows per CTA so the strided
 //                    result is written as contiguous runs.
-// For N <= 4096 the columns kernel alone is the whole transform (N2 = 1).
+// For N <= 4096 the columns kernel alone is the whole transform (N2 = 1); at N = 2 that is one radix-2 pass.
 // Shared-memory legs use the same Stockham radix-4/2 autosort passes as stft_generic.cu.
 #include <math.h>
 #include "common.cuh"
@@ -658,7 +658,7 @@ extern "C" size_t af_cwt_workspace_bytes(const AfCwtArgs *a) {
 }
 
 extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *workspace, float *outRe, float *outIm, void *stream) {
-    if (a->log2n < 2 || a->log2n > 24) return af_fail(AF_ERR_UNSUPPORTED, "CWT length 2^%d is outside [2^2, 2^24]", a->log2n);
+    if (a->log2n < 1 || a->log2n > 24) return af_fail(AF_ERR_UNSUPPORTED, "CWT length 2^%d is outside [2^1, 2^24]", a->log2n);
     CwtParams p;
     fill_params(a, &p);
     p.data = data; p.outRe = outRe; p.outIm = outIm;

@@ -17,7 +17,10 @@ int cwtObj_new(CWTObj *cwtObj, int num, int radix2Exp, int *samplate, float *low
                float *gamma, float *beta, int *isPad);
 float *cwtObj_getFreBandArr(CWTObj cwtObj);                       /* :336-339 */
 int *cwtObj_getBinBandArr(CWTObj cwtObj);                         /* :341-344 */
-/* :346-350.  dataArr: exactly 2^radix2Exp samples; outputs num x 2^radix2Exp, row 0 = highest band. */
+/* :346-350.  dataArr: exactly 2^radix2Exp samples; outputs num x 2^radix2Exp, row 0 = highest band.
+ * The transform runs for radix2Exp 1 .. 24 (isPad doubles the FFT length, and is only accepted up to radix2Exp 16).
+ * An object built with radix2Exp 25 .. 30 constructs, but every transform call on it (this one, cwtObj_cwtDet and the
+ * batched entry points) fails -- non-zero status, message in afb200_lastError() -- and leaves the outputs untouched. */
 void cwtObj_cwt(CWTObj cwtObj, float *dataArr, float *mRealArr4, float *mImageArr4);
 /* :485-528 / :352-358.  Derivative transform W' = IFFT(j * omega * wavelet * X) for synchrosqueezing.  enableDet(1)
  * must be called once; dataArr may be NULL to reuse the spectrum of the preceding single-clip cwtObj_cwt / cwtDet. */

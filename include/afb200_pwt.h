@@ -17,7 +17,10 @@ int pwtObj_new(PWTObj *pwtObj, int num, int radix2Exp, int *samplate, float *low
                SpectralFilterBankNormalType *normalType, int *isPadding);
 float *pwtObj_getFreBandArr(PWTObj pwtObj);                       /* :323-326, borrowed */
 int *pwtObj_getBinBandArr(PWTObj pwtObj);                         /* :328-331, borrowed */
-/* :333-336.  dataArr: exactly 2^radix2Exp samples; outputs num x 2^radix2Exp. */
+/* :333-336.  dataArr: exactly 2^radix2Exp samples; outputs num x 2^radix2Exp.  The transform runs for radix2Exp
+ * 1 .. 24 (isPadding doubles the FFT length, and is only accepted up to radix2Exp 16); an object built with radix2Exp
+ * 25 .. 30 constructs, but every transform call on it fails (non-zero status, message in afb200_lastError()) and leaves the
+ * outputs untouched. */
 void pwtObj_pwt(PWTObj pwtObj, float *dataArr, float *mRealArr3, float *mImageArr3);
 void pwtObj_enableDet(PWTObj pwtObj, int flag);                   /* :350-390 */
 /* :338-344.  Derivative transform (bank x j omega); dataArr may be NULL to reuse the preceding call's spectrum. */

@@ -95,8 +95,12 @@ def cwt_oracle(w, x, det=False, bank=None):
 
 
 def cwt_bank(w):
+    """The oracle bank at the transform length: N + 2 * pad columns (pad = N / 2 when the object pads), band frequencies
+    of the unpadded length."""
+    pad = w.fft_length // 2 if w.is_padding else 0
     return O.cwt_filterbank(w.num, w.fft_length, w.samplate, af.enum_value(w.wavelet_type), af.enum_value(w.scale_type),
-                            low=w.low_fre, high=w.high_fre, bpo=w.bin_per_octave, gamma=w.gamma, beta=w.beta)[0]
+                            low=w.low_fre, high=w.high_fre, bpo=w.bin_per_octave, gamma=w.gamma, beta=w.beta,
+                            pad_length=pad)[0]
 
 
 def pwt_oracle(p, x, det=False):

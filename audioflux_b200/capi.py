@@ -352,8 +352,22 @@ NMF_API = {
 }
 
 
+# cross-correlation and the chirp z-transform (include/dsp/xcorr_algorithm.h, czt_algorithm.h; include/afb200_xcorr.h,
+# afb200_czt.h) and the additive batched entry points (include/afb200_ext.h)
+DSP_API = {
+    "xcorrObj_new": (C.c_int, [P(vp)]),
+    "xcorrObj_xcorr": (C.c_int, [vp, vp, vp, C.c_int, c_int_p, vp, c_float_p]),
+    "xcorrObj_free": (None, [vp]),
+    "xcorrObj_xcorrBatch": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, c_int_p, vp, vp, vp, C.c_int, vp]),
+    "cztObj_new": (C.c_int, [P(vp), C.c_int]),
+    "cztObj_czt": (None, [vp, vp, vp, C.c_float, C.c_float, vp, vp]),
+    "cztObj_free": (None, [vp]),
+    "cztObj_cztBatch": (C.c_int, [vp, vp, vp, C.c_int, C.c_float, C.c_float, vp, vp, C.c_int, vp]),
+}
+
+
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API, NMF_API,
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API, NMF_API, DSP_API,
                               REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""

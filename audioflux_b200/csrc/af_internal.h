@@ -71,6 +71,10 @@ void af_pipe_free(AfPipe *pipe);
  * launch on `stream` (created on first use); af_fence_wait blocks until it has passed (no-op when NULL) */
 int af_fence_record(void **ev, void *stream);
 int af_fence_wait(void *ev);
+/* device-side ordering: later work on `stream` waits for the launch *ev last recorded (no-op when NULL).  An object
+ * whose device state is written and read from several streams brackets each use with af_fence_order(fence, st) and
+ * af_fence_record(&fence, st): the fence then chains every use, whatever stream it ran on. */
+int af_fence_order(void *ev, void *stream);
 void af_fence_free(void *ev);
 /* clips per group of a device workspace of perClip bytes per clip: a quarter of the free memory, at most cap bytes,
  * at least one clip and at most `batch` */
@@ -500,6 +504,37 @@ typedef struct {
     float thresh;
 } AfNmfArgs;
 int af_launch_nmf(const AfNmfArgs *a, void *stream);
+
+/* Cross-correlation (kernels/xcorr.cu) of `batch` pairs of rows a, b [batch][n] (b NULL: the autocorrelation of each row
+ * of a), M = the smallest power of two >= 2n: out [batch][2n-1] = IFFT_M(FFT_M(a) conj(FFT_M(b))) at lags -(n-1) .. n-1,
+ * divided by sqrtf(float(sum a^2) float(sum b^2)) when coeff; maxValue / maxIndex (batch each, either NULL) receive the
+ * row's __vmax.  M <= AF_XCORR_SHORT_MAX: one launch (k_xcorr, one CTA per pair).  Longer: the four-step forward legs of
+ * the CWT path in groups of pairs over the object's workspace `work` (grown as needed, at most about 512 MB a group),
+ * every use of it bracketed by the object's fence (af_fence_order / af_fence_record). */
+#define AF_XCORR_SHORT_MAX (1 << 14)
+typedef struct {
+    const float *a, *b;
+    float *out, *maxValue;
+    int *maxIndex;
+    int n, batch, coeff;
+    AfDevBuf *work;
+    void **fence;
+} AfXcorrArgs;
+int af_launch_xcorr(const AfXcorrArgs *a, void *stream);
+
+/* Chirp z-transform (kernels/czt.cu), N = 2^log2n, M = 2N <= 2^(AFB200_CZT_MAX_EXP + 1), one launch (k_czt, one CTA per
+ * row): g = x * pre over the N inputs (re / im either NULL), zero-padded to M; y = IFFT_M(FFT_M(g) H);
+ * re3 / im3 [batch][M]: y[N-1+k] post[k] for k < N, then y[N .. M-1].  `tables`: pre (N complex), post (N complex) and H
+ * (M complex, bit-reversed order), interleaved float pairs.  af_launch_czt_filter turns the chirp filter h, uploaded in
+ * the H slot in natural order, into H in place (one launch). */
+typedef struct {
+    const float *re, *im;
+    float *re3, *im3;
+    const float *tables;
+    int log2n, batch;
+} AfCztArgs;
+int af_launch_czt(const AfCztArgs *a, void *stream);
+int af_launch_czt_filter(float *H, int log2m, void *stream);
 
 void af_count_launch(int n);
 

@@ -224,6 +224,7 @@ int af_fence_record(void **ev, void *stream) {
     if (!*ev && (rc = af_event_create(ev))) return rc;
     return af_event_record(*ev, stream);
 }
+int af_fence_order(void *ev, void *stream) { return ev ? af_stream_wait_event(stream, ev) : AF_OK; }
 int af_fence_wait(void *ev) { return ev ? af_cuda_check(cudaEventSynchronize((cudaEvent_t)ev), "cudaEventSynchronize") : AF_OK; }
 void af_fence_free(void *ev) { af_event_destroy(ev); }
 

@@ -76,6 +76,24 @@ __device__ __forceinline__ void af_fft_inplace_dif(float2 *a, int nc, const floa
     }
 }
 
+// the companion of af_fft_inplace_dif: the same forward transform over one buffer by in-place radix-2
+// decimation-in-time passes, from bit-reversed input (a[__brev(j) >> (32 - log2nc)] holds element j) to natural-order
+// output.  After af_fft_inplace_dif, pointwise work in bit-reversed order and conj -> this -> conj / nc invert without
+// a permutation.  All threads of the block must call it.
+__device__ __forceinline__ void af_fft_inplace_dit(float2 *a, int nc, int log2nc, const float2 *tw = nullptr) {
+    for (int half = 1, shift = log2nc - 1; half < nc; half <<= 1, shift--) {
+        for (int i = threadIdx.x; i < (nc >> 1); i += blockDim.x) {
+            const int k = i & (half - 1), base = ((i - k) << 1) + k;
+            const float2 u = a[base];
+            float2 v = a[base + half];
+            if (k) v = af_cmul(v, af_tw(tw, k, shift, 2 * half));              // exp(-2 pi i k / (2 half)) = tw[k << shift]
+            a[base] = make_float2(u.x + v.x, u.y + v.y);
+            a[base + half] = make_float2(u.x - v.x, u.y - v.y);
+        }
+        __syncthreads();
+    }
+}
+
 // host side: cached device tables per (device, log2 n): [0, n) exp(-2 pi i j / n) and, behind it, [0, n] exp(-2 pi i j / (2n))
 // (the real-FFT post-pass twiddles of a 2n-point real transform packed into n complex points)
 const float2 *af_twiddle_table(int log2n);

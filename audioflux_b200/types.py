@@ -139,6 +139,12 @@ class ResampleQualityType(Enum):
     FAST = 2
 
 
+class XcorrNormalType(Enum):
+    """normalisation of a cross-correlation (include/dsp/xcorr_algorithm.h:14-18)"""
+    NONE = 0
+    COEFF = 1
+
+
 class NoveltyType(Enum):
     """novelty function of an onset (include/mir/onset_algorithm.h:13-30)"""
     FLUX = 0

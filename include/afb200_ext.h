@@ -34,6 +34,8 @@
 #include "afb200_wpt.h"
 #include "afb200_swt.h"
 #include "afb200_nmf.h"
+#include "afb200_xcorr.h"
+#include "afb200_czt.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -266,6 +268,22 @@ int swtObj_swtBatch(SWTObj swtObj, const float *data, int batch, float *mData1, 
  * IS matrices of 513 x 431 need about 7.3 GB.  When that allocation fails the call returns an error and writes nothing. */
 int nmfBatch(const float *V, int batch, int n, int m, int k, float *W, float *H, const int *maxIter, const int *type,
              const float *thresh, const int *norm, int *iters, int memKind, void *stream);
+
+/* cross-correlation of a batch of pairs (afb200_xcorr.h): a, b batch x length (b NULL: the autocorrelation of each row of
+ * a) -> out batch x (2 length - 1); maxValue and maxIndex (batch each, either may be NULL) receive each row's maximum and
+ * its first index.  normType NULL means XcorrNormal_Coeff, as in xcorrObj_xcorr.  Each row is bit-identical to
+ * xcorrObj_xcorr on that pair, whatever the batch.  Returns -1 for length < 1 or batch < 0 and -2 for length above
+ * AFB200_XCORR_MAX_LENGTH.  Up to 8192 samples (transforms of up to 2^14 points) one kernel launch per staging chunk;
+ * longer rows run the four-step transforms of the CWT path in bounded groups of pairs. */
+int xcorrObj_xcorrBatch(XcorrObj xcorrObj, const float *a, const float *b, int length, int batch,
+                        XcorrNormalType *normType, float *out, float *maxValue, int *maxIndex, int memKind, void *stream);
+
+/* chirp z-transform of a batch of rows (afb200_czt.h): re, im batch x N (either may be NULL, not both) -> re3, im3
+ * batch x 2N, each row bit-identical to cztObj_czt on it.  The band rule of cztObj_czt applies once per call.  One kernel
+ * launch per staging chunk, plus one per change of the object's tables; a table change waits for the object's earlier
+ * launches. */
+int cztObj_cztBatch(CZTObj cztObj, const float *re, const float *im, int batch, float lowW, float highW,
+                    float *re3, float *im3, int memKind, void *stream);
 
 #ifdef __cplusplus
 }

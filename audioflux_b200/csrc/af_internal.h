@@ -291,11 +291,17 @@ typedef struct {
     int bankWidth;
     int *support;            /* device, 3 x num ints: per bank row the bins [lo, hi) above 2^-28 of its peak (+ scratch); NULL = no pruning */
     int *supportReady;       /* host flag of the owning object: 0 until the launcher has filled `support` */
-    int forwardOnly;         /* 1: only the forward transform of the `batch` real sequences -> workspace[batch][N] float2 (long-frame STFT) */
 } AfCwtArgs;
 size_t af_cwt_workspace_bytes(const AfCwtArgs *a);
 /* data == NULL: skip the forward transform and reuse the spectra a previous call left in `workspace` */
 int af_launch_cwt(const AfCwtArgs *a, const float *data, void *workspace, float *outRe, float *outIm, void *stream);
+/* forward FFT of `rows` real sequences x [rows][2^log2n], 2^15 <= 2^log2n <= 2^20, by the CWT's four-step forward legs
+ * (kernels/cwt.cu): the spectra [rows][2^log2n] float2 at the start of `workspace`, which has
+ * af_fft_rows_workspace_bytes(log2n, rows) bytes */
+size_t af_fft_rows_workspace_bytes(int log2n, int rows);
+int af_launch_fft_rows(const float *x, int log2n, int rows, void *workspace, void *stream);
+/* rows per chunk of a long-row pass whose workspace (its real rows and af_fft_rows_workspace_bytes) stays within 512 MB */
+long long af_fft_rows_chunk(int log2n, long long rows);
 int af_launch_cwt_bank_table(const AfCwtArgs *a, float *bank /* device num x n */, void *stream);
 
 /* ---------------- BFT core shared with the SpectrogramObj front door (host/af_bft.c) ---------------- */

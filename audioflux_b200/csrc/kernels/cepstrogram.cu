@@ -31,25 +31,7 @@ struct CepsParams {
     int dataLength, hop, timeLength, specWidth;
 };
 
-// bin k (0 .. N/2) of the N-point real FFT whose N/2-point packed transform is z: X[k] = E[k] + W_N^k O[k]
-__device__ __forceinline__ float2 real_bin(const CepsParams &p, const float2 *z, int k) {
-    const int nc = p.nc;
-    const float2 zk = z[k == nc ? 0 : k], zp = z[k == 0 ? 0 : nc - k];
-    const float er = 0.5f * (zk.x + zp.x), ei = 0.5f * (zk.y - zp.y);
-    const float orr = 0.5f * (zk.y + zp.y), oi = -0.5f * (zk.x - zp.x);
-    const float2 w = p.tw ? __ldg(p.tw + nc + k) : af_twiddle(k, p.n);     // exp(-2 pi i k / N)
-    float xr = er + (w.x * orr - w.y * oi), xi = ei + (w.x * oi + w.y * orr);
-    if (k == 0 || k == nc) xi = 0.0f;
-    return make_float2(xr, xi);
-}
-
 __device__ __forceinline__ float log_power(float re, float im) { return logf(fmaxf(re * re + im * im, 1e-16f)); }
-
-// value v at position k (0 .. N/2) of a real even N-sequence, in the float view f of a packed buffer
-__device__ __forceinline__ void put_even(float *f, int n, int k, float v) {
-    f[k] = v;
-    if (k > 0 && k < n / 2) f[n - k] = v;
-}
 
 template <bool kPlanes>
 __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
@@ -69,7 +51,7 @@ __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
             for (int k = threadIdx.x; k <= nc; k += blockDim.x) {
                 float v = log_power(__ldg(re + k), __ldg(im + k));
                 if (p.specWidth == n && k > 0 && k < nc) v = 0.5f * (v + log_power(__ldg(re + n - k), __ldg(im + n - k)));
-                put_even(reinterpret_cast<float *>(L), n, k, v);
+                af_put_even(reinterpret_cast<float *>(L), n, k, v);
             }
         } else {
             const long long clip = f / p.timeLength, t = f % p.timeLength;
@@ -83,8 +65,8 @@ __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
             const float2 *X = af_stockham(A, B, nc, p.log2nc, p.tw);
             L = X == A ? B : A;
             for (int k = threadIdx.x; k <= nc; k += blockDim.x) {
-                const float2 z = real_bin(p, X, k);
-                put_even(reinterpret_cast<float *>(L), n, k, log_power(z.x, z.y));
+                const float2 z = af_real_bin(X, af_real_tw(p.tw, nc, k), k, nc);
+                af_put_even(reinterpret_cast<float *>(L), n, k, log_power(z.x, z.y));
             }
         }
         __syncthreads();
@@ -92,16 +74,16 @@ __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
         const float2 *Y = af_stockham(L, L == A ? B : A, nc, p.log2nc, p.tw);
         float2 *F = Y == A ? B : A;                                    // free: the envelope's input, packed
         for (int k = threadIdx.x; k <= nc; k += blockDim.x) {
-            const float y = real_bin(p, Y, k).x * inv;
+            const float y = af_real_bin(Y, af_real_tw(p.tw, nc, k), k, nc).x * inv;
             if (p.cep) p.cep[row + k] = y;
-            if (p.env) put_even(reinterpret_cast<float *>(F), n, k, k <= c ? y : 0.0f);
+            if (p.env) af_put_even(reinterpret_cast<float *>(F), n, k, k <= c ? y : 0.0f);
             if (p.det) ys[k] = y;
         }
         __syncthreads();
 
         if (p.env) {
             const float2 *V = af_stockham(F, F == A ? B : A, nc, p.log2nc, p.tw);
-            for (int k = threadIdx.x; k <= nc; k += blockDim.x) p.env[row + k] = real_bin(p, V, k).x;
+            for (int k = threadIdx.x; k <= nc; k += blockDim.x) p.env[row + k] = af_real_bin(V, af_real_tw(p.tw, nc, k), k, nc).x;
             F = V == A ? B : A;
         }
         if (p.det) {                                                   // y on {c+1 .. N-c}, y[m] = y[N-m] above N/2
@@ -109,7 +91,7 @@ __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
             for (int m = threadIdx.x; m < n; m += blockDim.x) d[m] = m > c && m <= n - c ? ys[m <= nc ? m : n - m] : 0.0f;
             __syncthreads();
             const float2 *W = af_stockham(F, F == A ? B : A, nc, p.log2nc, p.tw);
-            for (int k = threadIdx.x; k <= nc; k += blockDim.x) p.det[row + k] = real_bin(p, W, k).x;
+            for (int k = threadIdx.x; k <= nc; k += blockDim.x) p.det[row + k] = af_real_bin(W, af_real_tw(p.tw, nc, k), k, nc).x;
         }
         __syncthreads();                                               // the buffers are free for the next frame
     }
@@ -117,10 +99,8 @@ __global__ void __launch_bounds__(1024) k_cepstrogram(CepsParams p) {
 
 template <bool kPlanes>
 int launch(const CepsParams &p, unsigned grid, int threads, size_t smem, cudaStream_t st) {
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_cepstrogram<kPlanes>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cepstrogram)");
-    }
+    const int rc = af_smem_optin(k_cepstrogram<kPlanes>, smem, "k_cepstrogram");
+    if (rc) return rc;
     k_cepstrogram<kPlanes><<<grid, threads, smem, st>>>(p);
     AF_LAUNCH_CHECK("k_cepstrogram");
     return AF_OK;
@@ -147,8 +127,7 @@ extern "C" int af_launch_cepstrogram(const AfCepsArgs *a, void *stream) {
     p.framesPerCta = n <= 256 ? 2048 / n : 1;
     const long long grid = (p.frames + p.framesPerCta - 1) / p.framesPerCta;
     if (grid > 0x7fffffffLL) return af_fail(AF_ERR_ARG, "cepstrogram: too many frames in one launch");
-    int threads = nc / 4;
-    threads = threads < 32 ? 32 : threads > 1024 ? 1024 : threads;
+    const int threads = af_cta_threads(nc / 4, 1024);
     const size_t smem = sizeof(float2) * 2 * (size_t)nc + (p.det ? sizeof(float) * (size_t)(nc + 1) : 0);
     cudaStream_t st = (cudaStream_t)stream;
     return planes ? launch<true>(p, (unsigned)grid, threads, smem, st) : launch<false>(p, (unsigned)grid, threads, smem, st);

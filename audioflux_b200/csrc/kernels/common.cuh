@@ -11,6 +11,17 @@
         if (e__ != cudaSuccess) return af_fail(AF_ERR_CUDA, "%s launch: %s", what, cudaGetErrorString(e__)); \
     } while (0)
 
+// dynamic shared memory above the default 48 KB needs the kernel's opt-in before its launch
+template <typename K>
+static inline int af_smem_optin(K kernel, size_t bytes, const char *name) {
+    if (bytes <= 48 * 1024) return AF_OK;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    return e == cudaSuccess ? AF_OK : af_fail(AF_ERR_CUDA, "cudaFuncSetAttribute(%s): %s", name, cudaGetErrorString(e));
+}
+
+// CTA size: `want` threads, clamped to [lo, hi]
+static inline int af_cta_threads(int want, int hi, int lo = 32) { return want < lo ? lo : want > hi ? hi : want; }
+
 __device__ __forceinline__ uint32_t af_smem_u32(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

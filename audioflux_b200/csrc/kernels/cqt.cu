@@ -453,8 +453,8 @@ extern "C" int af_launch_cqt_octave(const AfCqtOctPlan *plan, const float *sig, 
         AF_LAUNCH_CHECK("k_cqt_octave_direct");
         return AF_OK;
     }
-    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
-    if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave)");
+    const int rc = af_smem_optin(k_cqt_octave, plan->smem, "k_cqt_octave");
+    if (rc) return rc;
     dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
     k_cqt_octave<<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK("k_cqt_octave");
@@ -499,8 +499,8 @@ extern "C" int af_launch_cqt_octave_tc(const AfCqtOctPlan *plan, const float *si
     p.bfrag = reinterpret_cast<const float4 *>(bfrag); p.scale = scale;
     p.outRe = outRe; p.outIm = outIm; p.outStride = (long long)timeLength * num; p.num = num; p.colOff = colOff;
     p.warps = plan->warps; p.TT = plan->TT; p.rowLen = plan->rowLen;
-    cudaError_t e = cudaFuncSetAttribute(k_cqt_octave_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
-    if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_tc)");
+    const int rc = af_smem_optin(k_cqt_octave_tc, plan->smem, "k_cqt_octave_tc");
+    if (rc) return rc;
     dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
     k_cqt_octave_tc<<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK("k_cqt_octave_tc");

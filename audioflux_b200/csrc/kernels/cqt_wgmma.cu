@@ -234,14 +234,12 @@ extern "C" int af_launch_cqt_octave_wgmma(const AfCqtOctPlan *plan, const float 
     p.rowLen = plan->rowLen;
     p.TT = plan->TT;
     const dim3 grid((unsigned)((timeLength + p.TT - 1) / p.TT), (unsigned)batch);
-    cudaError_t e;
+    int rc;
     if (plan->mt == kWgMT) {
-        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<kWgMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_wgmma)");
+        if ((rc = af_smem_optin(k_cqt_octave_wgmma<kWgMT>, plan->smem, "k_cqt_octave_wgmma"))) return rc;
         k_cqt_octave_wgmma<kWgMT><<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     } else {
-        e = cudaFuncSetAttribute(k_cqt_octave_wgmma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, plan->smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_cqt_octave_wgmma)");
+        if ((rc = af_smem_optin(k_cqt_octave_wgmma<1>, plan->smem, "k_cqt_octave_wgmma"))) return rc;
         k_cqt_octave_wgmma<1><<<grid, plan->threads, plan->smem, (cudaStream_t)stream>>>(p);
     }
     AF_LAUNCH_CHECK("k_cqt_octave_wgmma");

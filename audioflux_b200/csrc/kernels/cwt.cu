@@ -14,6 +14,7 @@
 // For N <= 4096 the columns kernel alone is the whole transform (N2 = 1); at N = 2 that is one radix-2 pass.
 // Shared-memory legs use the same Stockham radix-4/2 autosort passes as stft_generic.cu.
 #include <math.h>
+#include <string.h>
 #include "common.cuh"
 #include "fft32_gen.cuh"
 
@@ -629,25 +630,54 @@ void fill_params(const AfCwtArgs *a, CwtParams *p) {
     while (p->rows > 1 && sizeof(float2) * 2 * (size_t)p->rows * (p->N2 + 1) > budget) p->rows >>= 1;
 }
 
-template <typename K>
-int set_smem(K kernel, size_t bytes, const char *name) {
-    if (bytes <= 48 * 1024) return AF_OK;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    return e == cudaSuccess ? AF_OK : af_cuda_check(e, name);
+// fast path (N = 2^19): warp-level forward legs, persistent fused inverse legs over a small ring of inter-leg slots
+bool cwt_fused_enabled(int log2n) { return log2n == 19; }
+constexpr int kGroupItems = 2;                           // 3 slots x 2 items x 4 MB = 24 MB: half of the 50 MB L2 of an H100
+
+// shared memory of the columns / rows legs outside the fast path
+size_t smem_cols(const CwtParams &p) { return sizeof(float2) * (2 * (size_t)p.cols * (p.N1 + 1) + p.N1 + p.N2); }
+size_t smem_rows(const CwtParams &p) { return sizeof(float2) * (2 * (size_t)p.rows * (p.N2 + 1) + p.N2); }
+int check_leg_smem(const CwtParams &p) {
+    if (smem_cols(p) > 220 * 1024 || smem_rows(p) > 220 * 1024)
+        return af_fail(AF_ERR_UNSUPPORTED, "CWT length 2^%d does not fit the shared-memory FFT legs", p.log2N);
+    return AF_OK;
+}
+
+// the forward legs: the real rows p.data [batch][N] -> spectra p.spec [batch][N], through one inter-leg slot per row at
+// p.work
+int launch_forward(const CwtParams &p, cudaStream_t st) {
+    int rc;
+    if (cwt_fused_enabled(p.log2N)) {
+        // warp-level transforms (see k_cwt_cols_w / k_cwt_rows_w)
+        const size_t smC = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (1024 + p.N2 + 1024);
+        const size_t smR = sizeof(c64) * (size_t)kWRows * kWRowPitch + sizeof(float2) * 512;
+        if ((rc = af_smem_optin(k_cwt_cols_w<0>, smC, "k_cwt_cols_w<0>")) || (rc = af_smem_optin(k_cwt_rows_w<0>, smR, "k_cwt_rows_w<0>"))) return rc;
+        k_cwt_cols_w<0><<<dim3((unsigned)p.batch, (unsigned)(p.N2 / kWCols)), kWCols * 32, smC, st>>>(p);
+        AF_LAUNCH_CHECK("k_cwt_cols_w<0>");
+        k_cwt_rows_w<0><<<dim3((unsigned)p.batch, (unsigned)(p.N1 / kWRows)), kWRows * 16, smR, st>>>(p);
+        AF_LAUNCH_CHECK("k_cwt_rows_w<0>");
+        return AF_OK;
+    }
+    if ((rc = check_leg_smem(p))) return rc;
+    const size_t smemC = smem_cols(p), smemR = smem_rows(p);
+    if ((rc = af_smem_optin(k_cwt_cols<0>, smemC, "k_cwt_cols<0>")) || (rc = af_smem_optin(k_cwt_rows<0>, smemR, "k_cwt_rows<0>"))) return rc;
+    k_cwt_cols<0><<<dim3((unsigned)p.batch, (unsigned)((p.N2 + p.cols - 1) / p.cols)), 512, smemC, st>>>(p);
+    AF_LAUNCH_CHECK("k_cwt_cols<0>");
+    if (p.N2 > 1) {
+        k_cwt_rows<0><<<dim3((unsigned)p.batch, (unsigned)((p.N1 + p.rows - 1) / p.rows)), 512, smemR, st>>>(p);
+        AF_LAUNCH_CHECK("k_cwt_rows<0>");
+    }
+    return AF_OK;
 }
 
 }  // namespace
-
-// fast path (N = 2^19): persistent fused inverse legs over a small ring of inter-leg slots
-static int cwt_fused_enabled(const AfCwtArgs *a) { return a->log2n == 19; }
-constexpr int kGroupItems = 2;                           // 3 slots x 2 items x 4 MB = 24 MB: half of the 50 MB L2 of an H100
 
 // workspace = forward spectrum (batch x N float2) + inter-leg buffer: batch x num x N float2 when N > 4096, or -- fused
 // fast path -- a ring of kRing x kGroupItems item slots plus the unit counters
 extern "C" size_t af_cwt_workspace_bytes(const AfCwtArgs *a) {
     const size_t N = (size_t)1 << a->log2n;
     size_t bytes = sizeof(float2) * N * (size_t)a->batch;
-    if (cwt_fused_enabled(a)) {
+    if (cwt_fused_enabled(a->log2n)) {
         // the forward transform of the chunk uses one inter-leg slot per clip, the fused inverse the ring
         size_t slots = (size_t)kRing * kGroupItems;
         if ((size_t)a->batch > slots) slots = (size_t)a->batch;
@@ -666,11 +696,8 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
     p.work = p.spec + (size_t)p.N * a->batch;
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    if (cwt_fused_enabled(a)) {
-        // warp-level transforms (see k_cwt_cols_w / k_cwt_rows_w): forward legs, then both inverse legs fused
-        const size_t smC = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (1024 + p.N2 + 1024);
-        const size_t smR = sizeof(c64) * (size_t)kWRows * kWRowPitch + sizeof(float2) * 512;
-        if ((rc = set_smem(k_cwt_cols_w<0>, smC, "smem k_cwt_cols_w<0>")) || (rc = set_smem(k_cwt_rows_w<0>, smR, "smem k_cwt_rows_w<0>"))) return rc;
+    if (cwt_fused_enabled(a->log2n)) {
+        // forward legs, then both inverse legs fused
         const unsigned cb = (unsigned)(p.N2 / kWCols), rb = (unsigned)(p.N1 / kWRows), items = (unsigned)(a->batch * a->num);
         if (a->support && a->supportReady) {
             if (!*a->supportReady) {                       // once per object: peak and [lo, hi) of every bank row
@@ -687,13 +714,7 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
             }
             p.support = a->support;
         }
-        if (data) {                                        // NULL: reuse the spectra already in the workspace
-            k_cwt_cols_w<0><<<dim3((unsigned)a->batch, cb), kWCols * 32, smC, st>>>(p);
-            AF_LAUNCH_CHECK("k_cwt_cols_w<0>");
-            k_cwt_rows_w<0><<<dim3((unsigned)a->batch, rb), kWRows * 16, smR, st>>>(p);
-            AF_LAUNCH_CHECK("k_cwt_rows_w<0>");
-        }
-        if (a->forwardOnly) return AF_OK;
+        if (data && (rc = launch_forward(p, st))) return rc;   // NULL: reuse the spectra already in the workspace
         FusedParams f;
         f.p = p;
         f.items = (int)items; f.groupItems = kGroupItems; f.groups = (f.items + f.groupItems - 1) / f.groupItems;
@@ -707,40 +728,50 @@ extern "C" int af_launch_cwt(const AfCwtArgs *a, const float *data, void *worksp
         cudaError_t e = cudaMemsetAsync(f.counters, 0, (size_t)(1 + 2 * f.groups) * sizeof(unsigned), st);
         if (e != cudaSuccess) return af_cuda_check(e, "cudaMemsetAsync(cwt counters)");
         const size_t smF = sizeof(c64) * (size_t)kWCols * kWColPitch + sizeof(float2) * (2048 + p.N2 + 512);
-        if ((rc = set_smem(k_cwt_fused_w, smF, "smem k_cwt_fused_w"))) return rc;
+        if ((rc = af_smem_optin(k_cwt_fused_w, smF, "k_cwt_fused_w"))) return rc;
         int sms = af_sm_count();
         if (sms <= 0) sms = 132;
         k_cwt_fused_w<<<(unsigned)(2 * sms), 256, smF, st>>>(f);
         AF_LAUNCH_CHECK("k_cwt_fused_w");
         return AF_OK;
     }
-    const int threads = 512;
-    const size_t smemC = sizeof(float2) * (2 * (size_t)p.cols * (p.N1 + 1) + p.N1 + p.N2);
-    const size_t smemR = sizeof(float2) * (2 * (size_t)p.rows * (p.N2 + 1) + p.N2);
-    if (smemC > 220 * 1024 || smemR > 220 * 1024) return af_fail(AF_ERR_UNSUPPORTED, "CWT length 2^%d does not fit the shared-memory FFT legs", a->log2n);
-    if ((rc = set_smem(k_cwt_cols<0>, smemC, "smem k_cwt_cols<0>")) || (rc = set_smem(k_cwt_cols<1>, smemC, "smem k_cwt_cols<1>")) ||
-        (rc = set_smem(k_cwt_rows<0>, smemR, "smem k_cwt_rows<0>")) || (rc = set_smem(k_cwt_rows<1>, smemR, "smem k_cwt_rows<1>"))) return rc;
-    const unsigned colBlocks = (unsigned)((p.N2 + p.cols - 1) / p.cols);
-    const unsigned rowBlocks = (unsigned)((p.N1 + p.rows - 1) / p.rows);
-    // forward transform of every clip
-    if (data) {                                            // NULL: reuse the spectra already in the workspace
-        k_cwt_cols<0><<<dim3((unsigned)a->batch, colBlocks), threads, smemC, st>>>(p);
-        AF_LAUNCH_CHECK("k_cwt_cols<0>");
-        if (p.N2 > 1) {
-            k_cwt_rows<0><<<dim3((unsigned)a->batch, rowBlocks), threads, smemR, st>>>(p);
-            AF_LAUNCH_CHECK("k_cwt_rows<0>");
-        }
-    }
-    if (a->forwardOnly) return AF_OK;
+    if ((rc = check_leg_smem(p))) return rc;
+    const size_t smemC = smem_cols(p), smemR = smem_rows(p);
+    if ((rc = af_smem_optin(k_cwt_cols<1>, smemC, "k_cwt_cols<1>")) || (rc = af_smem_optin(k_cwt_rows<1>, smemR, "k_cwt_rows<1>"))) return rc;
+    if (data && (rc = launch_forward(p, st))) return rc;   // NULL: reuse the spectra already in the workspace
     // per (clip, scale): wavelet * spectrum -> inverse transform -> planes
     const unsigned items = (unsigned)(a->batch * a->num);
-    k_cwt_cols<1><<<dim3(items, colBlocks), threads, smemC, st>>>(p);
+    k_cwt_cols<1><<<dim3(items, (unsigned)((p.N2 + p.cols - 1) / p.cols)), 512, smemC, st>>>(p);
     AF_LAUNCH_CHECK("k_cwt_cols<1>");
     if (p.N2 > 1) {
-        k_cwt_rows<1><<<dim3(items, rowBlocks), threads, smemR, st>>>(p);
+        k_cwt_rows<1><<<dim3(items, (unsigned)((p.N1 + p.rows - 1) / p.rows)), 512, smemR, st>>>(p);
         AF_LAUNCH_CHECK("k_cwt_rows<1>");
     }
     return AF_OK;
+}
+
+// long real FFTs for other transforms (STFT / ISTFT frames and cross-correlation rows of 2^15 .. 2^20 points): the forward
+// legs alone, workspace = spectra + one inter-leg slot per row
+extern "C" size_t af_fft_rows_workspace_bytes(int log2n, int rows) { return 2 * sizeof(float2) * ((size_t)rows << log2n); }
+
+extern "C" long long af_fft_rows_chunk(int log2n, long long rows) {
+    const size_t perRow = sizeof(float) * ((size_t)1 << log2n) + af_fft_rows_workspace_bytes(log2n, 1);   // 20 bytes per sample
+    long long chunk = (long long)(((size_t)512 << 20) / perRow);
+    if (chunk < 1) chunk = 1;
+    return chunk < rows ? chunk : rows;
+}
+
+extern "C" int af_launch_fft_rows(const float *x, int log2n, int rows, void *workspace, void *stream) {
+    if (log2n < 15 || log2n > 20) return af_fail(AF_ERR_UNSUPPORTED, "long FFT length 2^%d is outside [2^15, 2^20]", log2n);
+    AfCwtArgs a;
+    memset(&a, 0, sizeof(a));
+    a.log2n = log2n; a.num = 1; a.batch = rows; a.dataLength = 1 << log2n;
+    CwtParams p;
+    fill_params(&a, &p);
+    p.data = x; p.outRe = nullptr; p.outIm = nullptr;
+    p.spec = static_cast<float2 *>(workspace);
+    p.work = p.spec + (size_t)p.N * rows;
+    return launch_forward(p, (cudaStream_t)stream);
 }
 
 extern "C" int af_launch_cwt_bank_table(const AfCwtArgs *a, float *bank, void *stream) {

@@ -30,11 +30,6 @@ __device__ __forceinline__ float2 cmul_ref(float2 a, float2 b) {   // __complexM
     return make_float2(a.x * b.x - a.y * b.y, a.y * b.x + a.x * b.y);
 }
 
-int threads_for(int M) {
-    const int t = M / 2;
-    return t < 32 ? 32 : t > kMaxThreads ? kMaxThreads : t;
-}
-
 __global__ void __launch_bounds__(kMaxThreads) k_czt(CztParams p) {
     extern __shared__ float2 a[];
     const int N = p.N, M = p.M, tid = threadIdx.x, bd = blockDim.x;
@@ -77,13 +72,6 @@ __global__ void __launch_bounds__(kMaxThreads) k_czt_filter(float2 *H, int M, co
     for (int j = threadIdx.x; j < M; j += blockDim.x) H[j] = a[j];
 }
 
-template <typename K>
-int prepare(K kernel, size_t smem, const char *what) {
-    if (smem <= 48 * 1024) return AF_OK;
-    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    return e == cudaSuccess ? AF_OK : af_cuda_check(e, what);
-}
-
 }  // namespace
 
 extern "C" int af_launch_czt_filter(float *H, int log2m, void *stream) {
@@ -92,9 +80,9 @@ extern "C" int af_launch_czt_filter(float *H, int log2m, void *stream) {
     const float2 *tw = af_twiddle_table(log2m);
     if (!tw) return af_fail(AF_ERR_CUDA, "czt: twiddle table 2^%d", log2m);
     const size_t smem = sizeof(float2) * (size_t)M;
-    int rc = prepare(k_czt_filter, smem, "cudaFuncSetAttribute(k_czt_filter)");
+    const int rc = af_smem_optin(k_czt_filter, smem, "k_czt_filter");
     if (rc) return rc;
-    k_czt_filter<<<1, threads_for(M), smem, (cudaStream_t)stream>>>(reinterpret_cast<float2 *>(H), M, tw);
+    k_czt_filter<<<1, af_cta_threads(M / 2, kMaxThreads), smem, (cudaStream_t)stream>>>(reinterpret_cast<float2 *>(H), M, tw);
     AF_LAUNCH_CHECK("k_czt_filter");
     return AF_OK;
 }
@@ -111,9 +99,9 @@ extern "C" int af_launch_czt(const AfCztArgs *a, void *stream) {
     p.tw = af_twiddle_table(p.log2m);
     if (!p.tw) return af_fail(AF_ERR_CUDA, "czt: twiddle table 2^%d", p.log2m);
     const size_t smem = sizeof(float2) * (size_t)p.M;
-    int rc = prepare(k_czt, smem, "cudaFuncSetAttribute(k_czt)");
+    const int rc = af_smem_optin(k_czt, smem, "k_czt");
     if (rc) return rc;
-    k_czt<<<(unsigned)a->batch, threads_for(p.M), smem, (cudaStream_t)stream>>>(p);
+    k_czt<<<(unsigned)a->batch, af_cta_threads(p.M / 2, kMaxThreads), smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK("k_czt");
     return AF_OK;
 }

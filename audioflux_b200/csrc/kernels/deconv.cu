@@ -59,10 +59,8 @@ extern "C" int af_launch_cq_deconv(const float *in, int rows, int num, int mode,
     while (L < 2 * num) { L <<= 1; lg++; }                 /* util_ceilPowerTwo(2 * num) */
     const size_t smem = sizeof(float2) * 3 * (size_t)L + sizeof(float) * (size_t)L;
     if (smem > 200 * 1024) return af_fail(AF_ERR_UNSUPPORTED, "cqhc / deconv: num=%d too large", num);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_cq_deconv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "smem k_cq_deconv");
-    }
+    const int rc = af_smem_optin(k_cq_deconv, smem, "k_cq_deconv");
+    if (rc) return rc;
     k_cq_deconv<<<(unsigned)rows, 128, smem, (cudaStream_t)stream>>>(in, num, L, lg, mode, hcNum, bpo, out0, out1);
     AF_LAUNCH_CHECK("k_cq_deconv");
     return AF_OK;

@@ -24,7 +24,7 @@
 // The file is compiled with -fmad=false (Makefile): every float step is rounded on its own, as in the reference.
 #include <climits>
 
-#include "common.cuh"
+#include "block_reduce.cuh"
 #include "stockham.cuh"
 
 namespace {
@@ -40,52 +40,6 @@ struct HrParams {
     long long frames;
     int w, log2w, maxLength, dataLength, hop, T;
 };
-
-// bin k (0 .. W) of the 2W-point real FFT whose W-point packed transform is z: X[k] = E[k] + W_2W^k O[k]
-__device__ __forceinline__ float2 real_bin(const HrParams &p, const float2 *z, int k) {
-    const int nc = p.w;
-    const float2 zk = z[k == nc ? 0 : k], zp = z[k == 0 ? 0 : nc - k];
-    const float er = 0.5f * (zk.x + zp.x), ei = 0.5f * (zk.y - zp.y);
-    const float orr = 0.5f * (zk.y + zp.y), oi = -0.5f * (zk.x - zp.x);
-    const float2 w = __ldg(p.tw + nc + k);                             // exp(-2 pi i k / 2W)
-    float xr = er + (w.x * orr - w.y * oi), xi = ei + (w.x * oi + w.y * orr);
-    if (k == 0 || k == nc) xi = 0.0f;
-    return make_float2(xr, xi);
-}
-
-// block minimum (isMax = false) or maximum of an int; every thread gets it.  red: 32 ints
-__device__ int block_reduce_int(int v, bool isMax, int *red) {
-    v = isMax ? __reduce_max_sync(FULL, v) : __reduce_min_sync(FULL, v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    __syncthreads();                                                   // red[] may still be read from the last reduction
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    v = red[0];
-    for (int i = 1; i < nw; i++) v = isMax ? max(v, red[i]) : min(v, red[i]);
-    return v;
-}
-
-// (v, i) beats (w, j): i is a candidate and either j is none, v > w, or they tie and i comes first
-__device__ __forceinline__ bool beats(float v, int i, float w, int j) {
-    return i >= 0 && (j < 0 || v > w || (v == w && i < j));
-}
-
-// first index of the block's maximum over the candidates (i >= 0); -1 when there is none.  redv / redi: 32 each
-__device__ int block_argmax(float v, int i, float *redv, int *redi) {
-    for (int o = 16; o; o >>= 1) {
-        const float w = __shfl_xor_sync(FULL, v, o);
-        const int j = __shfl_xor_sync(FULL, i, o);
-        if (beats(w, j, v, i)) { v = w; i = j; }
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    __syncthreads();
-    if (lane == 0) { redv[warp] = v; redi[warp] = i; }
-    __syncthreads();
-    v = redv[0]; i = redi[0];
-    for (int k = 1; k < nw; k++)
-        if (beats(redv[k], redi[k], v, i)) { v = redv[k]; i = redi[k]; }
-    return i;
-}
 
 // in-place inclusive prefix sum of s[0 .. n): each thread sums a run of consecutive values, then the runs are offset
 __device__ void block_scan(float *s, int n, float *redv) {
@@ -126,18 +80,15 @@ __device__ void hr_frame(const HrParams &p, long long f, int m, float2 *A, float
     const float2 *X = af_stockham(A, B, W, p.log2w, p.tw);
     float2 *P = X == A ? B : A;
     for (int k = tid; k <= W; k += bd) {
-        const float2 z = real_bin(p, X, k);
-        const float v = z.x * z.x + z.y * z.y;
-        float *pf = reinterpret_cast<float *>(P);
-        pf[k] = v;
-        if (k > 0 && k < W) pf[n - k] = v;
+        const float2 z = af_real_bin(X, __ldg(p.tw + W + k), k, W);          // exp(-2 pi i k / 2W)
+        af_put_even(reinterpret_cast<float *>(P), n, k, z.x * z.x + z.y * z.y);
     }
     __syncthreads();
     const float2 *Y = af_stockham(P, P == A ? B : A, W, p.log2w, p.tw);
     float *const r = reinterpret_cast<float *>(Y == A ? B : A);       // r[0 .. L]; the prefix sums E behind it
     float *const E = r + W;
     const float inv = 1.0f / (float)n;
-    for (int k = tid; k <= L; k += bd) r[k] = real_bin(p, Y, k).x * inv;
+    for (int k = tid; k <= L; k += bd) r[k] = af_real_bin(Y, __ldg(p.tw + W + k), k, W).x * inv;
     for (int j = tid; j < W; j += bd) {
         const float v = __ldg(x + j) * __ldg(p.window + j);
         E[j] = v * v;
@@ -220,13 +171,6 @@ __global__ void __launch_bounds__(kMaxThreads) k_harmonic_ratio_carry(HrParams p
     }
 }
 
-template <typename K>
-int prepare(K kernel, size_t smem, const char *what) {
-    if (smem <= 48 * 1024) return AF_OK;
-    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    return e == cudaSuccess ? AF_OK : af_cuda_check(e, what);
-}
-
 }  // namespace
 
 extern "C" int af_launch_harmonic_ratio(const AfHarmonicRatioArgs *a, void *stream) {
@@ -245,12 +189,11 @@ extern "C" int af_launch_harmonic_ratio(const AfHarmonicRatioArgs *a, void *stre
     if (!p.tw) return af_fail(AF_ERR_CUDA, "harmonic ratio: twiddle table 2^%d", a->log2w);
     p.w = W; p.log2w = a->log2w; p.maxLength = a->maxLength;
     p.dataLength = a->dataLength; p.hop = a->hop; p.T = a->timeLength;
-    int threads = W / 4;
-    threads = threads < 32 ? 32 : threads > kMaxThreads ? kMaxThreads : threads;
+    const int threads = af_cta_threads(W / 4, kMaxThreads);
     const size_t smem = sizeof(float2) * 2 * (size_t)W;
     int rc;
-    if ((rc = prepare(k_harmonic_ratio, smem, "cudaFuncSetAttribute(k_harmonic_ratio)")) ||
-        (rc = prepare(k_harmonic_ratio_carry, smem, "cudaFuncSetAttribute(k_harmonic_ratio_carry)")))
+    if ((rc = af_smem_optin(k_harmonic_ratio, smem, "k_harmonic_ratio")) ||
+        (rc = af_smem_optin(k_harmonic_ratio_carry, smem, "k_harmonic_ratio_carry")))
         return rc;
     cudaStream_t st = (cudaStream_t)stream;
     k_harmonic_ratio<<<(unsigned)p.frames, threads, smem, st>>>(p);

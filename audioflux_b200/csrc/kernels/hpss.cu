@@ -170,10 +170,8 @@ extern "C" int af_launch_hpss_mask(const AfHpssArgs *a, void *stream) {
     if (gx > 0x7fffffffLL || gy > 65535) return af_fail(AF_ERR_ARG, "hpss mask: too many tiles in one launch");
     const size_t smem = hpss_smem_bytes(a->hOrder, a->pOrder);
     cudaStream_t st = (cudaStream_t)stream;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_hpss_mask, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_hpss_mask)");
-    }
+    const int rc = af_smem_optin(k_hpss_mask, smem, "k_hpss_mask");
+    if (rc) return rc;
     k_hpss_mask<<<dim3((unsigned)gx, (unsigned)gy), kKB, smem, st>>>(p);
     AF_LAUNCH_CHECK("k_hpss_mask");
     return AF_OK;

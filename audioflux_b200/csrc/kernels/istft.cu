@@ -7,11 +7,10 @@
 // Two kernels: frames (one CTA per frame, shared-memory Stockham FFT) and a gather over the <= n/hop frames that
 // cover an output sample, summed in ascending frame order like the reference's loop (bit-stable, no atomics).
 // Frames of 2^15 .. 2^20 points (the reference accepts radix2Exp up to 30, src/stft_algorithm.c:114-117) do not fit a
-// CTA: Re(IFFT_n(X)) is taken from ONE real-input forward transform of the four-step kernels (kernels/cwt.cu, forward
-// leg) by the Hartley identity -- with H = the Hermitian part of X (the only part Re(IFFT) sees) and the real sequence
+// CTA: Re(IFFT_n(X)) is taken from ONE real-input forward transform of the four-step legs (af_launch_fft_rows,
+// kernels/cwt.cu) by the Hartley identity -- with H = the Hermitian part of X (the only part Re(IFFT) sees) and the real sequence
 // c[k] = Re H[k] + Im H[k],  C = FFT_n(c):   Re(IFFT_n(X))[j] = (Re C[j] + Im C[j]) / n.
 #include <math.h>
-#include <string.h>
 #include "common.cuh"
 #include "stockham.cuh"
 
@@ -63,7 +62,7 @@ __global__ void k_istft_frames_inplace(const float *__restrict__ re, const float
     const float inv = 1.0f / (float)n;
     float *f = frames + row * n;
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
-        float v = a[__brev((unsigned)j) >> (32 - log2n)].x * inv;
+        float v = a[af_brev(j, log2n)].x * inv;
         if (weightMode && window) v *= window[j];
         f[j] = v;
     }
@@ -118,32 +117,27 @@ __global__ void __launch_bounds__(256) k_istft_long_post(const float2 *__restric
 
 }  // namespace
 
-// frames of more than 16384 points: chunks of frames through a stream-ordered workspace (real sequence + spectrum +
-// inter-leg buffer = 20 bytes per sample, <= 512 MB at a time), as the forward side does (stft_generic.cu)
+// frames of more than 16384 points: chunks of frames (af_fft_rows_chunk) through a stream-ordered workspace, as the
+// forward side does (stft_generic.cu)
 static int launch_istft_frames_long(const float *re, const float *im, int width, int n, int log2n, long long rows,
                                     const float *window, int weightMode, float *frames, cudaStream_t st) {
-    const size_t perFrame = (size_t)n * (sizeof(float) + 2 * sizeof(float2));
-    long long chunk = (long long)(((size_t)512 << 20) / perFrame);
-    if (chunk < 1) chunk = 1;
-    if (chunk > rows) chunk = rows;
+    const long long chunk = af_fft_rows_chunk(log2n, rows);
+    const size_t specBytes = af_fft_rows_workspace_bytes(log2n, (int)chunk);
     void *ws = nullptr;
-    cudaError_t e = cudaMallocAsync(&ws, perFrame * (size_t)chunk, st);
+    cudaError_t e = cudaMallocAsync(&ws, specBytes + sizeof(float) * (size_t)n * chunk, st);
     if (e != cudaSuccess) return af_cuda_check(e, "cudaMallocAsync(long-frame ISTFT workspace)");
-    float2 *spec = static_cast<float2 *>(ws);                              // [chunk][n] spectrum + [chunk][n] inter-leg buffer
-    float *c = reinterpret_cast<float *>(spec + 2 * (size_t)chunk * n);
+    float2 *spec = static_cast<float2 *>(ws);
+    float *c = reinterpret_cast<float *>(static_cast<char *>(ws) + specBytes);
     int rc = AF_OK;
     for (long long r0 = 0; r0 < rows && rc == AF_OK; r0 += chunk) {
         const int nf = (int)(rows - r0 < chunk ? rows - r0 : chunk);
         const long long cells = (long long)nf * n;
         k_istft_long_pre<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(re, im, width, n, r0, nf, c);
         af_count_launch(1);
-        AfCwtArgs a;
-        memset(&a, 0, sizeof(a));
-        a.log2n = log2n; a.num = 1; a.batch = nf; a.padLength = 0; a.dataLength = n; a.forwardOnly = 1;
-        if ((rc = af_launch_cwt(&a, c, spec, nullptr, nullptr, st))) break;
+        if ((rc = af_launch_fft_rows(c, log2n, nf, spec, st))) break;
         k_istft_long_post<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(spec, n, r0, nf, window, weightMode, frames);
         af_count_launch(1);
-        if (cudaGetLastError() != cudaSuccess) rc = af_fail(AF_ERR_CUDA, "long-frame ISTFT launch failed");
+        if ((e = cudaGetLastError()) != cudaSuccess) rc = af_cuda_check(e, "long-frame ISTFT launch");
     }
     cudaFreeAsync(ws, st);
     return rc;
@@ -167,15 +161,12 @@ extern "C" int af_launch_istft(const float *re, const float *im, int width, int 
         AF_LAUNCH_CHECK("k_istft_ola");
         return AF_OK;
     }
-    size_t smem = sizeof(float2) * 2 * (size_t)fftLength;
-    const bool inplace = smem > 200 * 1024;                     /* 16384 points: one buffer, in-place passes */
-    if (inplace) smem /= 2;
-    if (smem > 48 * 1024) {
-        cudaError_t e = inplace ? cudaFuncSetAttribute(k_istft_frames_inplace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                : cudaFuncSetAttribute(k_istft_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_istft_frames)");
-    }
-    int threads = fftLength / 4; if (threads < 32) threads = 32; if (threads > 1024) threads = 1024;
+    const bool inplace = af_fft_inplace(fftLength);
+    const size_t smem = sizeof(float2) * (inplace ? 1 : 2) * (size_t)fftLength;
+    const int rc = inplace ? af_smem_optin(k_istft_frames_inplace, smem, "k_istft_frames_inplace")
+                           : af_smem_optin(k_istft_frames, smem, "k_istft_frames");
+    if (rc) return rc;
+    const int threads = af_cta_threads(fftLength / 4, 1024);
     if (inplace)
         k_istft_frames_inplace<<<(unsigned)((long long)batch * timeLength), threads, smem, st>>>(re, im, width, fftLength, log2n, window,
                                                                                                 weightMode, frames, af_twiddle_table(log2n));

@@ -71,8 +71,8 @@ inline int af_mfcc_launch_ct(void (*const kernels[4])(P), const char *name, int 
     if (sms <= 0) sms = 132;
     const long long grid = tiles < (long long)sms ? tiles : (long long)sms;
     void (*k)(P) = kernels[ct == 2 ? 0 : ct == 3 ? 1 : ct == 5 ? 2 : 3];
-    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return af_cuda_check(e, name);   // (cudaFuncSetAttribute)
+    const int rc = af_smem_optin(k, smem, name);
+    if (rc) return rc;
     k<<<(unsigned)grid, threads, smem, (cudaStream_t)stream>>>(p);
     AF_LAUNCH_CHECK(name);
     return AF_OK;

@@ -153,22 +153,18 @@ extern "C" int af_launch_nsgt(const AfNsgtArgs *a, void *stream) {
     for (int l = 0; l < 14; l++) p.tw[l] = (l >= 1 && l <= log2MaxM) ? af_twiddle_table(l) : nullptr;
     if (a->nGroups > 0) {
         if ((long long)a->nGroups * a->batch > 0x7fffffffLL) return af_fail(AF_ERR_ARG, "NSGT: too many clips in one launch");
-        int threads = a->maxM / 4;
-        threads = threads < 64 ? 64 : threads > 512 ? 512 : threads;
         const size_t smem = sizeof(float2) * 2 * (size_t)a->maxM;
-        if (smem > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(k_nsgt_bluestein, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_nsgt_bluestein)");
-        }
-        k_nsgt_bluestein<<<(unsigned)(a->nGroups * a->batch), threads, smem, st>>>(p);
+        const int rc = af_smem_optin(k_nsgt_bluestein, smem, "k_nsgt_bluestein");
+        if (rc) return rc;
+        k_nsgt_bluestein<<<(unsigned)(a->nGroups * a->batch), af_cta_threads(a->maxM / 4, 512, 64), smem, st>>>(p);
         AF_LAUNCH_CHECK("k_nsgt_bluestein");
     }
     if (a->nDirect > 0) {
         if ((long long)a->nDirect * a->batch > 0x7fffffffLL) return af_fail(AF_ERR_ARG, "NSGT: too many clips in one launch");
         const size_t smem = sizeof(float2) * ((size_t)a->maxDirectL + kDirTile + AF_NSGT_FINE +
                                               (a->maxDirectL - 1) / AF_NSGT_FINE + 1);
-        cudaError_t e = cudaFuncSetAttribute(k_nsgt_direct, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_nsgt_direct)");
+        const int rc = af_smem_optin(k_nsgt_direct, smem, "k_nsgt_direct");
+        if (rc) return rc;
         k_nsgt_direct<<<(unsigned)(a->nDirect * a->batch), kDirThreads, smem, st>>>(p);
         AF_LAUNCH_CHECK("k_nsgt_direct");
     }

@@ -16,7 +16,7 @@
 //      greedy `wait` suppression and writes the points;
 //   4. the rest of the clip's points row is zeroed and its count stored.
 // No product is formed anywhere in the file (sums, differences, one division), so nothing can be contracted into an FMA.
-#include "common.cuh"
+#include "block_reduce.cuh"
 
 namespace {
 
@@ -41,21 +41,6 @@ __global__ void __launch_bounds__(256) k_onset_maxfilter(const float *__restrict
     }
 }
 
-// block reduction of fminf (isMax = 0) or fmaxf (isMax = 1); every thread gets the result
-__device__ float block_reduce(float v, int isMax, float *red) {
-    for (int o = 16; o; o >>= 1) {
-        const float w = __shfl_xor_sync(FULL, v, o);
-        v = isMax ? fmaxf(v, w) : fminf(v, w);
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();                       // red[] may still be read from the previous reduction
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    v = red[0];
-    for (int w = 1; w < kWarps; w++) v = isMax ? fmaxf(v, red[w]) : fminf(v, red[w]);
-    return v;
-}
-
 __global__ void __launch_bounds__(kThreads) k_onset_pick(const AfOnsetPickArgs a) {
     __shared__ float red[kWarps];
     __shared__ unsigned cand[kWarps];
@@ -67,7 +52,7 @@ __global__ void __launch_bounds__(kThreads) k_onset_pick(const AfOnsetPickArgs a
     // 1. normalisation
     float mn = __int_as_float(0x7f800000);
     for (int i = tid; i < T; i += kThreads) mn = fminf(mn, e[i]);
-    mn = block_reduce(mn, 0, red);
+    mn = block_reduce_float<kWarps>(mn, 0, red);
     const float e0 = e[0];
     if (e0 != e0) mn = e0;
     __syncthreads();                       // every thread has read e[0] before it changes
@@ -77,7 +62,7 @@ __global__ void __launch_bounds__(kThreads) k_onset_pick(const AfOnsetPickArgs a
         e[i] = v;
         mx = fmaxf(mx, v);
     }
-    mx = block_reduce(mx, 1, red);         // its barriers publish the differences
+    mx = block_reduce_float<kWarps>(mx, 1, red);       // its barriers publish the differences
     const float d0 = e[0];
     if (d0 != d0) mx = d0;
     __syncthreads();                       // every thread has read e[0] before it is divided

@@ -102,10 +102,8 @@ __global__ void __launch_bounds__(kThreads) k_resample(RsParams p) {
 
 template <bool kTableSmem>
 int launch(const RsParams &p, unsigned grid, size_t smem, cudaStream_t st) {
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_resample<kTableSmem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_resample)");
-    }
+    const int rc = af_smem_optin(k_resample<kTableSmem>, smem, "k_resample");
+    if (rc) return rc;
     k_resample<kTableSmem><<<grid, kThreads, smem, st>>>(p);
     AF_LAUNCH_CHECK("k_resample");
     return AF_OK;

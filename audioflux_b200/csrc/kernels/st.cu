@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(1024) k_st_rows(StParams p) {
         if (kInplace) {
             af_fft_inplace_dif(a, n, p.tw);
             for (int j = threadIdx.x; j < n; j += blockDim.x) {
-                const float2 y = a[__brev((unsigned)j) >> (32 - p.log2n)];
+                const float2 y = a[af_brev(j, p.log2n)];
                 p.outRe[row + j] = y.x * inv;
                 p.outIm[row + j] = -y.y * inv;
             }
@@ -198,22 +198,18 @@ extern "C" int af_launch_st(const float *data, const float *specRe, const float 
     p.groups = (rows + p.rowsPerCta - 1) / p.rowsPerCta;
     p.tw = af_twiddle_table(log2n);
     if ((long long)p.groups * batch > 0x7fffffffLL) return af_fail(AF_ERR_ARG, "ST: too many rows in one launch");
-    int threads = n / 4;
-    threads = threads < 32 ? 32 : threads > 1024 ? 1024 : threads;
-    const bool inplace = n > 8192;
+    const int threads = af_cta_threads(n / 4, 1024);
+    const bool inplace = af_fft_inplace(n);
     size_t smem = sizeof(float2) * (inplace ? 1 : 2) * (size_t)n;
     if (smem < 32 * sizeof(double)) smem = 32 * sizeof(double);     // the mean's reduction scratch
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned grid = (unsigned)((long long)p.groups * batch);
+    int rc;
     if (inplace) {
-        cudaError_t e = cudaFuncSetAttribute(k_st_rows<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_st_rows)");
+        if ((rc = af_smem_optin(k_st_rows<true>, smem, "k_st_rows"))) return rc;
         k_st_rows<true><<<grid, threads, smem, st>>>(p);
     } else {
-        if (smem > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(k_st_rows<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_st_rows)");
-        }
+        if ((rc = af_smem_optin(k_st_rows<false>, smem, "k_st_rows"))) return rc;
         k_st_rows<false><<<grid, threads, smem, st>>>(p);
     }
     AF_LAUNCH_CHECK("k_st_rows");
@@ -233,14 +229,10 @@ extern "C" int af_launch_fst(const float *specRe, const float *specIm, float *pa
     f.n = n; f.log2n = log2n; f.segs = log2n - 1;
     for (int l = 0; l < 14; l++) f.tw[l] = (l >= 1 && l <= log2n - 2) ? af_twiddle_table(l) : nullptr;
     if ((long long)f.segs * batch > 0x7fffffffLL) return af_fail(AF_ERR_ARG, "FST: too many clips in one launch");
-    int threads = n / 16;
-    threads = threads < 32 ? 32 : threads > 256 ? 256 : threads;
     const size_t smem = sizeof(float2) * 2 * (size_t)(n / 4);      // two buffers of the longest segment
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_fst_segments, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_fst_segments)");
-    }
-    k_fst_segments<<<(unsigned)(f.segs * batch), threads, smem, st>>>(f);
+    const int rc = af_smem_optin(k_fst_segments, smem, "k_fst_segments");
+    if (rc) return rc;
+    k_fst_segments<<<(unsigned)(f.segs * batch), af_cta_threads(n / 16, 256), smem, st>>>(f);
     AF_LAUNCH_CHECK("k_fst_segments");
 
     ExpandParams e;

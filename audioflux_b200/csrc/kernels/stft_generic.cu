@@ -10,9 +10,8 @@
 // with the real-FFT post-pass.  This is the general path; the MFCC configuration has its own
 // fused kernel (mfcc_fused.cu).  Frames longer than 16384 points (the reference accepts radix2Exp up to 30,
 // src/stft_algorithm.c:114-117) do not fit a CTA: they are gathered (window, padding) into a workspace, transformed by the
-// four-step kernels of the CWT path (kernels/cwt.cu, forward leg only) and written out by a mode-specific pass.
+// four-step forward legs of the CWT path (af_launch_fft_rows, kernels/cwt.cu) and written out by a mode-specific pass.
 #include <math.h>
-#include <string.h>
 #include "common.cuh"
 #include "stockham.cuh"
 
@@ -73,6 +72,8 @@ __global__ void k_stft_generic(StftParams p) {
     const int width = nc + 1;
     const long long row = (long long)clip * p.timeLength + frame;
     for (int k = threadIdx.x; k <= nc; k += blockDim.x) {
+        // (written out rather than through af_real_bin: with FMA contraction on, the helper's inlined form rounds the
+        // imaginary part differently here, and the STFT planes must not change)
         float2 zk = a[k == nc ? 0 : k], zp = a[k == 0 ? 0 : nc - k];
         float er = 0.5f * (zk.x + zp.x), ei = 0.5f * (zk.y - zp.y);
         float orr = 0.5f * (zk.y + zp.y), oi = -0.5f * (zk.x - zp.x);
@@ -191,77 +192,38 @@ extern "C" int af_launch_stft(const AfFrameSrc *src, int mode, float normValue, 
         AF_LAUNCH_CHECK("k_stft_n2");
         return AF_OK;
     }
-    int threads = p.nc / 4; if (threads < 32) threads = 32; if (threads > 1024) threads = 1024;
-    size_t smem = sizeof(float2) * 2 * (size_t)p.nc;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_stft_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_stft_generic)");
-    }
-    k_stft_generic<<<(unsigned)frames, threads, smem, st>>>(p);
+    const size_t smem = sizeof(float2) * 2 * (size_t)p.nc;
+    const int rc = af_smem_optin(k_stft_generic, smem, "k_stft_generic");
+    if (rc) return rc;
+    k_stft_generic<<<(unsigned)frames, af_cta_threads(p.nc / 4, 1024), smem, st>>>(p);
     AF_LAUNCH_CHECK("k_stft_generic");
     return AF_OK;
 }
 
-// frames of more than 16384 points: chunks of frames through a stream-ordered workspace (gathered frames + spectrum +
-// inter-leg buffer = 20 bytes per sample, <= 512 MB at a time)
+// frames of more than 16384 points: chunks of frames (af_fft_rows_chunk) through a stream-ordered workspace
 static int launch_stft_long(StftParams p, long long frames, cudaStream_t st) {
     const int n = p.n;
     int log2n = 0;
     while ((1 << log2n) < n) log2n++;
-    const size_t perFrame = (size_t)n * (sizeof(float) + 2 * sizeof(float2));
-    long long chunk = (long long)(((size_t)512 << 20) / perFrame);
-    if (chunk < 1) chunk = 1;
-    if (chunk > frames) chunk = frames;
+    const long long chunk = af_fft_rows_chunk(log2n, frames);
+    const size_t specBytes = af_fft_rows_workspace_bytes(log2n, (int)chunk);
     void *ws = nullptr;
-    cudaError_t e = cudaMallocAsync(&ws, perFrame * (size_t)chunk, st);
+    cudaError_t e = cudaMallocAsync(&ws, specBytes + sizeof(float) * (size_t)n * chunk, st);
     if (e != cudaSuccess) return af_cuda_check(e, "cudaMallocAsync(long-frame STFT workspace)");
-    float2 *spec = static_cast<float2 *>(ws);                              // [chunk][n] spectrum + [chunk][n] inter-leg buffer
-    float *dFrames = reinterpret_cast<float *>(spec + 2 * (size_t)chunk * n);
+    float2 *spec = static_cast<float2 *>(ws);
+    float *dFrames = reinterpret_cast<float *>(static_cast<char *>(ws) + specBytes);
     int rc = AF_OK;
     for (long long f0 = 0; f0 < frames && rc == AF_OK; f0 += chunk) {
         const int nf = (int)(frames - f0 < chunk ? frames - f0 : chunk);
         const long long cells = (long long)nf * n;
         k_frames_gather<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(p, f0, nf, dFrames);
         af_count_launch(1);
-        AfCwtArgs a;
-        memset(&a, 0, sizeof(a));
-        a.log2n = log2n; a.num = 1; a.batch = nf; a.padLength = 0; a.dataLength = n; a.forwardOnly = 1;
-        // (the workspace handed to the CWT launcher: spectrum first, its inter-leg slots right behind)
-        if ((rc = af_launch_cwt(&a, dFrames, spec, nullptr, nullptr, st))) break;
+        if ((rc = af_launch_fft_rows(dFrames, log2n, nf, spec, st))) break;
         const long long outCells = (long long)nf * (n / 2 + 1);
         k_long_post<<<(unsigned)((outCells + 255) / 256), 256, 0, st>>>(p, f0, nf, spec);
         af_count_launch(1);
-        if (cudaGetLastError() != cudaSuccess) rc = af_fail(AF_ERR_CUDA, "long-frame STFT launch failed");
+        if ((e = cudaGetLastError()) != cudaSuccess) rc = af_cuda_check(e, "long-frame STFT launch");
     }
     cudaFreeAsync(ws, st);
     return rc;
-}
-
-// ---- twiddle tables shared by the Stockham kernels (STFT general path, ISTFT) ----
-#include <mutex>
-#include <vector>
-const float2 *af_twiddle_table(int log2n) {
-    static std::mutex mu;
-    static float2 *cache[64][32];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || log2n < 1 || log2n > 24) return nullptr;
-    std::lock_guard<std::mutex> lock(mu);
-    if (cache[dev][log2n]) return cache[dev][log2n];
-    const size_t n = (size_t)1 << log2n;
-    std::vector<float2> h(2 * n + 1);
-    for (size_t j = 0; j < n; j++) {
-        const double a = -2.0 * M_PI * (double)j / (double)n;
-        h[j] = make_float2((float)cos(a), (float)sin(a));
-    }
-    for (size_t j = 0; j <= n; j++) {
-        const double a = -2.0 * M_PI * (double)j / (double)(2 * n);
-        h[n + j] = make_float2((float)cos(a), (float)sin(a));
-    }
-    float2 *d = nullptr;
-    if (cudaMalloc(&d, sizeof(float2) * h.size()) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    // (pageable source: wait for the DMA itself, the Stockham kernels run on non-blocking streams -- see af_dev_upload)
-    if (cudaMemcpy(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaStreamSynchronize(cudaStreamLegacy) != cudaSuccess) { cudaGetLastError(); cudaFree(d); return nullptr; }
-    cache[dev][log2n] = d;
-    return d;
 }

@@ -94,6 +94,49 @@ __device__ __forceinline__ void af_fft_inplace_dit(float2 *a, int nc, int log2nc
     }
 }
 
-// host side: cached device tables per (device, log2 n): [0, n) exp(-2 pi i j / n) and, behind it, [0, n] exp(-2 pi i j / (2n))
-// (the real-FFT post-pass twiddles of a 2n-point real transform packed into n complex points)
+// the one-buffer in-place passes replace the two Stockham buffers from 16384 points (2 x 128 KB) up
+static inline bool af_fft_inplace(int nc) { return nc > 8192; }
+
+// position of element j in the bit-reversed order that af_fft_inplace_dif leaves and af_fft_inplace_dit reads
+__device__ __forceinline__ int af_brev(int j, int log2nc) { return log2nc ? (int)(__brev((unsigned)j) >> (32 - log2nc)) : 0; }
+
+// ---- real sequences: an N-point real FFT as an nc = N/2-point complex FFT of z[j] = x[2j] + i x[2j+1] ----
+
+// W_N^k = exp(-2 pi i k / N), k <= nc: from the second half of af_twiddle_table(log2 nc), or evaluated without a table
+__device__ __forceinline__ float2 af_real_tw(const float2 *tw, int nc, int k) {
+    return tw ? __ldg(tw + nc + k) : af_twiddle(k, 2 * nc);
+}
+
+// post-pass: X[k] (k = 0 .. nc) from zk = Z[k mod nc], zp = Z[(nc - k) mod nc] of the packed transform Z and w = W_N^k,
+// X[k] = E[k] + W_N^k O[k]; X[0] and X[nc] are real
+__device__ __forceinline__ float2 af_real_post(float2 zk, float2 zp, float2 w, int k, int nc) {
+    const float er = 0.5f * (zk.x + zp.x), ei = 0.5f * (zk.y - zp.y);
+    const float orr = 0.5f * (zk.y + zp.y), oi = -0.5f * (zk.x - zp.x);
+    float xr = er + (w.x * orr - w.y * oi), xi = ei + (w.x * oi + w.y * orr);
+    if (k == 0 || k == nc) xi = 0.0f;
+    return make_float2(xr, xi);
+}
+
+// the post-pass over a packed transform Z in natural order (af_stockham)
+__device__ __forceinline__ float2 af_real_bin(const float2 *Z, float2 w, int k, int nc) {
+    return af_real_post(Z[k == nc ? 0 : k], Z[k == 0 ? 0 : nc - k], w, k, nc);
+}
+
+// pre-pass of the inverse, conjugated: packed point k of the inverse real transform of the Hermitian X, from pk = X[k],
+// pm = X[nc - k] and w = W_N^k: conj(E + i O), E = (pk + conj pm) / 2, O = (pk - conj pm) / 2 * conj(w)
+__device__ __forceinline__ float2 af_real_pre_conj(float2 pk, float2 pm, float2 w) {
+    const float er = 0.5f * (pk.x + pm.x), ei = 0.5f * (pk.y - pm.y);
+    const float dr = 0.5f * (pk.x - pm.x), di = 0.5f * (pk.y + pm.y);
+    const float orr = dr * w.x + di * w.y, oi = di * w.x - dr * w.y;
+    return make_float2(er - oi, -(ei + orr));
+}
+
+// value v at position k (0 .. N/2) of a real even N-sequence, in the float view f of a packed buffer
+__device__ __forceinline__ void af_put_even(float *f, int n, int k, float v) {
+    f[k] = v;
+    if (k > 0 && k < n / 2) f[n - k] = v;
+}
+
+// host side (stockham.cu): cached device tables per (device, log2 n): [0, n) exp(-2 pi i j / n) and, behind it,
+// [0, n] exp(-2 pi i j / (2n)) (the real-FFT twiddles of a 2n-point real transform packed into n complex points)
 const float2 *af_twiddle_table(int log2n);

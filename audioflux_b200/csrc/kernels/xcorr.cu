@@ -12,21 +12,18 @@
 //   3. af_fft_inplace_dit (natural order) and one more conjugation give r = IFFT_M(P), the reference's 1/M included;
 //   4. the 2n-1 lags in the reference's order, divided by the Coeff scale, and __vmax's first arg-max.
 // Longer rows (M = 2^15 .. 2^20): the zero-padded signals go through the CWT path's four-step forward legs
-// (AfCwtArgs.forwardOnly); k_xcorr_cross forms the Hermitian P and writes its Hartley sequence c = Re P + Im P; a second
+// (af_launch_fft_rows); k_xcorr_cross forms the Hermitian P and writes its Hartley sequence c = Re P + Im P; a second
 // forward pass gives C, and Re C[j] + Im C[j] = M r[j].  k_xcorr_finish writes the lags and per-segment arg-max
 // candidates, k_xcorr_argmax reduces them in a fixed order (no atomics).  The workspace belongs to the object and is kept
 // between calls.
 //
 // Sums of squares are float products summed in double in a fixed order, like __vsum's double accumulator.  The file is
 // compiled with -fmad=false (Makefile): the scale and the post-passes are rounded step by step.
-#include <string.h>
-
-#include "common.cuh"
+#include "block_reduce.cuh"
 #include "stockham.cuh"
 
 namespace {
 
-constexpr unsigned FULL = 0xffffffffu;
 constexpr int kMaxThreads = 1024;
 constexpr int kPadSegs = 32;            // long path: segments of a padded row (partial sums of squares per segment)
 constexpr int kFinishSegs = 128;        // long path: segments of an output row (arg-max candidates per segment)
@@ -40,62 +37,17 @@ struct XcParams {
     int n, M, nc, log2nc, coeff;
 };
 
-// (v, i) beats (w, j): i is a candidate and either j is none, v > w, or they tie and i comes first
-__device__ __forceinline__ bool beats(float v, int i, float w, int j) {
-    return i >= 0 && (j < 0 || v > w || (v == w && i < j));
-}
-
-// first index of the block's maximum over the candidates (i >= 0); -1 when there is none.  redv / redi: 32 each
-__device__ int block_argmax(float v, int i, float *redv, int *redi) {
-    for (int o = 16; o; o >>= 1) {
-        const float w = __shfl_xor_sync(FULL, v, o);
-        const int j = __shfl_xor_sync(FULL, i, o);
-        if (beats(w, j, v, i)) { v = w; i = j; }
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    __syncthreads();
-    if (lane == 0) { redv[warp] = v; redi[warp] = i; }
-    __syncthreads();
-    v = redv[0]; i = redi[0];
-    for (int k = 1; k < nw; k++)
-        if (beats(redv[k], redi[k], v, i)) { v = redv[k]; i = redi[k]; }
-    return i;
-}
-
-// block sum of a double in a fixed order (tree within each warp, then the warps in order); every thread gets it
-__device__ double block_sum(double v, double *red) {
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    __syncthreads();
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    v = red[0];
-    for (int k = 1; k < nw; k++) v += red[k];
-    return v;
-}
-
 // xcorrObj_xcorr's Coeff scale (:85-103): sqrtf of the product of the two float sums
 __device__ __forceinline__ float coeff_scale(double s1, double s2) {
     const float f1 = (float)s1, f2 = (float)s2;
     return sqrtf(f1 * f2);
 }
 
-__device__ __forceinline__ int brev(int k, int log2nc) { return log2nc ? (int)(__brev((unsigned)k) >> (32 - log2nc)) : 0; }
-
-__device__ __forceinline__ float2 w_m(const XcParams &p, int k) {       // exp(-2 pi i k / M), k <= nc
-    return p.tw ? __ldg(p.tw + p.nc + k) : af_twiddle(k, p.M);
-}
-
 // bin k (0 .. nc) of the M-point real FFT whose nc-point packed transform z is stored in bit-reversed order
 __device__ __forceinline__ float2 real_bin(const XcParams &p, const float2 *z, int k) {
     const int nc = p.nc;
-    const float2 zk = z[brev(k == nc ? 0 : k, p.log2nc)], zp = z[brev(k == 0 ? 0 : nc - k, p.log2nc)];
-    const float er = 0.5f * (zk.x + zp.x), ei = 0.5f * (zk.y - zp.y);
-    const float orr = 0.5f * (zk.y + zp.y), oi = -0.5f * (zk.x - zp.x);
-    const float2 w = w_m(p, k);
-    float xr = er + (w.x * orr - w.y * oi), xi = ei + (w.x * oi + w.y * orr);
-    if (k == 0 || k == nc) xi = 0.0f;
-    return make_float2(xr, xi);
+    const float2 zk = z[af_brev(k == nc ? 0 : k, p.log2nc)], zp = z[af_brev(k == 0 ? 0 : nc - k, p.log2nc)];
+    return af_real_post(zk, zp, af_real_tw(p.tw, nc, k), k, nc);
 }
 
 __device__ __forceinline__ float2 cross(const XcParams &p, const float2 *A, const float2 *B, int k) {
@@ -103,16 +55,6 @@ __device__ __forceinline__ float2 cross(const XcParams &p, const float2 *A, cons
     if (!p.b) return make_float2(x.x * x.x + x.y * x.y, 0.0f);
     const float2 y = real_bin(p, B, k);
     return make_float2(x.x * y.x + x.y * y.y, x.y * y.x - x.x * y.y);   // x conj(y)
-}
-
-// packed bin k of the inverse real transform, conjugated: conj(E + i O), E = (P[k] + conj P[nc-k]) / 2,
-// O = (P[k] - conj P[nc-k]) / 2 * exp(+2 pi i k / M)
-__device__ __forceinline__ float2 inv_pack_conj(const XcParams &p, float2 pk, float2 pm, int k) {
-    const float er = 0.5f * (pk.x + pm.x), ei = 0.5f * (pk.y - pm.y);
-    const float dr = 0.5f * (pk.x - pm.x), di = 0.5f * (pk.y + pm.y);
-    const float2 w = w_m(p, k);                                        // conj(w) = exp(+2 pi i k / M)
-    const float orr = dr * w.x + di * w.y, oi = di * w.x - dr * w.y;
-    return make_float2(er - oi, -(ei + orr));
 }
 
 // r[m] = IFFT_M(P)[m] from the natural-order DIT result y (r[2j] + i r[2j+1] = conj(y[j]) / nc)
@@ -150,10 +92,10 @@ __global__ void __launch_bounds__(kMaxThreads) k_xcorr(XcParams p) {
     for (int k = tid; k <= nc / 2; k += bd) {
         const int m = nc - k;
         const float2 pk = cross(p, A, B, k), pm = cross(p, A, B, m);
-        const float2 yk = inv_pack_conj(p, pk, pm, k);
-        const float2 ym = k > 0 && m != k ? inv_pack_conj(p, pm, pk, m) : yk;
-        A[brev(k, p.log2nc)] = yk;
-        if (k > 0 && m != k) A[brev(m, p.log2nc)] = ym;
+        const float2 yk = af_real_pre_conj(pk, pm, af_real_tw(p.tw, nc, k));
+        const float2 ym = k > 0 && m != k ? af_real_pre_conj(pm, pk, af_real_tw(p.tw, nc, m)) : yk;
+        A[af_brev(k, p.log2nc)] = yk;
+        if (k > 0 && m != k) A[af_brev(m, p.log2nc)] = ym;
     }
     __syncthreads();
     af_fft_inplace_dit(A, nc, p.log2nc, p.tw);
@@ -278,18 +220,13 @@ __global__ void __launch_bounds__(kFinishSegs) k_xcorr_argmax(const float *__res
 
 int launch_long(const AfXcorrArgs *a, int M, int log2M, cudaStream_t st) {
     const int autoc = a->b == nullptr, per = autoc ? 1 : 2;
-    AfCwtArgs cw;
-    memset(&cw, 0, sizeof(cw));
-    cw.log2n = log2M; cw.num = 1; cw.padLength = 0; cw.dataLength = M; cw.forwardOnly = 1;
-    // per pair: padded rows (per x M floats) and the CWT workspace (per x M spectra + inter-leg slots), candidates and sums
-    cw.batch = per;
-    const size_t perPair = (size_t)per * M * sizeof(float) + af_cwt_workspace_bytes(&cw) +
+    // per pair: padded rows (per x M floats), the long FFT's workspace (per x M spectra + inter-leg slots), candidates and sums
+    const size_t perPair = (size_t)per * M * sizeof(float) + af_fft_rows_workspace_bytes(log2M, per) +
                            (size_t)kFinishSegs * (sizeof(float) + sizeof(int)) + (size_t)per * kPadSegs * sizeof(double);
     int chunk = (int)(((size_t)512 << 20) / perPair);
     if (chunk < 1) chunk = 1;
     if (chunk > a->batch) chunk = a->batch;
-    cw.batch = per * chunk;
-    const size_t wsBytes = af_cwt_workspace_bytes(&cw);
+    const size_t wsBytes = af_fft_rows_workspace_bytes(log2M, per * chunk);
     const size_t rowsBytes = (size_t)per * chunk * M * sizeof(float);
     const size_t candBytes = (size_t)chunk * kFinishSegs * (sizeof(float) + sizeof(int));
     const size_t sumBytes = (size_t)per * chunk * kPadSegs * sizeof(double);
@@ -311,12 +248,10 @@ int launch_long(const AfXcorrArgs *a, int M, int log2M, cudaStream_t st) {
         const float *pa = a->a + (size_t)p0 * n, *pb = autoc ? nullptr : a->b + (size_t)p0 * n;
         k_xcorr_pad<<<dim3(kPadSegs, per * nb), kLongThreads, 0, st>>>(pa, pb, n, M, nb, rows, sums);
         af_count_launch(1);
-        cw.batch = per * nb;
-        if ((rc = af_launch_cwt(&cw, rows, ws, nullptr, nullptr, st))) break;
+        if ((rc = af_launch_fft_rows(rows, log2M, per * nb, ws, st))) break;
         k_xcorr_cross<<<dim3((unsigned)((M + kLongThreads - 1) / kLongThreads), nb), kLongThreads, 0, st>>>(ws, M, nb, autoc, rows);
         af_count_launch(1);
-        cw.batch = nb;
-        if ((rc = af_launch_cwt(&cw, rows, ws, nullptr, nullptr, st))) break;
+        if ((rc = af_launch_fft_rows(rows, log2M, nb, ws, st))) break;
         float *out = a->out + (size_t)p0 * L;
         k_xcorr_finish<<<dim3(kFinishSegs, nb), kLongThreads, 0, st>>>(ws, sums, n, M, nb, autoc, a->coeff, out, candV, candI);
         af_count_launch(1);
@@ -345,14 +280,10 @@ extern "C" int af_launch_xcorr(const AfXcorrArgs *a, void *stream) {
     p.n = a->n; p.M = M; p.nc = M / 2; p.log2nc = log2M - 1; p.coeff = a->coeff;
     p.tw = p.log2nc >= 1 ? af_twiddle_table(p.log2nc) : nullptr;
     if (p.log2nc >= 1 && !p.tw) return af_fail(AF_ERR_CUDA, "xcorr: twiddle table 2^%d", p.log2nc);
-    int threads = p.nc / 2;
-    threads = threads < 32 ? 32 : threads > kMaxThreads ? kMaxThreads : threads;
     const size_t smem = sizeof(float2) * 2 * (size_t)p.nc;
-    if (smem > 48 * 1024) {
-        const cudaError_t e = cudaFuncSetAttribute(k_xcorr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return af_cuda_check(e, "cudaFuncSetAttribute(k_xcorr)");
-    }
-    k_xcorr<<<(unsigned)a->batch, threads, smem, st>>>(p);
+    const int rc = af_smem_optin(k_xcorr, smem, "k_xcorr");
+    if (rc) return rc;
+    k_xcorr<<<(unsigned)a->batch, af_cta_threads(p.nc / 2, kMaxThreads), smem, st>>>(p);
     AF_LAUNCH_CHECK("k_xcorr");
     return AF_OK;
 }

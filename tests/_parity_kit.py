@@ -1,6 +1,6 @@
 """What the per-object parity suites share: the reference build, the golden files that stand in for it where it is not
-built, the check of an object's C API across the headers and libraries, the helpers of direct calls on the device, and
-the reference's own Python package bound to this library."""
+built, the check of an object's C API across the headers and libraries, the batched call with host or device pointers,
+the helpers of direct calls on the device, and the reference's own Python package bound to this library."""
 import ctypes as C
 import os
 import re
@@ -88,6 +88,34 @@ def dptr(t):
 def stream():
     import torch
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+class Out:
+    """an argument of run_batch: a plane the call writes or updates in place, starting as the numpy array a"""
+
+    def __init__(self, a):
+        self.a = a
+
+
+def run_batch(lib, name, args, device):
+    """lib.<name>(*args, memKind, stream), a *Batch entry point, with host pointers (memKind 0, no stream) or with
+    device pointers (memKind 1, the current stream).  Out(a) marks a plane the call writes; other numpy arrays are
+    inputs, passed by address or first copied to a CUDA tensor; None, scalars and ctypes objects pass through unchanged.
+    Asserts status 0, and synchronises after a call with device pointers.  -> the Out planes as numpy, in argument
+    order"""
+    planes = {k: np.ascontiguousarray(a.a if isinstance(a, Out) else a)
+              for k, a in enumerate(args) if isinstance(a, (Out, np.ndarray))}
+    if device:
+        import torch
+        planes = {k: torch.from_numpy(a).cuda() for k, a in planes.items()}
+        ptrs, tail = {k: dptr(t) for k, t in planes.items()}, (1, stream())
+    else:
+        ptrs, tail = {k: a.ctypes.data for k, a in planes.items()}, (0, None)
+    rc = getattr(lib, name)(*(ptrs.get(k, a) for k, a in enumerate(args)), *tail)
+    assert rc == 0, lib.afb200_lastError()
+    if device:
+        torch.cuda.synchronize()
+    return [planes[k].cpu().numpy() if device else planes[k] for k, a in enumerate(args) if isinstance(a, Out)]
 
 
 def count_launches(lib, fn, warm):

@@ -1,6 +1,7 @@
 """Writes the golden files of the per-object suites from the reference build: spectral.npz, nsgt.npz, st.npz,
-cepstrogram.npz, resample.npz and hpss.npz, each from the store (GOLD) of tests/test_<object>_cpu.py, so that their
-oracle tests run where no reference build exists.  Needs oracle/_ref (make -C oracle REF=<audioFlux tree>).
+cepstrogram.npz, resample.npz, hpss.npz, onset.npz, harmonic_ratio.npz, wavelet.npz, nmf.npz and dsp.npz, each from the
+store (GOLD) of tests/test_<object>_cpu.py, so that their oracle tests run where no reference build exists.  Needs
+oracle/_ref (make -C oracle REF=<audioFlux tree>).
 
     python tests/golden/make_golden_objects.py [--out DIR] [object ...]"""
 import argparse
@@ -14,7 +15,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
 from oracle import ref_lib as R  # noqa: E402
 
-OBJECTS = ("spectral", "nsgt", "st", "cepstrogram", "resample", "hpss")
+OBJECTS = ("spectral", "nsgt", "st", "cepstrogram", "resample", "hpss", "onset", "harmonic_ratio", "wavelet", "nmf", "dsp")
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])

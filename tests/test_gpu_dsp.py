@@ -4,43 +4,28 @@ the float64 oracle and the reference build (its stored outputs where it is not b
 length 2^1 .. 2^20 row by row, both sides of the switch to the long path; the batch bit-identical to the legacy call
 with host pointers across staging chunks and with device pointers back to back around a CZT table change; the CZT
 tables and the long Xcorr workspace ordered across streams (busy caller streams, the host-pointer pipeline's own
-stream, a second stream); every call as on a fresh object; one launch per chunk (plus one per CZT table change); the reference's own Xcorr and CZT classes on
-libaudioflux_b200.so; and the register / spill budget of the new kernels (compile only, no GPU needed)."""
+stream, a second stream); every call as on a fresh object; one launch per chunk (plus one per CZT table change); and the
+reference's own Xcorr and CZT classes on libaudioflux_b200.so."""
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 import warnings
 
 import numpy as np
 import pytest
 
 import _dsp_oracle as D
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
-from test_dsp_cpu import CZ, XC, _scale, check_xcorr
-from test_register_budgets import CSRC, _ptxas_entries, makefile_nvcc_line
+from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
+from test_dsp_cpu import CZ, GOLD, XC, _scale, check_xcorr
 
 import audioflux_b200 as af
 
 TOL = 1e-4                 # of max |want| of the row
 gpu = pytest.mark.gpu
-GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "dsp.npz")
 
 
 def _stored(name):
     """the reference's output of a case: live from the build, else from the golden file, else None"""
-    ref = ref_lib_or_none()
-    if ref is not None:
-        if name in XC:
-            v, mv, i = D.c_xcorr_case(ref, name, XC[name])
-            return v, mv, i
-        return D.c_czt_case(ref, name, CZ[name])
-    g = np.load(GOLDEN)
-    if name not in g.files:
-        return None
-    v = g[name]
-    return (v[:-2], v[-2], int(v[-1])) if name in XC else v
+    v = GOLD.outputs({name}).get(name)
+    return (v[:-2], v[-2], int(v[-1])) if v is not None and name in XC else v
 
 
 @gpu
@@ -105,27 +90,8 @@ def test_every_transform_length(product_lib, cuda_device):
 
 def _xcorr_batch_c(lib, o, a, b, norm, device):
     B, n = a.shape
-    L = 2 * n - 1
-    nt = C.byref(C.c_int(norm))
-    if device:
-        import torch
-        ad = torch.from_numpy(a).cuda()
-        bd = None if b is None else torch.from_numpy(b).cuda()
-        out = torch.full((B, L), 7.0, device="cuda")
-        mv = torch.full((B,), 7.0, device="cuda")
-        ix = torch.full((B,), 7, dtype=torch.int32, device="cuda")
-        rc = lib.xcorrObj_xcorrBatch(o, dptr(ad), None if bd is None else dptr(bd), n, B, nt, dptr(out), dptr(mv),
-                                     dptr(ix), 1, stream())
-        assert rc == 0, lib.afb200_lastError()
-        torch.cuda.synchronize()
-        return out.cpu().numpy(), mv.cpu().numpy(), ix.cpu().numpy()
-    out = np.full((B, L), 7.0, np.float32)
-    mv = np.full(B, 7.0, np.float32)
-    ix = np.full(B, 7, np.int32)
-    rc = lib.xcorrObj_xcorrBatch(o, a.ctypes.data, None if b is None else b.ctypes.data, n, B, nt, out.ctypes.data,
-                                 mv.ctypes.data, ix.ctypes.data, 0, None)
-    assert rc == 0, lib.afb200_lastError()
-    return out, mv, ix
+    outs = Out(np.full((B, 2 * n - 1), 7.0, np.float32)), Out(np.full(B, 7.0, np.float32)), Out(np.full(B, 7, np.int32))
+    return run_batch(lib, "xcorrObj_xcorrBatch", (o, a, b, n, B, C.byref(C.c_int(norm)), *outs), device)
 
 
 def _same_as_legacy(lib, res, a, b, norm, rows):
@@ -158,22 +124,11 @@ def test_xcorr_batch_equals_legacy(product_lib, cuda_device):
     product_lib.xcorrObj_free(o)
 
 
-def _czt_batch_c(lib, o, re, im, band, device):
+def _czt_batch_c(lib, o, re, im, band):
+    """cztObj_cztBatch with host pointers -> (real, imaginary) numpy [B, 2N]"""
     B, N = (re if re is not None else im).shape
-    if device:
-        import torch
-        rd = None if re is None else torch.from_numpy(re).cuda()
-        idd = None if im is None else torch.from_numpy(im).cuda()
-        o3 = [torch.full((B, 2 * N), 7.0, device="cuda") for _ in range(2)]
-        rc = lib.cztObj_cztBatch(o, None if rd is None else dptr(rd), None if idd is None else dptr(idd), B, *band,
-                                 dptr(o3[0]), dptr(o3[1]), 1, stream())
-        assert rc == 0, lib.afb200_lastError()
-        return o3, (rd, idd)
-    o3 = [np.full((B, 2 * N), 7.0, np.float32) for _ in range(2)]
-    rc = lib.cztObj_cztBatch(o, None if re is None else re.ctypes.data, None if im is None else im.ctypes.data, B, *band,
-                             o3[0].ctypes.data, o3[1].ctypes.data, 0, None)
-    assert rc == 0, lib.afb200_lastError()
-    return o3, None
+    return run_batch(lib, "cztObj_cztBatch", (o, re, im, B, *band, Out(np.full((B, 2 * N), 7.0, np.float32)),
+                                              Out(np.full((B, 2 * N), 7.0, np.float32))), False)
 
 
 @gpu
@@ -188,14 +143,19 @@ def test_czt_batch_equals_legacy(product_lib, cuda_device):
     re = rng.standard_normal((9000, N)).astype(np.float32)
     im = rng.standard_normal((9000, N)).astype(np.float32)
     band = (0.15, 0.25)
-    (hr, hi), _ = _czt_batch_c(product_lib, o, re, im, band, False)
+    hr, hi = _czt_batch_c(product_lib, o, re, im, band)
     for k in (0, 4095, 4096, 8191, 8192, 8999):
         want = D.c_czt(product_lib, leg, re[k], im[k], *band, N)
         assert np.array_equal(hr[k], want.real.astype(np.float32)) and np.array_equal(hi[k], want.imag.astype(np.float32)), k
     calls = []
     for band, (x, y) in (((0.0, 1.0), (re[:50], None)), ((0.01, 0.02), (None, im[:70])), ((0.3, 0.2), (re[:5], im[:5])),
                          ((0.0, 0.5), (re[:40], im[:40])), ((0.0, 1.0), (re[:3], None))):
-        o3, keep = _czt_batch_c(product_lib, o, x, y, band, True)
+        B = (x if x is not None else y).shape[0]
+        keep = [None if v is None else torch.from_numpy(v).cuda() for v in (x, y)]
+        o3 = [torch.full((B, 2 * N), 7.0, device="cuda") for _ in range(2)]
+        rc = product_lib.cztObj_cztBatch(o, *(None if t is None else dptr(t) for t in keep), B, *band, dptr(o3[0]),
+                                         dptr(o3[1]), 1, stream())
+        assert rc == 0, product_lib.afb200_lastError()
         calls.append((band, x, y, o3, keep))
     torch.cuda.synchronize()
     for band, x, y, o3, _ in calls:
@@ -236,13 +196,13 @@ def test_czt_tables_ordered_across_streams(product_lib, cuda_device):
     with torch.cuda.stream(s1):
         torch.cuda._sleep(200_000_000)
     dev(0, A, s1)                                          # first use + band A, behind the busy stream
-    (h1r, h1i), _ = _czt_batch_c(lib, o, x, None, A, False)   # same band, the pipeline's stream
+    h1r, h1i = _czt_batch_c(lib, o, x, None, A)            # same band, the pipeline's stream
     dev(1, A, s2)                                          # same band, a second stream
     with torch.cuda.stream(s2):
         torch.cuda._sleep(200_000_000)
     dev(2, A, s2)                                          # still reading band A long after ...
     dev(3, A, s1)                                          # ... this one, the last launch on the object
-    (h2r, h2i), _ = _czt_batch_c(lib, o, x, None, Bd, False)  # band B overwrites the tables
+    h2r, h2i = _czt_batch_c(lib, o, x, None, Bd)           # band B overwrites the tables
     torch.cuda.synchronize()
     for k in (0, B - 1):
         wa = D.c_czt(lib, leg, x[k], None, *A, N)
@@ -373,32 +333,3 @@ def test_reference_classes_on_b200(raf, cuda_device):
         warnings.simplefilter("ignore")
         assert np.array_equal(oc.czt(z[0, 0] + 1j * z[0, 1], 0.15, 0.25), g3)
 
-
-@pytest.mark.parametrize("source, kernels", (("xcorr.cu", ("k_xcorr_argmax", "k_xcorr_finish", "k_xcorr_cross",
-                                                           "k_xcorr_pad", "k_xcorr")),
-                                             ("czt.cu", ("k_czt_filter", "k_czt"))))
-def test_kernel_budget(source, kernels):
-    """the new kernels spill nothing, compiled with the Makefile's own nvcc line (-fmad=false), and the one-CTA-per-row
-    kernels fit 1024 threads"""
-    cmd = makefile_nvcc_line(source)
-    nvcc = shutil.which(cmd[0])
-    if nvcc is None:
-        pytest.skip(f"nvcc not found: {cmd[0]}")
-    cmd[0] = nvcc
-    assert "-fmad=false" in cmd
-    with tempfile.TemporaryDirectory() as tmp:
-        o = cmd.index("-o")
-        cmd[o + 1] = os.path.join(tmp, source + ".o")
-        r = subprocess.run(cmd + ["-Xptxas", "-v"], cwd=CSRC, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    seen = {}
-    for entry, figures in _ptxas_entries()(r.stderr).items():
-        for name in kernels:                               # longest names first: k_xcorr is a prefix of the others
-            if name + "E" in entry or name + "N" in entry:
-                assert name not in seen, entry
-                seen[name] = figures
-                break
-    assert set(seen) == set(kernels), r.stderr
-    for name, (regs, stack, st, ld) in seen.items():
-        assert st == 0 and ld == 0 and stack == 0, (name, regs, stack, st, ld)
-        assert regs <= 64, (name, regs)

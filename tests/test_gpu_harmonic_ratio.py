@@ -2,19 +2,13 @@
 reference build (within 1e-4 of max |value| of the clip, a frame whose crossing or arg-max the oracle finds undetermined
 equal to one of its candidates instead, and the count of such frames capped); the batch bit-identical to the legacy
 call with host pointers across staging chunks, with device pointers back to back, and for clips whose carry starts at
-frame 0; two launches per chunk; the refusals; the reference's own HarmonicRatio class on libaudioflux_b200.so; and the
-register / spill budget of both kernels (compile only, no GPU needed)."""
-import os
-import shutil
-import subprocess
-import tempfile
-
+frame 0; two launches per chunk; the refusals; and the reference's own HarmonicRatio class on libaudioflux_b200.so."""
 import numpy as np
 import pytest
 
 import _harmonic_ratio_oracle as HO
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
-from test_register_budgets import CSRC, _ptxas_entries, makefile_nvcc_line
+from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
+from test_harmonic_ratio_cpu import GOLD
 
 import audioflux_b200 as af
 
@@ -24,11 +18,8 @@ gpu = pytest.mark.gpu
 UNDETERMINED = []          # (case, frames) decided by a candidate, reported at the end
 
 
-def _reference(name, kw):
-    ref = ref_lib_or_none()
-    if ref is not None:
-        return HO.c_case(ref, name, kw)
-    return np.load(os.path.join(os.path.dirname(__file__), "golden", "harmonic_ratio.npz"))[name]
+def _reference(name):
+    return GOLD.outputs({name})[name]
 
 
 def _check(got, want, cands, what):
@@ -46,7 +37,7 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     assert product_lib.afb200_lastError() in (b"", None)
     want, cands, _ = HO.oracle_case(name, kw)
     alt = _check(got, want, cands, (name, "oracle"))
-    ref = _reference(name, kw)
+    ref = _reference(name)
     assert got.shape == ref.shape
     scale = max(np.abs(ref).max(initial=0.0), 1e-30)
     far = np.flatnonzero(~(np.abs(got - ref) <= TOL * scale))
@@ -73,19 +64,8 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
 def _batch(lib, o, x, device, fill=7.0):
     b, n = x.shape
     T = lib.harmonicRatioObj_calTimeLength(o, n)
-    if device:
-        import torch
-        xd = torch.from_numpy(np.ascontiguousarray(x)).cuda()
-        v = torch.full((b, T), fill, device="cuda")
-        rc = lib.harmonicRatioObj_harmonicRatioBatch(o, dptr(xd), n, b, dptr(v), 1, stream())
-        assert rc == 0, lib.afb200_lastError()
-        torch.cuda.synchronize()
-        return v.cpu().numpy()
-    x = np.ascontiguousarray(x, np.float32)
-    v = np.full((b, T), fill, np.float32)
-    rc = lib.harmonicRatioObj_harmonicRatioBatch(o, x.ctypes.data, n, b, v.ctypes.data, 0, None)
-    assert rc == 0, lib.afb200_lastError()
-    return v
+    return run_batch(lib, "harmonicRatioObj_harmonicRatioBatch",
+                     (o, np.ascontiguousarray(x, np.float32), n, b, Out(np.full((b, T), fill, np.float32))), device)[0]
 
 
 def _clips(n, length, seed, dc_every=3):
@@ -192,29 +172,3 @@ def test_report_undetermined():
     print(f"harmonic ratio: {total} frame(s) decided by an oracle candidate: {UNDETERMINED}")
     assert total <= 20
 
-
-def test_kernel_budget():
-    """k_harmonic_ratio and k_harmonic_ratio_carry spill nothing, compiled with the Makefile's own nvcc line"""
-    cmd = makefile_nvcc_line("harmonic_ratio.cu")
-    nvcc = shutil.which(cmd[0])
-    if nvcc is None:
-        pytest.skip(f"nvcc not found: {cmd[0]}")
-    cmd[0] = nvcc
-    assert "-fmad=false" in cmd
-    with tempfile.TemporaryDirectory() as tmp:
-        o = cmd.index("-o")
-        cmd[o + 1] = os.path.join(tmp, "harmonic_ratio.cu.o")
-        r = subprocess.run(cmd + ["-Xptxas", "-v"], cwd=CSRC, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    seen = {}
-    for entry, figures in _ptxas_entries()(r.stderr).items():
-        for name in ("k_harmonic_ratio_carry", "k_harmonic_ratio"):
-            if name + "E" in entry or name + "N" in entry:
-                assert name not in seen, entry
-                seen[name] = figures
-                break
-    assert set(seen) == {"k_harmonic_ratio", "k_harmonic_ratio_carry"}, r.stderr
-    for name, (regs, stack, st, ld) in seen.items():
-        assert st == 0 and ld == 0 and stack == 0, (name, regs, stack, st, ld)
-        assert regs <= 64, (name, regs)                  # 1024 threads per CTA
-    assert seen["k_harmonic_ratio"][0] <= 32             # two CTAs of 1024 threads per SM

@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 
 import _hpss_oracle as HO
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
+from _parity_kit import Out, count_launches, dptr, ref_lib_or_none, run_batch, stream
+from _parity_kit import raf  # noqa: F401  (a fixture)
 
 import audioflux_b200 as af
 
@@ -27,18 +28,9 @@ def _batch(lib, o, x, device, outputs="hp"):
     x = np.ascontiguousarray(x, np.float32)
     b, n = x.shape
     m = lib.hpssObj_calDataLength(o, n)
-    if device:
-        import torch
-        xd = torch.from_numpy(x).cuda()
-        outs = [torch.full((b, m), 7.0, device="cuda") if c in outputs else None for c in "hp"]
-        ptrs = [None if t is None else dptr(t) for t in outs]
-        assert lib.hpssObj_hpssBatch(o, dptr(xd), n, b, *ptrs, 1, stream()) == 0, lib.afb200_lastError()
-        torch.cuda.synchronize()
-        return [None if t is None else t.cpu().numpy() for t in outs]
-    outs = [np.full((b, m), 7.0, np.float32) if c in outputs else None for c in "hp"]
-    ptrs = [None if a is None else a.ctypes.data for a in outs]
-    assert lib.hpssObj_hpssBatch(o, x.ctypes.data, n, b, *ptrs, 0, None) == 0, lib.afb200_lastError()
-    return outs
+    planes = [Out(np.full((b, m), 7.0, np.float32)) if c in outputs else None for c in "hp"]
+    got = iter(run_batch(lib, "hpssObj_hpssBatch", (o, x, n, b, *planes), device))
+    return [None if p is None else next(got) for p in planes]
 
 
 def _legacy(lib, o, x, outputs="hp"):

@@ -1,22 +1,16 @@
 """NMF on the GPU: every oracle case through nmf / nmfBatch against the oracle and the reference build (W and H within
 1e-4 of their max, the iteration counts equal modulo an undetermined stop); the batch bit-identical to per-matrix nmf
 calls, matrices that stop at different iterations included, with host pointers across staging chunks and with device
-pointers; the launch count independent of the batch; the reference's own audioflux nmf on libaudioflux_b200.so; and the
-register / spill budget of the four kernels (compile only, no GPU needed)."""
+pointers; the launch count independent of the batch; and the reference's own audioflux nmf on libaudioflux_b200.so."""
 import ctypes as C
 import importlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import _nmf_oracle as NO
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
-from test_nmf_cpu import TOL, check_against
-from test_register_budgets import CSRC, _ptxas_entries, makefile_nvcc_line
+from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
+from test_nmf_cpu import GOLD, TOL, check_against
 
 import audioflux_b200 as af
 
@@ -24,12 +18,8 @@ CASES = dict(NO.cases())
 gpu = pytest.mark.gpu
 
 
-def _reference(name, kw):
-    ref = ref_lib_or_none()
-    if ref is not None:
-        W, H = NO.c_nmf(ref, kw)
-        return W, H, NO.c_iters(ref, kw, W, H, NO.oracle_case(kw)[2])
-    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "nmf.npz"))
+def _reference(name):
+    g = GOLD.outputs({f"{name}/{a}" for a in ("W", "H", "iters")})
     return g[f"{name}/W"], g[f"{name}/H"], int(g[f"{name}/iters"])
 
 
@@ -38,20 +28,9 @@ def _batch(lib, V, k, kw, device, W=None, H=None):
     b, n, m = V.shape
     W = np.broadcast_to(np.arange(1, n * k + 1, dtype=np.float32).reshape(n, k), (b, n, k)).copy() if W is None else W
     H = np.broadcast_to(np.arange(1, k * m + 1, dtype=np.float32).reshape(k, m), (b, k, m)).copy() if H is None else H
-    it = np.full(b, -7, np.int32)
-    args = (NO._opt(C.c_int, kw["max_iter"]), NO._opt(C.c_int, kw["tp"]), NO._opt(C.c_float, kw["thresh"]),
-            NO._opt(C.c_int, kw["norm"]))
-    if device:
-        import torch
-        t = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in (V, W, H, it)]
-        rc = lib.nmfBatch(dptr(t[0]), b, n, m, k, dptr(t[1]), dptr(t[2]), *args, dptr(t[3]), 1, stream())
-        torch.cuda.synchronize()
-        W, H, it = (x.cpu().numpy() for x in t[1:])
-    else:
-        V = np.ascontiguousarray(V)
-        rc = lib.nmfBatch(V.ctypes.data, b, n, m, k, W.ctypes.data, H.ctypes.data, *args, it.ctypes.data, 0, None)
-    assert rc == 0, lib.afb200_lastError()
-    return W, H, it
+    return run_batch(lib, "nmfBatch", (V, b, n, m, k, Out(W), Out(H), NO._opt(C.c_int, kw["max_iter"]),
+                                       NO._opt(C.c_int, kw["tp"]), NO._opt(C.c_float, kw["thresh"]),
+                                       NO._opt(C.c_int, kw["norm"]), Out(np.full(b, -7, np.int32))), device)
 
 
 @gpu
@@ -65,7 +44,7 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     assert np.array_equal(Wb[0], W) and np.array_equal(Hb[0], H)
     iters = int(it[0])
     check_against(kw, W, H, iters, (name, "oracle"))
-    Wr, Hr, ir = _reference(name, kw)
+    Wr, Hr, ir = _reference(name)
     _, _, _, stat = NO.oracle_case(kw, stop=False)
     assert NO.counts_agree(iters, ir, stat, NO.resolved(kw)["thresh"]), (name, iters, ir)
     if iters == ir:
@@ -183,27 +162,3 @@ def test_stop_counts_match_oracle(product_lib, cuda_device):
     print(f"nmf: cases whose count differs from the oracle's by an undetermined stop: {differ}")
     assert len(differ) <= 2, differ
 
-
-def test_kernel_budget():
-    """the four NMF kernels spill nothing and fit at least two 256-thread CTAs per SM, compiled with the Makefile's own
-    nvcc line"""
-    cmd = makefile_nvcc_line("nmf.cu")
-    nvcc = shutil.which(cmd[0])
-    if nvcc is None:
-        pytest.skip(f"nvcc not found: {cmd[0]}")
-    cmd[0] = nvcc
-    assert "-fmad=false" in cmd
-    with tempfile.TemporaryDirectory() as tmp:
-        o = cmd.index("-o")
-        cmd[o + 1] = os.path.join(tmp, "nmf.cu.o")
-        r = subprocess.run(cmd + ["-Xptxas", "-v"], cwd=CSRC, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    seen = {}
-    for entry, figures in _ptxas_entries()(r.stderr).items():
-        for name in ("k_nmf_d", "k_nmf_h", "k_nmf_w", "k_nmf_norm"):
-            if name + "E" in entry:
-                seen[name] = figures
-    assert set(seen) == {"k_nmf_d", "k_nmf_h", "k_nmf_w", "k_nmf_norm"}, r.stderr
-    for name, (regs, stack, st, ld) in seen.items():
-        assert st == 0 and ld == 0 and stack == 0, (name, regs, stack, st, ld)
-        assert regs <= 96, (name, regs)                  # 256-thread CTAs: two per SM at least

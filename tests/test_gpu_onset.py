@@ -1,19 +1,16 @@
 """Onset detection on the GPU: every oracle case through onsetObj_onset against the numpy oracle and the reference build
 (novelty curve within 1e-4, the peak picking exact on the GPU's own curve, the points equal to the reference's up to
 named near-ties); the batch bit-identical to the legacy call with host and device pointers and across staging chunks;
-device calls queued back to back; the launch count; one clip of 100 000 frames; the reference's own Onset class running
-on libaudioflux_b200.so; and the register / spill budget of the two onset kernels (compile only, no GPU needed)."""
-import os
-import shutil
-import subprocess
-import tempfile
+device calls queued back to back; the launch count; one clip of 100 000 frames; and the reference's own Onset class
+running on libaudioflux_b200.so."""
+import ctypes as C
 
 import numpy as np
 import pytest
 
 import _onset_oracle as OO
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
-from test_register_budgets import CSRC, _ptxas_entries, makefile_nvcc_line
+from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
+from test_onset_cpu import GOLD
 
 import audioflux_b200 as af
 
@@ -27,41 +24,22 @@ def _check_points(evn, pts, evn_b, pts_b, pp, what):
     assert ok, (what, "decisions differ away from a near-tie at frames", diff)
 
 
-def _reference(name, kw):
+def _reference(name):
     """the reference build's (evn, points) of a case, from the golden file where the build is missing"""
-    ref = ref_lib_or_none()
-    if ref is not None:
-        return OO.c_case(ref, name, kw)
-    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "onset.npz"))
-    return g[f"{name}__evn"], g[f"{name}__pts"]
+    out = GOLD.outputs({f"{name}__evn", f"{name}__pts"})
+    return out[f"{name}__evn"], out[f"{name}__pts"]
 
 
 def _batch(lib, o, x, ph, prm, idx, device):
     """onsetObj_onsetBatch on x [batch, T, M] -> numpy (evn, points, counts)"""
-    import ctypes as C
     b, T, _ = x.shape
     par = None if prm is None else OO.NoveltyParam(*prm)
-    pa = None if par is None else C.addressof(par)
-    ia, il = (None, 0) if idx is None else (idx.ctypes.data, len(idx))
-    if device:
-        import torch
-        xd = torch.from_numpy(np.ascontiguousarray(x)).cuda()
-        pd = None if ph is None else torch.from_numpy(np.ascontiguousarray(ph)).cuda()
-        e = torch.full((b, T), 7.0, device="cuda")
-        p = torch.full((b, T), 7, dtype=torch.int32, device="cuda")
-        c = torch.full((b,), 7, dtype=torch.int32, device="cuda")
-        rc = lib.onsetObj_onsetBatch(o, dptr(xd), None if pd is None else dptr(pd), b, pa, ia, il, dptr(e), dptr(p),
-                                     dptr(c), 1, stream())
-        assert rc == 0, lib.afb200_lastError()
-        torch.cuda.synchronize()
-        return e.cpu().numpy(), p.cpu().numpy(), c.cpu().numpy()
-    x = np.ascontiguousarray(x, np.float32)
     ph = None if ph is None else np.ascontiguousarray(ph, np.float32)
-    e, p, c = np.full((b, T), 7, np.float32), np.full((b, T), 7, np.int32), np.full(b, 7, np.int32)
-    rc = lib.onsetObj_onsetBatch(o, x.ctypes.data, None if ph is None else ph.ctypes.data, b, pa, ia, il, e.ctypes.data,
-                                 p.ctypes.data, c.ctypes.data, 0, None)
-    assert rc == 0, lib.afb200_lastError()
-    return e, p, c
+    return run_batch(lib, "onsetObj_onsetBatch",
+                     (o, np.ascontiguousarray(x, np.float32), ph, b, None if par is None else C.addressof(par),
+                      None if idx is None else idx.ctypes.data, 0 if idx is None else len(idx),
+                      Out(np.full((b, T), 7, np.float32)), Out(np.full((b, T), 7, np.int32)),
+                      Out(np.full(b, 7, np.int32))), device)
 
 
 def _legacy(lib, o, x, ph, prm, idx):
@@ -80,7 +58,7 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     # the pick stage exactly: the oracle's peak picking on the GPU's own curve
     assert np.array_equal(OO.pick(evn, pp), pts), name
     want_evn, want_pts = OO.oracle_case(name, kw)
-    ref_evn, ref_pts = _reference(name, kw)
+    ref_evn, ref_pts = _reference(name)
     assert np.abs(evn.astype(np.float64) - want_evn).max() <= TOL, name
     assert np.abs(evn.astype(np.float64) - ref_evn).max() <= TOL, name
     _check_points(evn, pts, want_evn, want_pts, pp, (name, "oracle"))
@@ -136,7 +114,6 @@ def test_batch_across_chunks(product_lib, cuda_device):
 @gpu
 def test_device_calls_back_to_back(product_lib, cuda_device):
     """calls with different bin lists, parameters and clip counts queued on one object without a synchronise"""
-    import ctypes as C
     import torch
     T, M = 200, 96
     st, o = OO.c_new(product_lib, T, M, 256, 22050, 2, 0)
@@ -263,25 +240,3 @@ def _power_to_db(p, min_db=-80.0):
         v = (np.float32(10) * np.log10((p / p.max()).astype(np.float32))).astype(np.float32)
     return np.maximum(v, np.float32(min_db)).astype(np.float32)
 
-
-def test_kernel_budget():
-    """k_onset_maxfilter and k_onset_pick spill nothing, compiled with the Makefile's own nvcc line"""
-    cmd = makefile_nvcc_line("onset.cu")
-    nvcc = shutil.which(cmd[0])
-    if nvcc is None:
-        pytest.skip(f"nvcc not found: {cmd[0]}")
-    cmd[0] = nvcc
-    with tempfile.TemporaryDirectory() as tmp:
-        o = cmd.index("-o")
-        cmd[o + 1] = os.path.join(tmp, "onset.cu.o")
-        r = subprocess.run(cmd + ["-Xptxas", "-v"], cwd=CSRC, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    seen = {}
-    for entry, figures in _ptxas_entries()(r.stderr).items():
-        for name in ("k_onset_maxfilter", "k_onset_pick"):
-            if name in entry:
-                assert name not in seen, entry
-                seen[name] = figures
-    assert set(seen) == {"k_onset_maxfilter", "k_onset_pick"}, r.stderr
-    for name, (regs, stack, st, ld) in seen.items():
-        assert st == 0 and ld == 0 and stack == 0, (name, regs, stack, st, ld)

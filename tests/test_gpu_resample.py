@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 
 import _resample_oracle as RO
-from _parity_kit import count_launches, dptr, raf, ref_lib_or_none, stream  # noqa: F401  (raf: a fixture)
+from _parity_kit import Out, count_launches, dptr, ref_lib_or_none, run_batch, stream
+from _parity_kit import raf  # noqa: F401  (a fixture)
 
 import audioflux_b200 as af
 
@@ -28,16 +29,7 @@ def _batch(lib, o, x, device):
     x = np.ascontiguousarray(x, np.float32)
     b, n = x.shape
     m = lib.resampleObj_calDataLength(o, n)
-    if device:
-        import torch
-        xd = torch.from_numpy(x).cuda()
-        out = torch.full((b, m), 7.0, device="cuda")
-        assert lib.resampleObj_resampleBatch(o, dptr(xd), n, b, dptr(out), 1, stream()) == 0, lib.afb200_lastError()
-        torch.cuda.synchronize()
-        return out.cpu().numpy()
-    out = np.full((b, m), 7.0, np.float32)
-    assert lib.resampleObj_resampleBatch(o, x.ctypes.data, n, b, out.ctypes.data, 0, None) == 0, lib.afb200_lastError()
-    return out
+    return run_batch(lib, "resampleObj_resampleBatch", (o, x, n, b, Out(np.full((b, m), 7.0, np.float32))), device)[0]
 
 
 def _legacy_rows(lib, o, x):

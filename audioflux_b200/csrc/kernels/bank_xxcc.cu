@@ -272,12 +272,23 @@ extern "C" int af_launch_copy_cols(const float *in, int rows, int width, int lo,
     return AF_OK;
 }
 
+// warps (rows) per CTA of the warp-per-row cepstral kernels: `most` while they fit the default 48 KB of shared memory,
+// else as many as fit the 227 KB opt-in; 0 when one row does not fit.  Each row is computed by its own warp in the same
+// order whatever the CTA size, so the size only changes how many rows share an SM.
+static int xxcc_warps(size_t perWarp, int most) {
+    if (perWarp * most <= 48 * 1024) return most;
+    const size_t fit = (size_t)227 * 1024 / perWarp;
+    return fit < (size_t)most ? (int)fit : most;
+}
+
 extern "C" int af_launch_xxcc(const float *in, int rows, int num, int ccNum, int rectifyType, const float *dctT,
                               float *out, void *stream) {
     if (rows <= 0) return AF_OK;
-    const int warps = 8;
-    size_t smem = sizeof(float) * (size_t)warps * num;
-    if (smem > 48 * 1024) return af_fail(AF_ERR_UNSUPPORTED, "xxcc: num=%d too large", num);
+    const int warps = xxcc_warps(sizeof(float) * (size_t)num, 8);
+    if (!warps) return af_fail(AF_ERR_UNSUPPORTED, "xxcc: num=%d too large (one row must fit 227 KB of shared memory)", num);
+    const size_t smem = sizeof(float) * (size_t)warps * num;
+    const int rc = af_smem_optin(k_xxcc, smem, "k_xxcc");
+    if (rc) return rc;
     k_xxcc<<<(unsigned)((rows + warps - 1) / warps), warps * 32, smem, (cudaStream_t)stream>>>(
         in, rows, num, ccNum, rectifyType, dctT, num, out);
     AF_LAUNCH_CHECK("k_xxcc");
@@ -288,9 +299,12 @@ extern "C" int af_launch_xxcc_standard(const float *in, const float *energy, int
                                        int rectifyType, int energyType, int order, const float *dctT,
                                        float *coe, float *d1, float *d2, void *stream) {
     if (rows <= 0) return AF_OK;
-    const int warps = 4;
-    size_t smem = sizeof(float) * (size_t)warps * (num + 2 * (num + 1));
-    if (smem > 48 * 1024) return af_fail(AF_ERR_UNSUPPORTED, "xxccStandard: num=%d too large", num);
+    const size_t perWarp = sizeof(float) * ((size_t)num + 2 * ((size_t)num + 1));
+    const int warps = xxcc_warps(perWarp, 4);
+    if (!warps) return af_fail(AF_ERR_UNSUPPORTED, "xxccStandard: num=%d too large (one row must fit 227 KB of shared memory)", num);
+    const size_t smem = perWarp * warps;
+    const int rc = af_smem_optin(k_xxcc_standard, smem, "k_xxcc_standard");
+    if (rc) return rc;
     k_xxcc_standard<<<(unsigned)((rows + warps - 1) / warps), warps * 32, smem, (cudaStream_t)stream>>>(
         in, energy, rows, num, ccNum, rectifyType, energyType, order, dctT, num, coe, d1, d2);
     AF_LAUNCH_CHECK("k_xxcc_standard");

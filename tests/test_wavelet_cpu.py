@@ -2,6 +2,7 @@
 against the reference's dwt_filterCoef for every supported combination; the refusals of every other listed one; the
 float64 oracle against the reference build (or its stored outputs in tests/golden/wavelet.npz) over every family,
 radix2Exp 2 .. 16 and num 1 .. radix2Exp-1; the modulo indexing the kernels use against the literal padding; the
+vectorised level steps and mDataArr index map of the level-by-level GPU suite against the literal oracle; the
 constructor statuses against the reference; and the symbols of the three headers."""
 import os
 import re
@@ -132,19 +133,110 @@ def test_golden_file_is_current():
     GOLD.check_file()
 
 
+LEVEL_CASES = W.level_cases(TABLE)
+
+
+def _swt_level_pairs():
+    """(n, dec * 2^i) of every SWT level the level-by-level GPU suite runs"""
+    return {(n, len(TABLE[key][0]) << i) for kind, num, n, key, _ in LEVEL_CASES.values() if kind == "swt"
+            for i in range(num)}
+
+
 def test_modulo_indexing_equals_literal_padding():
     """padded[m] = x[(m - f/2) mod L] for every length and filter length the objects produce: DWT / WPT levels
-    (L = 2^k >= 4 against every filter length) and SWT levels (any L, f = dec * 2^i up to past 8 L)"""
+    (L = 2^k >= 4 against every filter length), SWT levels (any L, f = dec * 2^i up to past 8 L), and every SWT level
+    of the level-by-level GPU suite, where f reaches 30 L"""
     decs = sorted({len(v[0]) for v in TABLE.values()})
     pairs = [(1 << k, d) for k in range(2, 17) for d in decs]
     pairs += [(n, d << i) for n in range(1, 300) for d in decs for i in range(12) if (d << i) <= 8 * n + 80]
+    levels = _swt_level_pairs()
+    assert max(f / n for n, f in levels) == 30 and sum(f > 8 * n + 80 for n, f in levels) >= 20
     short = 0
-    for n, f in pairs:
+    for n, f in pairs + sorted(levels):
         x = np.arange(n, dtype=np.float64) + 1
         lit = W.period_padding(x, f)
         assert lit.shape == (n + f,) and np.array_equal(lit, W.modulo_padding(x, f)), (n, f)
         short += n < f // 2
     assert short > 1000
+
+
+def test_level_case_coverage():
+    """what the level-by-level GPU suite claims to run"""
+    by = lambda kind: [c for c in LEVEL_CASES.values() if c[0] == kind]  # noqa: E731
+    for kind in KINDS:
+        assert {c[3] for c in by(kind)} == set(TABLE), kind
+    dwt, wpt, swt = by("dwt"), by("wpt"), by("swt")
+    assert {(e, num) for _, num, e, *_ in dwt} >= {(e, e - 1) for e in range(2, 21)}
+    assert all(len({c[3] for c in dwt if c[2] == e}) >= 2 for e in range(2, 21))
+    assert any(len(TABLE[key][0]) == 60 for _, num, e, key, _ in dwt if num == e - 1 and e >= 10)    # 15 wraps at L = 4
+    assert {(e, num) for _, num, e, *_ in wpt} >= {(e, num) for e in range(2, 15) for num in range(1, e)}
+    assert {(e, num, m) for _, num, e, _, m in wpt if e >= 18} == {(e, num, False) for e in (18, 19, 20)
+                                                                  for num in (3, e - 1)}
+    assert max(len(TABLE[key][0]) * (1 << num - 1) // 2 / n for _, num, n, key, _ in swt) == 15  # dec s/2 / n
+    assert {n // (1 << num) for _, num, n, *_ in swt} >= {1, 3, 5} and max(c[1] for c in swt) == 12
+    assert ("swt", 10, 1 << 20) in {c[:3] for c in swt}
+    for kind, num, size, key, m_data in dwt + wpt:
+        rows = num if kind == "dwt" else 1 << num
+        assert m_data == (4 * rows * (4 << size) <= W.M_DATA_BYTES and not (kind == "wpt" and size >= 18))
+
+
+def _small_level_cases():
+    """the level suite's DWT / WPT cases up to 2^10 and SWT cases up to 1280 samples, and every filter at num 1 .. 3"""
+    out = [c[:4] for c in LEVEL_CASES.values() if c[2] <= (10 if c[0] != "swt" else 1280)]
+    out += [(kind, num, 6 if kind != "swt" else 96, key) for kind in KINDS for num in (1, 2, 3) for key in TABLE]
+    return out
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_vectorised_oracle_matches_literal(kind):
+    """level(), wpt_level() and swt_level(), gathers over the unpadded input as the kernels read it, chained level by
+    level, equal the literal oracle (padding, convolution, decimation, WPT's _node order and swap) within float64
+    rounding, for every small case of the level suite"""
+    cases = [c for c in _small_level_cases() if c[0] == kind]
+    assert len(cases) >= 100
+    for _, num, size, key in cases:
+        lo, hi = (v.astype(np.float64) for v in TABLE[key])
+        n = size if kind == "swt" else 1 << size
+        x = W.level_clips(n, size)
+        for clip in x:
+            if kind == "swt":
+                want, got = np.stack(W.swt(clip, num, lo, hi)), np.stack(W.swt_fast(clip, num, lo, hi))
+            else:
+                want = getattr(W, kind)(clip, num, lo, hi, m_data=False)[0]
+                got = getattr(W, f"{kind}_fast")(clip, num, lo, hi)
+            assert got.shape == want.shape
+            assert np.abs(got - want).max() <= 1e-12 * max(np.abs(want).max(), 1.0), (kind, num, size, key)
+        batched = getattr(W, f"{kind}_fast")(x, num, lo, hi)            # leading axes: the four clips at once
+        single = [getattr(W, f"{kind}_fast")(c, num, lo, hi) for c in x]
+        if kind == "swt":
+            batched, single = np.stack(batched, 1), np.stack([np.stack(s) for s in single])
+        assert np.array_equal(batched, single)
+
+
+def test_level_scales():
+    """the scales level() and swt_level() return are the steps applied to |h| and |x|"""
+    rng = np.random.default_rng(1)
+    lo, hi = (v.astype(np.float64) for v in TABLE[W.DB30])
+    x = rng.standard_normal((3, 64))
+    a, d, sa, sd = W.level(x, lo, hi)
+    assert np.array_equal(sa, W.level(np.abs(x), np.abs(lo), np.abs(hi))[0])
+    assert np.array_equal(sd, W.level(np.abs(x), np.abs(lo), np.abs(hi))[1])
+    a, d, sa, sd = W.swt_level(x, 8, lo, hi)
+    assert np.array_equal(sa, W.swt_level(np.abs(x), 8, np.abs(lo), np.abs(hi))[0])
+    assert (sa >= np.abs(a)).all() and (sd >= np.abs(d)).all()
+
+
+@pytest.mark.parametrize("kind", ["dwt", "wpt"])
+def test_m_data_index_matches_literal_loops(kind):
+    """m_data_index(), the vectorised map the GPU suite checks mDataArr through, equals the literal loops of the
+    reference's mData layout, for every radix2Exp 2 .. 10 and num 1 .. radix2Exp - 1"""
+    lo, hi = (v.astype(np.float64) for v in TABLE[W.SYM4])
+    for e in range(2, 11):
+        x = np.random.default_rng(e).standard_normal(1 << e)
+        for num in range(1, e):
+            coef, m = getattr(W, kind)(x, num, lo, hi)
+            idx = W.m_data_index(1 << e, num, kind)
+            assert idx.shape == m.shape and np.array_equal(coef[idx], m), (e, num)
 
 
 @pytest.mark.parametrize("kind", KINDS)

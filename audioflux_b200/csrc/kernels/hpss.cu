@@ -155,8 +155,10 @@ static size_t hpss_smem_bytes(int hOrder, int pOrder) {
 extern "C" int af_launch_hpss_mask(const AfHpssArgs *a, void *stream) {
     if (a->clips <= 0 || a->timeLength <= 0) return AF_OK;
     if (a->hOrder < 1 || a->pOrder < 1 || !(a->hOrder & 1) || !(a->pOrder & 1) || a->hOrder > AFB200_HPSS_MAX_ORDER ||
-        a->pOrder > AFB200_HPSS_MAX_ORDER || (!a->hRe && !a->pRe))
-        return af_fail(AF_ERR_ARG, "hpss mask: orders %d / %d", a->hOrder, a->pOrder);
+        a->pOrder > AFB200_HPSS_MAX_ORDER)
+        return af_fail(AF_ERR_ARG, "hpss mask: orders %d / %d; odd orders 1 .. %d are supported", a->hOrder, a->pOrder,
+                       AFB200_HPSS_MAX_ORDER);
+    if (!a->hRe && !a->pRe) return af_fail(AF_ERR_ARG, "hpss mask: no output (hRe and pRe are both NULL)");
     HpssParams p;
     p.re = a->re; p.im = a->im;
     p.hRe = a->hRe; p.hIm = a->hIm; p.pRe = a->pRe; p.pIm = a->pIm;

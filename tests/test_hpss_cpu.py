@@ -1,9 +1,13 @@
 """Harmonic-percussive separation without a GPU: the numpy oracle against the reference build (or its stored outputs in
 tests/golden/hpss.npz), the constructor statuses and calDataLength of both libraries over a grid of parameters, the
-refusals (which need no device), the exported and bound symbols of include/afb200_hpss.h and afb200_ext.h, and the
-Python class's argument checks."""
+refusals (which need no device), the exported and bound symbols of include/afb200_hpss.h and afb200_ext.h, the
+Python class's argument checks, and the float32 model of k_hpss_mask that tests/test_gpu_hpss_cells.py holds the kernel
+to: its medians against scipy's median_filter, its masks against the float64 formula within 8 float32 ulps,
+and its ctypes mirror of AfHpssArgs against csrc/af_internal.h."""
+import ctypes as C
 import itertools
 import os
+import re
 
 import numpy as np
 import pytest
@@ -168,3 +172,75 @@ def test_python_class_checks(product_lib):
     # no channels: no device work, empty results of the right shape
     a, b = h.hpss_batch(np.zeros((0, 5000), np.float32))
     assert a.shape == b.shape == (0, HO.data_length(5000, 4096))
+
+
+# ------------------------------------------------------------------------------------------------ the mask model
+# shapes of the cell tests small enough for the float64 reference on every pattern here
+PIN_SHAPES = [s for s in HO.MASK_SHAPES if s[0] * s[1] * (s[2] + s[3]) <= 7_000_000]
+
+
+def test_pin_shapes_cover_every_order():
+    """the shapes pinned here still include every order the cell tests run"""
+    orders = {(h, p) for _, _, h, p in PIN_SHAPES}
+    assert {(1, 31), (21, 1), (1, 1), (3, 3), (5, 7), (21, 31), (31, 21), (63, 65), (127, 255), (383, 3), (3, 383),
+            (383, 383)} <= orders, orders
+
+
+@pytest.mark.parametrize("pattern", HO.PATTERNS)
+def test_mask_medians_match_scipy(pattern):
+    """the model's medians are scipy's median_filter (mode constant, cval 0), clip by clip, exactly; order 1 gives 0"""
+    from scipy.ndimage import median_filter
+    for T, W, h, p in PIN_SHAPES:
+        re, im = HO.mask_planes(pattern, T, W)
+        mag = np.sqrt(re * re + im * im)
+        mH, mP = HO.medians(mag, 3, h, p)
+        for c in range(3):
+            rows = slice(c * T, (c + 1) * T)
+            want = median_filter(mag[rows], size=(h, 1), mode="constant", cval=0.0) if h > 1 else 0 * mag[rows]
+            assert np.array_equal(mH[rows], want), (pattern, T, W, h, p, c)
+        want = median_filter(mag, size=(1, p), mode="constant", cval=0.0) if p > 1 else 0 * mag
+        assert np.array_equal(mP, want), (pattern, T, W, h, p)
+
+
+MODEL_ULPS = 8      # measured worst 6.7: each cell is about ten float32 roundings of positive terms, no cancellation
+
+
+@pytest.mark.parametrize("pattern", HO.PATTERNS)
+def test_mask_model_within_ulps_of_float64(pattern):
+    """the float32 model against the float64 formula, element by element, within MODEL_ULPS float32 ulps of the float64
+    value (the spacing of float32 there, 2^-149 in the subnormal range, so results that underflow get the same number
+    of subnormal steps); where the float64 value is 0 the model gives exactly +-0"""
+    for T, W, h, p in PIN_SHAPES:
+        re, im = HO.mask_planes(pattern, T, W)
+        got = HO.mask_model(re, im, 3, h, p)
+        want = HO.mask_ref64(re, im, 3, h, p)
+        for k in range(4):
+            assert got[k].dtype == np.float32
+            err = np.abs(got[k].astype(np.float64) - want[k])
+            ulp = np.spacing(np.abs(want[k]).astype(np.float32)).astype(np.float64)
+            bad = np.argwhere(err > MODEL_ULPS * ulp)
+            assert bad.size == 0, (pattern, T, W, h, p, k, bad[:5].tolist(), (err / ulp).max())
+            assert (got[k][want[k] == 0] == 0).all(), (pattern, T, W, h, p, k)
+
+
+def _c_struct_fields(header, name):
+    """[(field, C type)] of `typedef struct { ... } name;` in header, one entry per declarator ("float *" for a
+    pointer)"""
+    src = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^}]*)\}\s*" + name + r"\s*;", src).group(1)
+    fields = []
+    for decl in filter(None, (d.strip() for d in body.split(";"))):
+        base, names = re.fullmatch(r"(?:const\s+)?(\w+)\s+(.+)", decl, flags=re.S).groups()
+        for n in names.split(","):
+            n = n.strip()
+            fields.append((n.lstrip("*").strip(), base + " *" * n.count("*")))
+    return fields
+
+
+def test_hpss_args_mirror_matches_header():
+    """AfHpssArgs of _hpss_oracle, which the cell tests pass to af_launch_hpss_mask, has the header's fields in order,
+    so that a change to the struct fails here by name"""
+    from conftest import ROOT
+    ctypes_of = {"float *": HO.FLOAT_P, "int": C.c_int}
+    fields = _c_struct_fields(os.path.join(ROOT, "audioflux_b200", "csrc", "af_internal.h"), "AfHpssArgs")
+    assert [(n, ctypes_of[t]) for n, t in fields] == list(HO.AfHpssArgs._fields_), fields

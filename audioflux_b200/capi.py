@@ -314,6 +314,19 @@ HARMONIC_RATIO_API = {
     "harmonicRatioObj_harmonicRatioBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
 }
 
+# pitch by the pitch estimation filter (include/mir/_pitch_pef.h, include/afb200_pitch_pef.h) and the additive batched
+# entry point (include/afb200_ext.h)
+PITCH_PEF_API = {
+    "pitchPEFObj_new": (C.c_int, [P(vp), c_int_p, c_float_p, c_float_p, c_float_p, c_int_p, c_int_p, c_int_p, c_float_p,
+                                  c_float_p, c_float_p, c_int_p]),
+    "pitchPEFObj_calTimeLength": (C.c_int, [vp, C.c_int]),
+    "pitchPEFObj_setFilterParams": (None, [vp, C.c_float, C.c_float, C.c_float]),
+    "pitchPEFObj_pitch": (None, [vp, vp, C.c_int, vp]),
+    "pitchPEFObj_enableDebug": (None, [vp, C.c_int]),
+    "pitchPEFObj_free": (None, [vp]),
+    "pitchPEFObj_pitchBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -367,8 +380,8 @@ DSP_API = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, WAVELET_API, NMF_API, DSP_API,
-                              REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, PITCH_PEF_API, WAVELET_API, NMF_API,
+                              DSP_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -478,6 +478,28 @@ typedef struct {
 } AfHarmonicRatioArgs;
 int af_launch_harmonic_ratio(const AfHarmonicRatioArgs *a, void *stream);
 
+/* Pitch by the pitch estimation filter (kernels/pitch_pef.cu), n = 2^log2n (1 .. AFB200_PITCH_PEF_MAX_EXP), one launch:
+ * every frame t of every clip b (samples b * dataLength + t * hop .. + n-1) gets fre[b * T + t] = logFre[k], k the first
+ * arg-max over minIndex .. maxIndex of the correlation of the weighted log-frequency power with the filter (see
+ * include/afb200_pitch_pef.h), computed with an L = 2^log2L-point real transform.  `tables` (device) holds, in order:
+ * window n, lin n+1, logFre 2n, bandWidth 2n (floats), interpIndex 2n (ints), filter spectrum L/2 + 1 (float pairs). */
+typedef struct {
+    const float *data;            /* device: clips batch x dataLength */
+    const float *tables;
+    float *fre;                   /* device, batch x timeLength */
+    int log2n, log2L, padNum, minIndex, maxIndex, dataLength, hop, timeLength, batch;
+} AfPitchPefArgs;
+/* float offsets of the parts of `tables` */
+#define AF_PEF_LIN(n) (n)
+#define AF_PEF_LOG(n) (2 * (n) + 1)
+#define AF_PEF_BW(n) (4 * (n) + 1)
+#define AF_PEF_IDX(n) (6 * (n) + 1)
+#define AF_PEF_SPEC(n) (8 * (n) + 2)      /* even: float2-aligned */
+#define AF_PEF_TABLE_FLOATS(n, L) (8 * (size_t)(n) + 2 + (size_t)(L) + 2)
+int af_launch_pitch_pef(const AfPitchPefArgs *a, void *stream);
+/* in-place iterative radix-2 forward FFT in double, n a power of two (host/af_cqt_bank.c; setup only) */
+void af_fft_double(double *re, double *im, int n);
+
 /* Discrete wavelet transforms (kernels/wavelet.cu).  One split level of DWT / WPT: node k (0 .. nodes-1) of L samples
  * at in + b*inStride + k*L, periodically indexed, gives a[i] = sum_j loD[j] x[(2i + dec - dec/2 - j) mod L] and d[i]
  * likewise with hiD, i < L/2; a goes to lo + b*loStride + k*L + i and d to hi + b*hiStride + k*L + L/2 + i, the two

@@ -13,8 +13,8 @@
 #include <string.h>
 #include "../af_internal.h"
 
-/* in-place iterative radix-2 FFT in double (setup only) */
-static void fft_double(double *re, double *im, int n) {
+/* in-place iterative radix-2 FFT in double (setup only; af_internal.h) */
+void af_fft_double(double *re, double *im, int n) {
     for (int i = 1, j = 0; i < n; i++) {
         int bit = n >> 1;
         for (; j & bit; bit >>= 1) j ^= bit;
@@ -107,7 +107,7 @@ int af_cqt_bank_build(AfCqtBank *b, int num, int samplate, float minFre, int bpo
             re[st + j] = tr * rescale;
             im[st + j] = ti * rescale;
         }
-        fft_double(re, im, n);
+        af_fft_double(re, im, n);
         for (int k = 0; k < width; k++) {
             float vr = (float)re[k], vi = (float)im[k];
             if (vr * vr + vi * vi > thresh2) { b->kr[row * width + k] = vr; b->ki[row * width + k] = vi; }
@@ -133,7 +133,7 @@ int af_cqt_time_kernels(const AfCqtBank *b, float *kappaRe, float *kappaIm) {
             re[k] = k < width ? b->kr[(size_t)i * width + k] : 0.0;
             im[k] = k < width ? b->ki[(size_t)i * width + k] : 0.0;
         }
-        fft_double(re, im, n);       /* forward DFT over k gives sum_k K[k] e^{-2 pi i k n/N} */
+        af_fft_double(re, im, n);       /* forward DFT over k gives sum_k K[k] e^{-2 pi i k n/N} */
         for (int t = 0; t < n; t++) { kappaRe[(size_t)i * n + t] = (float)re[t]; kappaIm[(size_t)i * n + t] = (float)im[t]; }
     }
     free(re); free(im);

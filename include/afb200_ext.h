@@ -30,6 +30,7 @@
 #include "afb200_hpss.h"
 #include "afb200_onset.h"
 #include "afb200_harmonic_ratio.h"
+#include "afb200_pitch_pef.h"
 #include "afb200_dwt.h"
 #include "afb200_wpt.h"
 #include "afb200_swt.h"
@@ -249,6 +250,13 @@ int onsetObj_onsetBatch(OnsetObj onsetObj, const float *spec, const float *phase
  * then the frames without a crossing of their own. */
 int harmonicRatioObj_harmonicRatioBatch(HarmonicRatioObj harmonicRatioObj, const float *data, int dataLength, int batch,
                                         float *value, int memKind, void *stream);
+
+/* pitch (PEF) of a batch: data batch x dataLength -> freArr batch x T, T = (dataLength - n) / slideLength + 1 (0 below n
+ * samples).  Each clip is computed on its own: the call neither reads nor updates the streaming carry of isContinue.
+ * Each clip's row is bit-identical to pitchPEFObj_pitch on that clip without streaming, whatever the batch.  One kernel
+ * launch per staging chunk. */
+int pitchPEFObj_pitchBatch(PitchPEFObj pitchPEFObj, const float *data, int dataLength, int batch, float *freArr,
+                           int memKind, void *stream);
 
 /* discrete wavelet transforms of a batch of clips (data batch x N): coef batch x N and mData batch x rows x N (rows =
  * num for DWT, 2^num for WPT; NULL: not written); SWT: mData1, mData2 batch x num x fftLength.  One kernel launch per

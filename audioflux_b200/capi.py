@@ -327,6 +327,19 @@ PITCH_PEF_API = {
     "pitchPEFObj_pitchBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
 }
 
+# pitch by YIN (include/mir/_pitch_yin.h, include/afb200_pitch_yin.h) and the additive batched entry point
+# (include/afb200_ext.h)
+PITCH_YIN_API = {
+    "pitchYINObj_new": (C.c_int, [P(vp), c_int_p, c_float_p, c_float_p, c_int_p, c_int_p, c_int_p, c_int_p]),
+    "pitchYINObj_setThresh": (None, [vp, C.c_float]),
+    "pitchYINObj_calTimeLength": (C.c_int, [vp, C.c_int]),
+    "pitchYINObj_pitch": (None, [vp, vp, C.c_int, vp, vp, vp]),
+    "pitchYINObj_getTroughData": (C.c_int, [vp, P(P(C.c_float)), P(P(C.c_float)), P(P(C.c_int))]),
+    "pitchYINObj_enableDebug": (None, [vp, C.c_int]),
+    "pitchYINObj_free": (None, [vp]),
+    "pitchYINObj_pitchBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, vp]),
+}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -380,8 +393,8 @@ DSP_API = {
 
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
-                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, PITCH_PEF_API, WAVELET_API, NMF_API,
-                              DSP_API, REFERENCE_BUILDERS)) -> dict:
+                              RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, PITCH_PEF_API, PITCH_YIN_API,
+                              WAVELET_API, NMF_API, DSP_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -49,7 +49,7 @@ size_t af_dev_free_bytes(void);
  * A chunk is about `chunkBytes` of the larger side (in + in-out planes, or out + in-out planes), a multiple of 16
  * items when it holds at least 16, and at least one item.  Items must be independent of one another. */
 enum { AF_IN = 1, AF_OUT = 2, AF_INOUT = 3 };
-#define AF_PIPE_MAX_PLANES 6
+#define AF_PIPE_MAX_PLANES 7
 #define AF_PIPE_CHUNK_BYTES ((size_t)64 << 20)
 typedef struct {
     const void *ptr;      /* caller's pointer (host or device, as memKind says); NULL: the plane is not used in this call */
@@ -497,6 +497,19 @@ typedef struct {
 #define AF_PEF_SPEC(n) (8 * (n) + 2)      /* even: float2-aligned */
 #define AF_PEF_TABLE_FLOATS(n, L) (8 * (size_t)(n) + 2 + (size_t)(L) + 2)
 int af_launch_pitch_pef(const AfPitchPefArgs *a, void *stream);
+/* Pitch by YIN (kernels/pitch_yin.cu), n = 2^log2n (1 .. AFB200_PITCH_YIN_MAX_EXP), one launch: every frame t of every
+ * clip b (samples b * dataLength + t * hop .. + n-1) gets, with f = b * T + t, the outputs of
+ * include/afb200_pitch_yin.h: fre[f] and value1[f] (only in frames with a trough), value2[f], and the trough rows
+ * mFre / mTrough [f][yinLength/2 + 1] (zero past the count) with their count lens[f].  Each output but fre may be
+ * NULL.  1 <= minIndex <= maxIndex <= n - 1 - autoLength. */
+typedef struct {
+    const float *data;            /* device: clips batch x dataLength */
+    float *fre, *value1, *value2, *mFre, *mTrough;
+    int *lens;
+    int log2n, autoLength, minIndex, maxIndex, samplate, dataLength, hop, timeLength, batch;
+    float thresh;
+} AfPitchYinArgs;
+int af_launch_pitch_yin(const AfPitchYinArgs *a, void *stream);
 /* in-place iterative radix-2 forward FFT in double, n a power of two (host/af_cqt_bank.c; setup only) */
 void af_fft_double(double *re, double *im, int n);
 

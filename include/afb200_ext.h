@@ -31,6 +31,7 @@
 #include "afb200_onset.h"
 #include "afb200_harmonic_ratio.h"
 #include "afb200_pitch_pef.h"
+#include "afb200_pitch_yin.h"
 #include "afb200_dwt.h"
 #include "afb200_wpt.h"
 #include "afb200_swt.h"
@@ -256,6 +257,17 @@ int harmonicRatioObj_harmonicRatioBatch(HarmonicRatioObj harmonicRatioObj, const
  * Each clip's row is bit-identical to pitchPEFObj_pitch on that clip without streaming, whatever the batch.  One kernel
  * launch per staging chunk. */
 int pitchPEFObj_pitchBatch(PitchPEFObj pitchPEFObj, const float *data, int dataLength, int batch, float *freArr,
+                           int memKind, void *stream);
+
+/* pitch (YIN) of a batch: data batch x dataLength -> freArr, valueArr1, valueArr2 batch x T, mFreArr, mTroughArr
+ * batch x T x mLen (mLen = yinLength/2 + 1, entries past lenArr zero) and lenArr batch x T ints, T =
+ * (dataLength - n) / slideLength + 1 (0 below n samples).  Every output but freArr may be NULL: it is then neither
+ * computed nor written.  In frames without a trough freArr and valueArr1 are left as they are, on the device as well.
+ * Each clip is computed on its own: the call neither reads nor updates the streaming carry of isContinue.  Each clip's
+ * row is bit-identical to pitchYINObj_pitch on that clip without streaming, whatever the batch.  One kernel launch per
+ * staging chunk. */
+int pitchYINObj_pitchBatch(PitchYINObj pitchYINObj, const float *data, int dataLength, int batch, float *freArr,
+                           float *valueArr1, float *valueArr2, float *mFreArr, float *mTroughArr, int *lenArr,
                            int memKind, void *stream);
 
 /* discrete wavelet transforms of a batch of clips (data batch x N): coef batch x N and mData batch x rows x N (rows =

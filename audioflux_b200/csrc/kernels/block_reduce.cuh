@@ -12,8 +12,22 @@ __device__ __forceinline__ bool beats(float v, int i, float w, int j) {
     return i >= 0 && (j < 0 || v > w || (v == w && i < j));
 }
 
-// first index of the block's maximum over the candidates (i >= 0); -1 when there is none.  This is the reference's
-// __vmax once the caller keeps a NaN first value as the maximum and passes later NaNs over.  redv / redi: 32 each
+// the reference's __vmax (`max < v` from the first value on) in three steps: each thread offers its values with
+// vmax_take, block_argmax reduces the threads' candidates, and vmax_first applies the rule for the first value
+
+// one value v at index i: NaN is passed over, a strictly larger value replaces the candidate (bv, bi), so the first
+// maximum is kept.  Start with bi = -1
+__device__ __forceinline__ void vmax_take(float v, int i, float &bv, int &bi) {
+    const bool take = v == v && (bi < 0 || v > bv);
+    bv = take ? v : bv;
+    bi = take ? i : bi;
+}
+
+// __vmax's index from block_argmax's bi: the first index `first` when the first value v0 is NaN (it stays the maximum)
+// or when there is no candidate
+__device__ __forceinline__ int vmax_first(int bi, float v0, int first) { return v0 != v0 || bi < 0 ? first : bi; }
+
+// first index of the block's maximum over the candidates (i >= 0); -1 when there is none.  redv / redi: 32 each
 __device__ int block_argmax(float v, int i, float *redv, int *redi) {
     for (int o = 16; o; o >>= 1) {
         const float w = __shfl_xor_sync(0xffffffffu, v, o);

@@ -10,9 +10,8 @@
 //   3. the prefix sums of x^2 (a block scan; the reference sums sequentially, :249-256);
 //   4. the crossing: the first j in 2 .. maxLength where r[j], r[j-1] change sign, zeros included (a block minimum);
 //      minIndex = j - 1 (:259-266);
-//   5. g[k] = r[j] / sqrtf(r[0] E[j] + 1e-16) with the sum in double (:270-273), its first arg-max (__vmax's `max < v`:
-//      a NaN first value stays the maximum, later NaNs are passed over) and the parabolic refinement in double
-//      (util_qaudInterp, :277-285).
+//   5. g[k] = r[j] / sqrtf(r[0] E[j] + 1e-16) with the sum in double (:270-273), its first arg-max (__vmax: vmax_take,
+//      block_argmax, vmax_first) and the parabolic refinement in double (util_qaudInterp, :277-285).
 // The minIndex of a frame without a crossing is the last one an earlier frame of the same call found (it lives outside
 // the reference's frame loop).  That is the only coupling between frames, and it stays out of this pass: every frame
 // stores its crossing (-1 for none) in minIdx, and only frames with one store their value.
@@ -113,16 +112,12 @@ __device__ void hr_frame(const HrParams &p, long long f, int m, float2 *A, float
     const int len = L - m - 1;                                         // g[k] = gamma(m + 1 + k), k < len
     float bv = 0.f;
     int bi = -1;
-    for (int k = tid; k < len; k += bd) {
-        const float g = gamma(m + 1 + k);
-        if (g == g && (bi < 0 || g > bv)) { bv = g; bi = k; }
-    }
+    for (int k = tid; k < len; k += bd) vmax_take(gamma(m + 1 + k), k, bv, bi);
     bi = block_argmax(bv, bi, redv, redi);
     if (tid == 0) {
         float v = 0.0f;                                                // len 0: __vmax leaves the value at 0
         if (len > 0) {
-            const float g0 = gamma(m + 1);
-            const int k = g0 != g0 || bi < 0 ? 0 : bi;
+            const int k = vmax_first(bi, gamma(m + 1), 0);
             const float g = gamma(m + 1 + k);
             v = k == 0 || k == len - 1 ? g : qaud_interp(gamma(m + k), g, gamma(m + 2 + k));
         }

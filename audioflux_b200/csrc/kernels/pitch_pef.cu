@@ -8,13 +8,12 @@
 //      real-FFT post-pass give power[k] = re^2 + im^2, k = 0 .. n, kept in its own buffer;
 //   2. s[P + i] = (y1 + (log[i] - x1)(y2 - y1)/(x2 - x1)) * bandWidth[i], i < 2n: __vinterp_linear's step with its
 //      segment index from the object's table, the grids read from the device tables; s is zero elsewhere up to L;
-//   3. s, packed as L/2 complex points, is transformed in place (af_fft_inplace_dif: bit-reversed order); the real-FFT
-//      post-pass gives S[k] for the pair k, L/2 - k, then S conj(F) with the filter's spectrum F, and the pre-pass of
-//      the inverse real transform written conjugated at the same positions; af_fft_inplace_dit and one more
-//      conjugation give c = L IFFT_L(S conj F), the correlation c[k] = sum_j filter[j] s[j + k mod L].  The 1/L of the
-//      inverse is left out: a power-of-two scale changes no comparison;
-//   4. the first arg-max of c over the lags minIndex .. maxIndex (__vmax's `max < v`: a NaN first value stays the
-//      maximum, later NaNs are passed over), and fre = log[that lag].
+//   3. s, packed as L/2 complex points, is transformed in place (af_fft_inplace_dif: bit-reversed order);
+//      af_real_inverse turns S conj(F), S read by af_real_bin_brev and F the filter's spectrum, into (L/2) c, c the
+//      correlation c[k] = sum_j filter[j] s[j + k mod L], read by af_real_at.  The scale is left in: a power-of-two
+//      scale changes no comparison;
+//   4. the first arg-max of c over the lags minIndex .. maxIndex (__vmax: vmax_take, block_argmax, vmax_first), and
+//      fre = log[that lag].
 // Only the clips are read from HBM and one float per frame is written.
 //
 // The transform length.  The reference correlates at 8n (P > 0) or 4n (P = 0).  Any L >= P + 2n (s fits) and
@@ -44,22 +43,9 @@ struct PefParams {
     int n, log2n, nc, log2nc, pad, minIndex, maxIndex, dataLength, hop, T;
 };
 
-// bin k (0 .. nc) of the L-point real FFT whose nc-point packed transform z is in bit-reversed order
-__device__ __forceinline__ float2 real_bin_brev(const PefParams &p, const float2 *z, int k) {
-    const int nc = p.nc;
-    const float2 zk = z[af_brev(k == nc ? 0 : k, p.log2nc)], zp = z[af_brev(k == 0 ? 0 : nc - k, p.log2nc)];
-    return af_real_post(zk, zp, af_real_tw(p.tw2, nc, k), k, nc);
-}
-
 __device__ __forceinline__ float2 times_conj_filter(const PefParams &p, const float2 *z, int k) {
-    const float2 x = real_bin_brev(p, z, k), f = __ldg(p.spec + k);
+    const float2 x = af_real_bin_brev(z, p.tw2, k, p.nc, p.log2nc), f = __ldg(p.spec + k);
     return make_float2(x.x * f.x + x.y * f.y, x.y * f.x - x.x * f.y);
-}
-
-// lag m of the correlation from the natural-order DIT result y (c[2j] + i c[2j+1] = conj(y[j]))
-__device__ __forceinline__ float lag_value(const float2 *y, int m) {
-    const float2 v = y[m >> 1];
-    return (m & 1) ? -v.y : v.x;
 }
 
 __global__ void __launch_bounds__(kMaxThreads) k_pitch_pef(PefParams p) {
@@ -102,31 +88,14 @@ __global__ void __launch_bounds__(kMaxThreads) k_pitch_pef(PefParams p) {
     __syncthreads();
 
     af_fft_inplace_dif(S, nc, p.tw2);
-    // pairs (k, nc - k): each thread reads and writes only the bit-reversed positions of its own pair
-    for (int k = tid; k <= nc / 2; k += bd) {
-        const int m = nc - k;
-        const float2 pk = times_conj_filter(p, S, k), pm = times_conj_filter(p, S, m);
-        const float2 yk = af_real_pre_conj(pk, pm, af_real_tw(p.tw2, nc, k));
-        const float2 ym = k > 0 && m != k ? af_real_pre_conj(pm, pk, af_real_tw(p.tw2, nc, m)) : yk;
-        S[af_brev(k, p.log2nc)] = yk;
-        if (k > 0 && m != k) S[af_brev(m, p.log2nc)] = ym;
-    }
-    __syncthreads();
-    af_fft_inplace_dit(S, nc, p.log2nc, p.tw2);
+    af_real_inverse(S, nc, p.log2nc, p.tw2, [&](int k) { return times_conj_filter(p, S, k); });
 
     const int lo = p.minIndex, hi = p.maxIndex;
     float bv = 0.0f;
     int bi = -1;
-    for (int k = lo + tid; k <= hi; k += bd) {
-        const float v = lag_value(S, k);
-        if (v == v && (bi < 0 || v > bv)) { bv = v; bi = k; }
-    }
+    for (int k = lo + tid; k <= hi; k += bd) vmax_take(af_real_at(S, k), k, bv, bi);
     bi = block_argmax(bv, bi, redv, redi);
-    if (tid == 0) {
-        const float v0 = lag_value(S, lo);
-        if (v0 != v0 || bi < 0) bi = lo;                               // __vmax: a NaN first value stays the maximum
-        p.fre[f] = __ldg(p.logf + bi);
-    }
+    if (tid == 0) p.fre[f] = __ldg(p.logf + vmax_first(bi, af_real_at(S, lo), lo));
 }
 
 }  // namespace

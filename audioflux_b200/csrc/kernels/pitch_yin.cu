@@ -5,18 +5,17 @@
 //   1. the frame x and y[j] = x[A - j] (j <= A, 0 beyond) are read into two n-point real inputs packed as nc complex
 //      points each; one thread forms E, the running sum of x^2 over 0 .. A + M, in the reference's sequential float32
 //      order;
-//   2. both are transformed in place (af_fft_inplace_dif: bit-reversed order); per pair (k, nc - k) the real-FFT
-//      post-pass separates X[k] and Y[k], then X Y and the pre-pass of the inverse real transform, written conjugated at
-//      the same positions; af_fft_inplace_dit and one more conjugation give (n/2) c, c = IFFT_n(X Y), and
-//      r[k] = c[A + k] for k <= M (no product x[m] x[m + k] wraps there), scaled by 2/n exactly;
+//   2. both are transformed in place (af_fft_inplace_dif: bit-reversed order); af_real_inverse turns X Y, X and Y read
+//      by af_real_bin_brev, into (n/2) c, c = IFFT_n(X Y), written over the packed x; r[k] = c[A + k] for k <= M (no
+//      product x[m] x[m + k] wraps there), read by af_real_at and scaled by 2/n exactly;
 //   3. e2, d and their 1e-6 clamps (in double, as fabs() compares), then one thread forms the running sum of
 //      d[1 .. M] in the reference's order, and yin[k] = d[minIndex + k] / (mean + 1e-16) in double, as C promotes it;
 //      e2 and the running sums are where the reference's float32 cancellation lies, so the correlation's rounding is
 //      the only difference left;
 //   4. the trough flags and the row minimum over contiguous runs of the yin row per thread: the first trough by a
-//      block minimum, __vmin's first minimum (a NaN first value stays the minimum) by an arg-max of -yin, and, when the
-//      trough rows are requested, their positions by a block prefix count.  The parabolic offset of a trough is done
-//      in double, as C promotes it.
+//      block minimum, __vmin's first minimum by __vmax's steps (vmax_take, block_argmax, vmax_first) on -yin, and,
+//      when the trough rows are requested, their positions by a block prefix count.  The parabolic offset of a trough
+//      is done in double, as C promotes it.
 // Only the clips are read from HBM.
 //
 // Shared memory: 8n bytes for the two packed transforms (later d and the running sums) and 4 (A + M + 1) bytes for E
@@ -43,19 +42,6 @@ struct YinParams {
     int nc, log2nc, A, minIndex, M, Y, mLen, samplate, dataLength, hop, T;
     float thresh;
 };
-
-// bin k (0 .. nc) of the n-point real FFT whose nc-point packed transform z is in bit-reversed order
-__device__ __forceinline__ float2 real_bin_brev(const YinParams &p, const float2 *z, int k) {
-    const int nc = p.nc;
-    const float2 zk = z[af_brev(k == nc ? 0 : k, p.log2nc)], zp = z[af_brev(k == 0 ? 0 : nc - k, p.log2nc)];
-    return af_real_post(zk, zp, af_real_tw(p.tw, nc, k), k, nc);
-}
-
-// value m of the real result from the natural-order DIT output y (c[2j] + i c[2j+1] = conj(y[j]))
-__device__ __forceinline__ float lag_value(const float2 *y, int m) {
-    const float2 v = y[m >> 1];
-    return (m & 1) ? -v.y : v.x;
-}
 
 // the reference's clamp: fabs(v) >= 1e-6, a double comparison
 __device__ __forceinline__ float clamp_small(float v) { return fabs((double)v) >= 1e-6 ? v : 0.0f; }
@@ -141,22 +127,14 @@ __global__ void __launch_bounds__(kMaxThreads) k_pitch_yin(YinParams p) {
 
     af_fft_inplace_dif(X, nc, p.tw);
     af_fft_inplace_dif(Yc, nc, p.tw);
-    // pairs (k, nc - k): each thread reads the bit-reversed positions of its own pair in both transforms and writes
-    // them in X only
-    for (int k = tid; k <= nc / 2; k += bd) {
-        const int m = nc - k;
-        const float2 pk = af_cmul(real_bin_brev(p, X, k), real_bin_brev(p, Yc, k));
-        const float2 pm = af_cmul(real_bin_brev(p, X, m), real_bin_brev(p, Yc, m));
-        X[af_brev(k, p.log2nc)] = af_real_pre_conj(pk, pm, af_real_tw(p.tw, nc, k));
-        if (k > 0 && m != k) X[af_brev(m, p.log2nc)] = af_real_pre_conj(pm, pk, af_real_tw(p.tw, nc, m));
-    }
-    __syncthreads();
-    af_fft_inplace_dit(X, nc, p.log2nc, p.tw);
+    af_real_inverse(X, nc, p.log2nc, p.tw, [&](int k) {
+        return af_cmul(af_real_bin_brev(X, p.tw, k, nc, p.log2nc), af_real_bin_brev(Yc, p.tw, k, nc, p.log2nc));
+    });
 
     const float inv = 1.0f / (float)nc;                               // the unscaled chain gives nc c; exact
     const float e0 = clamp_small(E[A] - E[0]);
     for (int j = tid; j <= M; j += bd)                                 // :375-415
-        ys[j] = e0 + clamp_small(E[A + j] - E[j]) - 2.0f * clamp_small(lag_value(X, A + j) * inv);
+        ys[j] = e0 + clamp_small(E[A + j] - E[j]) - 2.0f * clamp_small(af_real_at(X, A + j) * inv);
     __syncthreads();
     if (tid == 0) running_sum(ys + 1, M, xs, false);                  // :426-436, the sums of d[1 .. k+1]
     __syncthreads();
@@ -178,8 +156,7 @@ __global__ void __launch_bounds__(kMaxThreads) k_pitch_yin(YinParams p) {
             if (first == INT_MAX) first = k;
             count++;
         }
-        const float v = yin[k];
-        if (v == v && (bi < 0 || -v > bv)) { bv = -v; bi = k; }
+        vmax_take(-yin[k], k, bv, bi);
     }
     first = block_reduce_int(first, false, redi);
     if (p.value2) bi = block_argmax(bv, bi, redv, redi);
@@ -188,7 +165,7 @@ __global__ void __launch_bounds__(kMaxThreads) k_pitch_yin(YinParams p) {
             p.fre[f] = trough_fre(p, yin, first);
             if (p.value1) p.value1[f] = yin[first];
         }
-        if (p.value2) p.value2[f] = yin[0] != yin[0] || bi < 0 ? yin[0] : yin[bi];    // __vmin
+        if (p.value2) p.value2[f] = yin[vmax_first(bi, yin[0], 0)];                    // __vmin
     }
     if (p.mFre || p.mTrough || p.lens) {                               // :585-625
         int total;

@@ -131,6 +131,37 @@ __device__ __forceinline__ float2 af_real_pre_conj(float2 pk, float2 pm, float2 
     return make_float2(er - oi, -(ei + orr));
 }
 
+// ---- in-place real correlation: af_fft_inplace_dif, a product per bin, af_real_inverse, af_real_at ----
+
+// bin k (0 .. nc) of the real FFT whose nc-point packed transform z is in bit-reversed order (af_fft_inplace_dif)
+__device__ __forceinline__ float2 af_real_bin_brev(const float2 *z, const float2 *tw, int k, int nc, int log2nc) {
+    const float2 zk = z[af_brev(k == nc ? 0 : k, log2nc)], zp = z[af_brev(k == 0 ? 0 : nc - k, log2nc)];
+    return af_real_post(zk, zp, af_real_tw(tw, nc, k), k, nc);
+}
+
+// nc times the real inverse IFFT_N (1/N included, N = 2 nc) of the Hermitian spectrum X[k] = spectrum(k), in place in
+// the nc points of a: per pair (k, nc - k), the conjugated pre-pass written at the pair's bit-reversed positions, then
+// af_fft_inplace_dit leaves the packed result in natural order (read it with af_real_at).
+// Each thread owns its pairs and overwrites their positions: spectrum(k) may read a only at the bit-reversed positions
+// of bins k and nc - k (as af_real_bin_brev does), never another pair's.  All threads of the block must call it.
+template <class Spectrum>
+__device__ __forceinline__ void af_real_inverse(float2 *a, int nc, int log2nc, const float2 *tw, Spectrum spectrum) {
+    for (int k = threadIdx.x; k <= nc / 2; k += blockDim.x) {
+        const int m = nc - k;
+        const float2 pk = spectrum(k), pm = spectrum(m);
+        a[af_brev(k, log2nc)] = af_real_pre_conj(pk, pm, af_real_tw(tw, nc, k));
+        if (k > 0 && m != k) a[af_brev(m, log2nc)] = af_real_pre_conj(pm, pk, af_real_tw(tw, nc, m));
+    }
+    __syncthreads();
+    af_fft_inplace_dit(a, nc, log2nc, tw);
+}
+
+// value m (0 .. 2 nc - 1) of the real result af_real_inverse leaves in y: r[2j] + i r[2j+1] = conj(y[j])
+__device__ __forceinline__ float af_real_at(const float2 *y, int m) {
+    const float2 v = y[m >> 1];
+    return (m & 1) ? -v.y : v.x;
+}
+
 // value v at position k (0 .. N/2) of a real even N-sequence, in the float view f of a packed buffer
 __device__ __forceinline__ void af_put_even(float *f, int n, int k, float v) {
     f[k] = v;

@@ -6,11 +6,9 @@
 //   1. each signal, zero-padded to M, is packed as M/2 complex points (x[2j] + i x[2j+1]) and transformed in place
 //      (af_fft_inplace_dif: bit-reversed order).  The two signals keep separate transforms: packing a and b into one
 //      complex transform would let the louder leak into the quieter one;
-//   2. the real-FFT post-pass gives A[k] and B[k] for the pair k, M/2 - k, then P = A conj(B) (|A|^2 for the
-//      autocorrelation) and the pre-pass of the inverse real transform, written conjugated at the same bit-reversed
-//      positions;
-//   3. af_fft_inplace_dit (natural order) and one more conjugation give r = IFFT_M(P), the reference's 1/M included;
-//   4. the 2n-1 lags in the reference's order, divided by the Coeff scale, and __vmax's first arg-max.
+//   2. af_real_inverse turns P = A conj(B) (|A|^2 for the autocorrelation), A and B read by af_real_bin_brev, into
+//      nc r, r = IFFT_M(P) with the reference's 1/M and nc = M/2; af_real_at times 1/nc gives r;
+//   3. the 2n-1 lags in the reference's order, divided by the Coeff scale, and __vmax's first arg-max.
 // Longer rows (M = 2^15 .. 2^20): the zero-padded signals go through the CWT path's four-step forward legs
 // (af_launch_fft_rows); k_xcorr_cross forms the Hermitian P and writes its Hartley sequence c = Re P + Im P; a second
 // forward pass gives C, and Re C[j] + Im C[j] = M r[j].  k_xcorr_finish writes the lags and per-segment arg-max
@@ -43,25 +41,11 @@ __device__ __forceinline__ float coeff_scale(double s1, double s2) {
     return sqrtf(f1 * f2);
 }
 
-// bin k (0 .. nc) of the M-point real FFT whose nc-point packed transform z is stored in bit-reversed order
-__device__ __forceinline__ float2 real_bin(const XcParams &p, const float2 *z, int k) {
-    const int nc = p.nc;
-    const float2 zk = z[af_brev(k == nc ? 0 : k, p.log2nc)], zp = z[af_brev(k == 0 ? 0 : nc - k, p.log2nc)];
-    return af_real_post(zk, zp, af_real_tw(p.tw, nc, k), k, nc);
-}
-
 __device__ __forceinline__ float2 cross(const XcParams &p, const float2 *A, const float2 *B, int k) {
-    const float2 x = real_bin(p, A, k);
+    const float2 x = af_real_bin_brev(A, p.tw, k, p.nc, p.log2nc);
     if (!p.b) return make_float2(x.x * x.x + x.y * x.y, 0.0f);
-    const float2 y = real_bin(p, B, k);
+    const float2 y = af_real_bin_brev(B, p.tw, k, p.nc, p.log2nc);
     return make_float2(x.x * y.x + x.y * y.y, x.y * y.x - x.x * y.y);   // x conj(y)
-}
-
-// r[m] = IFFT_M(P)[m] from the natural-order DIT result y (r[2j] + i r[2j+1] = conj(y[j]) / nc)
-__device__ __forceinline__ float lag_value(const XcParams &p, const float2 *y, int m) {
-    const float2 v = y[m >> 1];
-    const float inv = 1.0f / (float)p.nc;
-    return (m & 1) ? -v.y * inv : v.x * inv;
 }
 
 __global__ void __launch_bounds__(kMaxThreads) k_xcorr(XcParams p) {
@@ -88,17 +72,7 @@ __global__ void __launch_bounds__(kMaxThreads) k_xcorr(XcParams p) {
     __syncthreads();
     af_fft_inplace_dif(A, nc, p.tw);
     if (y) af_fft_inplace_dif(B, nc, p.tw);
-    // pairs (k, nc - k): each thread reads and writes only the bit-reversed positions of its own pair
-    for (int k = tid; k <= nc / 2; k += bd) {
-        const int m = nc - k;
-        const float2 pk = cross(p, A, B, k), pm = cross(p, A, B, m);
-        const float2 yk = af_real_pre_conj(pk, pm, af_real_tw(p.tw, nc, k));
-        const float2 ym = k > 0 && m != k ? af_real_pre_conj(pm, pk, af_real_tw(p.tw, nc, m)) : yk;
-        A[af_brev(k, p.log2nc)] = yk;
-        if (k > 0 && m != k) A[af_brev(m, p.log2nc)] = ym;
-    }
-    __syncthreads();
-    af_fft_inplace_dit(A, nc, p.log2nc, p.tw);
+    af_real_inverse(A, nc, p.log2nc, p.tw, [&](int k) { return cross(p, A, B, k); });
 
     float scale = 1.0f;
     if (p.coeff) {
@@ -107,25 +81,23 @@ __global__ void __launch_bounds__(kMaxThreads) k_xcorr(XcParams p) {
         scale = coeff_scale(s1, s2);
     }
     const int L = 2 * n - 1, M = p.M;
+    const float inv = 1.0f / (float)nc;
+    auto at = [&](int j) {
+        const int lag = j - (n - 1);
+        const float v = af_real_at(A, lag < 0 ? lag + M : lag) * inv;
+        return p.coeff ? v / scale : v;
+    };
     float *o = p.out + row * L;
     float bv = 0.0f;
     int bi = -1;
     for (int j = tid; j < L; j += bd) {
-        const int lag = j - (n - 1);
-        float v = lag_value(p, A, lag < 0 ? lag + M : lag);
-        if (p.coeff) v = v / scale;
+        const float v = at(j);
         o[j] = v;
-        if (v == v && (bi < 0 || v > bv)) { bv = v; bi = j; }
+        vmax_take(v, j, bv, bi);
     }
     bi = block_argmax(bv, bi, redv, redi);
     if (tid == 0) {
-        auto at = [&](int j) {
-            const int lag = j - (n - 1);
-            float v = lag_value(p, A, lag < 0 ? lag + M : lag);
-            return p.coeff ? v / scale : v;
-        };
-        const float v0 = at(0);
-        if (v0 != v0 || bi < 0) bi = 0;                                // __vmax: a NaN first value stays the maximum
+        bi = vmax_first(bi, at(0), 0);
         if (p.maxValue) p.maxValue[row] = at(bi);
         if (p.maxIndex) p.maxIndex[row] = bi;
     }
@@ -193,7 +165,7 @@ __global__ void __launch_bounds__(kLongThreads) k_xcorr_finish(const float2 *__r
         float v = (v2.x + v2.y) * inv;
         if (coeff) v = v / scale;
         o[j] = v;
-        if (v == v && (bi < 0 || v > bv)) { bv = v; bi = j; }
+        vmax_take(v, j, bv, bi);
     }
     bi = block_argmax(bv, bi, redv, redi);
     if (threadIdx.x == 0) {
@@ -212,7 +184,7 @@ __global__ void __launch_bounds__(kFinishSegs) k_xcorr_argmax(const float *__res
     int bi = block_argmax(candV[(size_t)pair * kFinishSegs + t], candI[(size_t)pair * kFinishSegs + t], redv, redi);
     if (t == 0) {
         const float *o = out + (size_t)pair * L;
-        if (o[0] != o[0] || bi < 0) bi = 0;                            // __vmax: a NaN first value stays the maximum
+        bi = vmax_first(bi, o[0], 0);
         if (maxValue) maxValue[pair] = o[bi];
         if (maxIndex) maxIndex[pair] = bi;
     }

@@ -2,7 +2,7 @@
 tests/golden/pitch_pef.npz) over frame sizes, samplates, cut frequencies, filter parameters, slides, windows and
 signals; the statuses of new and calTimeLength against the reference, streaming included; setFilterParams changing
 nothing; the refusals (which need no device); the exported and bound symbols of include/afb200_pitch_pef.h and
-afb200_ext.h; the register and spill budget of kernels/pitch_pef.cu; and the Python class's arguments.
+afb200_ext.h; and the Python class's arguments.
 
 Run as a script, it rewrites tests/golden/pitch_pef.npz from the reference build (oracle/_ref):
 
@@ -12,7 +12,6 @@ import pytest
 
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none      # first: conftest puts the root on sys.path
 import _pitch_pef_oracle as PO
-from test_register_budgets import Budget, test_kernel_budget as _kernel_budget
 
 CASES = dict(PO.cases())
 
@@ -23,9 +22,6 @@ def _live(keys):
 
 
 GOLD = GoldenStore("pitch_pef.npz", _live, lambda: set(CASES))
-
-# CTAs of up to 1024 threads, two per SM at n = 2^12: at most 32 registers
-BUDGET = Budget("pitch_pef.cu", {"k_pitch_pef": "k_pitch_pef"}, 32, 0, 0, ("-fmad=false",))
 
 
 @pytest.mark.parametrize("name", list(CASES))
@@ -157,10 +153,6 @@ def test_pitch_pef_symbols_exported_and_bound(product_lib):
     check_symbols(product_lib, "afb200_pitch_pef.h", "pitchPEFObj_", capi.PITCH_PEF_API,
                   {"pitchPEFObj_new", "pitchPEFObj_calTimeLength", "pitchPEFObj_setFilterParams", "pitchPEFObj_pitch",
                    "pitchPEFObj_enableDebug", "pitchPEFObj_free"}, {"pitchPEFObj_pitchBatch"})
-
-
-def test_kernel_budget():
-    _kernel_budget(BUDGET)
 
 
 def test_python_class(product_lib):

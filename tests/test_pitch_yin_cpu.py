@@ -2,8 +2,8 @@
 tests/golden/pitch_yin.npz) over frame sizes, samplates, autocorrelation lengths, slides, thresholds, signals and the
 shortest yin rows, for fre, value1, value2 and the trough rows; the statuses of new and calTimeLength against the
 reference over a grid with NULL pointers and fallbacks; streaming in the reference; the refusals (which need no
-device); the exported and bound symbols of include/afb200_pitch_yin.h and afb200_ext.h; the register and spill budget
-of kernels/pitch_yin.cu; and the Python class's arguments.
+device); the exported and bound symbols of include/afb200_pitch_yin.h and afb200_ext.h; and the Python
+class's arguments.
 
 Run as a script, it rewrites tests/golden/pitch_yin.npz from the reference build (oracle/_ref):
 
@@ -13,7 +13,6 @@ import pytest
 
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none      # first: conftest puts the root on sys.path
 import _pitch_yin_oracle as YO
-from test_register_budgets import Budget, test_kernel_budget as _kernel_budget
 
 CASES = dict(YO.cases())
 FILL = 7.0                       # the outputs start as this; frames without a trough keep it in fre and value1
@@ -33,9 +32,6 @@ def _live(keys):
 
 
 GOLD = GoldenStore("pitch_yin.npz", _live, lambda: {f"{c}/{k}" for c in CASES for k in PLANES})
-
-# CTAs of up to 1024 threads; the launcher sizes them for 1536 threads per SM (65 536 registers / 40, rounded down)
-BUDGET = Budget("pitch_yin.cu", {"k_pitch_yin": "k_pitch_yin"}, 40, 0, 0, ("-fmad=false",))
 
 
 def reference_outputs(name):
@@ -169,10 +165,6 @@ def test_pitch_yin_symbols_exported_and_bound(product_lib):
                   {"pitchYINObj_new", "pitchYINObj_setThresh", "pitchYINObj_calTimeLength", "pitchYINObj_pitch",
                    "pitchYINObj_getTroughData", "pitchYINObj_enableDebug", "pitchYINObj_free"},
                   {"pitchYINObj_pitchBatch"})
-
-
-def test_kernel_budget():
-    _kernel_budget(BUDGET)
 
 
 def test_python_class(product_lib):

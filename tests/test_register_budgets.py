@@ -44,6 +44,10 @@ BUDGETS = [
                         "k_xcorr_finish": "k_xcorr_finish", "k_xcorr_argmax": "k_xcorr_argmax"}, 64, 0, 0,
            ("-fmad=false",)),
     Budget("czt.cu", {"5k_czt": "k_czt", "k_czt_filter": "k_czt_filter"}, 64, 0, 0, ("-fmad=false",)),
+    # CTAs of up to 1024 threads, two per SM at n = 2^12: at most 32 registers
+    Budget("pitch_pef.cu", {"k_pitch_pef": "k_pitch_pef"}, 32, 0, 0, ("-fmad=false",)),
+    # CTAs of up to 1024 threads; the launcher sizes them for 1536 threads per SM (65 536 registers / 40, rounded down)
+    Budget("pitch_yin.cu", {"k_pitch_yin": "k_pitch_yin"}, 40, 0, 0, ("-fmad=false",)),
 ]
 
 

@@ -2,7 +2,7 @@
 
 Host-side mirror of the reference's operator interface (same class / method / argument
 names as python/audioflux/{stft,bft,cqt,cwt,nsgt,st,fst,cepstrogram,spectrogram}.py, feature/xxcc.py,
-dsp/resample.py, dsp/xcorr.py, dsp/czt.py, mir/hpss.py, mir/onset.py, mir/harmonic_ratio.py, mir/pitch_pef.py, mir/pitch_yin.py, dwt.py / swt.py / wpt.py and classic/nmf.py) over the C-ABI
+dsp/resample.py, dsp/xcorr.py, dsp/czt.py, mir/hpss.py, mir/onset.py, mir/harmonic_ratio.py, mir/pitch_pef.py, mir/pitch_yin.py, mir/pitch_ncf.py, mir/pitch_cep.py, dwt.py / swt.py / wpt.py and classic/nmf.py) over the C-ABI
 library ``lib/libaudioflux_b200.so``.  No CPU fallback exists.
 """
 from .types import *  # noqa: F401,F403
@@ -25,6 +25,8 @@ from .onset import Onset, NoveltyParam  # noqa: F401
 from .harmonic_ratio import HarmonicRatio  # noqa: F401
 from .pitch_pef import PitchPEF  # noqa: F401
 from .pitch_yin import PitchYIN  # noqa: F401
+from .pitch_ncf import PitchNCF  # noqa: F401
+from .pitch_cep import PitchCEP  # noqa: F401
 from .wavelet import DWT, SWT, WPT  # noqa: F401
 from .nmf import nmf, nmf_batch  # noqa: F401
 from .xcorr import Xcorr  # noqa: F401

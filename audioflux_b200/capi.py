@@ -340,6 +340,18 @@ PITCH_YIN_API = {
     "pitchYINObj_pitchBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, vp]),
 }
 
+# pitch by the normalised correlation and by the cepstrum (include/mir/_pitch_{ncf,cep}.h,
+# include/afb200_pitch_{ncf,cep}.h) and the additive batched entry points (include/afb200_ext.h)
+PITCH_NCF_API = {
+    "pitchNCFObj_new": (C.c_int, [P(vp), c_int_p, c_float_p, c_float_p, c_int_p, c_int_p, c_int_p, c_int_p]),
+    "pitchNCFObj_calTimeLength": (C.c_int, [vp, C.c_int]),
+    "pitchNCFObj_pitch": (None, [vp, vp, C.c_int, vp]),
+    "pitchNCFObj_enableDebug": (None, [vp, C.c_int]),
+    "pitchNCFObj_free": (None, [vp]),
+    "pitchNCFObj_pitchBatch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
+}
+PITCH_CEP_API = {k.replace("NCF", "CEP"): v for k, v in PITCH_NCF_API.items()}
+
 # setup-time builders exported (non-static) by the reference only; used by tests to
 # compare constant tables (src/dsp/flux_window.h, src/filterbank/*.h)
 REFERENCE_BUILDERS = {
@@ -394,7 +406,7 @@ DSP_API = {
 
 def bind(lib: C.CDLL, tables=(REFERENCE_API, EXTENSION_API, SPECTRAL_API, NSGT_API, ST_API, CEPSTROGRAM_API,
                               RESAMPLE_API, HPSS_API, ONSET_API, HARMONIC_RATIO_API, PITCH_PEF_API, PITCH_YIN_API,
-                              WAVELET_API, NMF_API, DSP_API, REFERENCE_BUILDERS)) -> dict:
+                              PITCH_NCF_API, PITCH_CEP_API, WAVELET_API, NMF_API, DSP_API, REFERENCE_BUILDERS)) -> dict:
     """Apply argtypes/restype for every symbol the library actually exports.
     Returns {name: bool present}."""
     present = {}

@@ -510,6 +510,18 @@ typedef struct {
     float thresh;
 } AfPitchYinArgs;
 int af_launch_pitch_yin(const AfPitchYinArgs *a, void *stream);
+/* Pitch by the normalised correlation (mode AF_PITCH_NCF) or the cepstrum (AF_PITCH_CEP) (kernels/pitch_ncf_cep.cu),
+ * n = 2^log2n (1 .. 14), one launch: every frame t of every clip b (samples b * dataLength + t * hop .. + n-1) gets
+ * fre[b * T + t] = samplate / (index + 1), index __vmax's first arg-max over minIndex .. maxIndex of the row of
+ * include/afb200_pitch_ncf.h or include/afb200_pitch_cep.h.  NCF: 1 <= minIndex <= maxIndex < n; CEP:
+ * 0 <= minIndex <= maxIndex < 2n. */
+enum { AF_PITCH_NCF = 0, AF_PITCH_CEP = 1 };
+typedef struct {
+    const float *data, *window;   /* device: clips batch x dataLength, window n floats */
+    float *fre;                   /* device, batch x timeLength */
+    int mode, log2n, minIndex, maxIndex, samplate, dataLength, hop, timeLength, batch;
+} AfPitchLagArgs;
+int af_launch_pitch_ncf_cep(const AfPitchLagArgs *a, void *stream);
 /* in-place iterative radix-2 forward FFT in double, n a power of two (host/af_cqt_bank.c; setup only) */
 void af_fft_double(double *re, double *im, int n);
 

@@ -32,6 +32,8 @@
 #include "afb200_harmonic_ratio.h"
 #include "afb200_pitch_pef.h"
 #include "afb200_pitch_yin.h"
+#include "afb200_pitch_ncf.h"
+#include "afb200_pitch_cep.h"
 #include "afb200_dwt.h"
 #include "afb200_wpt.h"
 #include "afb200_swt.h"
@@ -268,6 +270,15 @@ int pitchPEFObj_pitchBatch(PitchPEFObj pitchPEFObj, const float *data, int dataL
  * staging chunk. */
 int pitchYINObj_pitchBatch(PitchYINObj pitchYINObj, const float *data, int dataLength, int batch, float *freArr,
                            float *valueArr1, float *valueArr2, float *mFreArr, float *mTroughArr, int *lenArr,
+                           int memKind, void *stream);
+
+/* pitch (NCF, CEP) of a batch: data batch x dataLength -> freArr batch x T, T = (dataLength - n) / slideLength + 1 (0
+ * below n samples).  Each clip is computed on its own: the call neither reads nor updates the streaming carry of
+ * isContinue.  Each clip's row is bit-identical to pitchNCFObj_pitch / pitchCEPObj_pitch on that clip without
+ * streaming, whatever the batch.  One kernel launch per staging chunk. */
+int pitchNCFObj_pitchBatch(PitchNCFObj pitchNCFObj, const float *data, int dataLength, int batch, float *freArr,
+                           int memKind, void *stream);
+int pitchCEPObj_pitchBatch(PitchCEPObj pitchCEPObj, const float *data, int dataLength, int batch, float *freArr,
                            int memKind, void *stream);
 
 /* discrete wavelet transforms of a batch of clips (data batch x N): coef batch x N and mData batch x rows x N (rows =

@@ -54,11 +54,12 @@ def edges(num):
             "list": [num // 3, 1, num - 1, 7, num // 3, 0, num // 2, 2]}
 
 
-def apply_edge(lib, obj, mode, num):
-    idx = edges(num)[mode]
-    if mode == "range":
+def apply_edge(lib, obj, mode, num, idx=None):
+    """mode 'full', 'range...' (setEdge) or any other name (setEdgeArr) over edges(num)[mode], or over idx when given"""
+    idx = edges(num)[mode] if idx is None else list(idx)
+    if mode.startswith("range"):
         lib.spectralObj_setEdge(obj, idx[0], idx[-1])
-    elif mode == "list":
+    elif mode != "full":
         p = _libc.calloc(len(idx), 4)
         (C.c_int * len(idx)).from_address(p)[:] = idx
         lib.spectralObj_setEdgeArr(obj, C.c_void_p(p), len(idx))     # the object owns the array from here on
@@ -68,14 +69,15 @@ def apply_edge(lib, obj, mode, num):
 TWO_OUTPUTS = ("max", "mean", "var")        # features whose call returns (value, fre)
 
 
-def call_c(lib, name, x, fre, mode="full", phase=None, **kw):
-    """one reference-signature call on a fresh object; x [T, num] -> [T] (or (value, fre) for max / mean / var)"""
+def call_c(lib, name, x, fre, mode="full", phase=None, idx=None, **kw):
+    """one reference-signature call on a fresh object; x [T, num] -> [T] (or (value, fre) for max / mean / var).
+    idx: the bin list of the mode in place of edges(num)[mode]"""
     x = np.ascontiguousarray(x, np.float32)
     T, num = x.shape
     fre = np.ascontiguousarray(fre, np.float32)
     obj = C.c_void_p()
     assert lib.spectralObj_new(C.byref(obj), num, fre.ctypes.data) == 0
-    apply_edge(lib, obj, mode, num)
+    apply_edge(lib, obj, mode, num, idx)
     lib.spectralObj_setTimeLength(obj, T)
     o1, o2 = np.zeros(T, np.float32), np.zeros(T, np.float32)
     X, O1, O2 = x.ctypes.data, o1.ctypes.data, o2.ctypes.data

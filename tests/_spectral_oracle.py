@@ -25,6 +25,12 @@ def flatness(x, idx, fre=None):                                   # flux_spectra
         return np.where(m != 0, g / np.where(m != 0, m, 1), 0.0)
 
 
+def _pos(v):
+    """the reference's `v > 0 ? v : 0`: a NaN difference (NaN or inf - inf) counts as 0"""
+    with np.errstate(invalid="ignore"):
+        return np.where(v > 0, v, 0.0)
+
+
 def _temporal(x, idx, step, fn):
     T = x.shape[0]
     out = np.zeros(T)
@@ -38,7 +44,7 @@ def _temporal(x, idx, step, fn):
 def flux(x, idx, fre=None, step=1, p=2, is_positive=False, is_exp=False, tp=0):     # :58-105
     def f(c, q):
         v = c - q
-        v = np.maximum(v, 0) if is_positive else np.abs(v)
+        v = _pos(v) if is_positive else np.abs(v)
         with np.errstate(all="ignore"):
             s = (v * v if p == 2 else np.power(v, p)).sum()
         if tp:
@@ -165,11 +171,11 @@ def hfc(x, idx, fre=None):                                         # :439-458, a
 
 
 def sd(x, idx, fre=None, step=1, is_positive=False):               # :461-492
-    return _temporal(x, idx, step, lambda c, q: (np.maximum(c - q, 0) if is_positive else np.abs(c - q)).sum())
+    return _temporal(x, idx, step, lambda c, q: (_pos(c - q) if is_positive else np.abs(c - q)).sum())
 
 
 def sf(x, idx, fre=None, step=1, is_positive=False):               # :495-526
-    return _temporal(x, idx, step, lambda c, q: ((np.maximum(c - q, 0) if is_positive else np.abs(c - q)) ** 2).sum())
+    return _temporal(x, idx, step, lambda c, q: ((_pos(c - q) if is_positive else np.abs(c - q)) ** 2).sum())
 
 
 def mkl(x, idx, fre=None, tp=0):                                   # :529-555

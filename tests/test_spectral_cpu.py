@@ -1,5 +1,11 @@
 """Spectral descriptors without a GPU: the numpy oracle against the reference build (or its stored outputs in
-tests/golden/spectral.npz), the argument rules of SpectralObj, the exported C API and the loud failure without a GPU."""
+tests/golden/spectral.npz), frame by frame on the crafted rows and rolloff look-back runs of tests/_spectral_frames.py
+(tests/golden/spectral_frames.npz), the argument rules of SpectralObj, the exported C API and the loud failure without a
+GPU.
+
+Run as a script, it rewrites tests/golden/spectral_frames.npz from the reference build (oracle/_ref):
+
+    python tests/test_spectral_cpu.py"""
 import ctypes as C
 import os
 import re
@@ -9,6 +15,7 @@ import pytest
 
 from conftest import ROOT
 import _spectral_cases as SC
+import _spectral_frames as SF
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none
 
 import audioflux_b200 as af
@@ -66,6 +73,84 @@ def test_oracle_matches_reference(ref_out):
 
 def test_golden_file_matches_reference_build():
     GOLD.check_file()
+
+
+def test_frames_golden_file_matches_reference_build():
+    GOLD_FRAMES.check_file()
+
+
+def _frame_cases():
+    """(case, x [B, T, num], phase or None, fre, mode, idx, variants): the crafted rows in each bin-list mode, a quiet
+    and a loud clip over one bin and over two (where log(1 + u) rounds 1 + u to float32), and the two rolloff
+    look-back clips"""
+    for mode, idx in SF.extreme_modes().items():
+        x, ph, fre = SF.extreme_clip(mode)
+        yield f"crafted-{mode}", x[None], ph[None], fre, mode, idx, SC.VARIANTS
+    for setname, mode in (("linear", "one"), ("cqt", "two")):    # a quiet clip (1e-2) and a loud one (1e2)
+        x, ph, fre = SF.clips(setname, 40, 2, seed=6)
+        yield f"quiet-{setname}-{mode}", x, ph, fre, mode, SF.bin_sets()[(setname, mode)], \
+            [v for v in SC.VARIANTS if ph is not None or v[0] not in SC.SO.PHASE]
+    for kind, variants in SF.LOOKBACK_VARIANTS.items():
+        x, fre, _, _ = SF.lookback_clips(kind)
+        yield f"lookback-{kind}", x, None, fre, "full", list(range(x.shape[-1])), \
+            [v for v in variants or SC.VARIANTS if v[0] not in SC.SO.PHASE]
+
+
+def _frame_key(case, b, variant, part):
+    name, kw = variant
+    return f"{case}/{b}/{name}{sorted(kw.items())}/{part}"
+
+
+def _frame_keys():
+    return {_frame_key(case, b, v, part) for case, x, _, _, _, _, variants in _frame_cases()
+            for v in variants for b in range(x.shape[0]) for part in range(2 if v[0] in SC.TWO_OUTPUTS else 1)}
+
+
+def _frame_live(keys):
+    lib = ref_lib_or_none()
+    res = {}
+    for case, x, ph, fre, mode, idx, variants in _frame_cases():
+        for v in variants:
+            for b in range(x.shape[0]):
+                out = SC.call_c(lib, v[0], x[b], fre, mode, None if ph is None else ph[b], idx=idx, **v[1])
+                for part, o in enumerate(out if isinstance(out, tuple) else (out,)):
+                    if _frame_key(case, b, v, part) in keys:
+                        res[_frame_key(case, b, v, part)] = o
+    return res
+
+
+GOLD_FRAMES = GoldenStore("spectral_frames.npz", _frame_live, _frame_keys,
+                          equal=lambda a, b: SC.agree(a, b, exact=True) is None)
+
+
+def test_oracle_matches_reference_frame_by_frame():
+    """NaN / +-inf / denormal / negative / zero / tied rows, one- and two-bin lists of a quiet clip, and rolloff runs
+    without a crossing: inputs of tests/test_gpu_spectral_frames.py on which the GPU is judged by the oracle, each
+    frame on its own scale"""
+    ref = GOLD_FRAMES.outputs(_frame_keys())
+    rep = SF.Report()
+    for case, x, ph, fre, mode, idx, variants in _frame_cases():
+        for v in variants:
+            for b in range(x.shape[0]):
+                nparts = 2 if v[0] in SC.TWO_OUTPUTS else 1
+                got = [ref[_frame_key(case, b, v, part)] for part in range(nparts)]
+                SF.check_clip(rep, f"{case} b={b}", v[0], v[1], got, x[b], idx, fre, None if ph is None else ph[b])
+    assert rep.ok(), rep.text()
+
+
+@pytest.mark.parametrize("kind", list(SF.LOOKBACK_VARIANTS))
+def test_look_back_runs_are_what_they_claim(kind):
+    """the frames lookback_clips marks as crossing are exactly those whose rolloff crosses in the oracle's float32, and
+    every non-crossing run of 5 .. 70 frames is there"""
+    x, fre, thr, cross = SF.lookback_clips(kind)
+    for b in range(2):
+        r = np.asarray(x[b], np.float32)
+        s = np.add.accumulate(r, axis=1, dtype=np.float32)[:, -1]
+        with np.errstate(invalid="ignore"):
+            hit = (np.add.accumulate(np.abs(r), axis=1, dtype=np.float32) >= (s * np.float32(thr))[:, None]).any(1)
+        assert np.array_equal(hit, cross[b]), kind
+    runs = [len(r) for b in range(2) for r in "".join("x" if c else "." for c in cross[b]).split("x") if r]
+    assert {5, 31, 32, 33, 64, 70} <= set(runs) and not cross[0, 0] and not cross[1, 0]
 
 
 def test_constructor_and_edge_rules(product_lib):
@@ -147,3 +232,10 @@ def test_no_gpu_means_loud_failure_spectral(product_lib):
     assert (out == 7.0).all()
     assert b"no CUDA device" in product_lib.afb200_lastError()
     product_lib.spectralObj_free(obj)
+
+
+if __name__ == "__main__":
+    import sys
+    if ref_lib_or_none() is None:
+        sys.exit("oracle/_ref/libaudioflux_ref.so not built")
+    print(f"{GOLD_FRAMES.name}: {GOLD_FRAMES.write()} arrays")

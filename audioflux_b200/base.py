@@ -170,6 +170,54 @@ class FrameAxis:
         return np.linspace(0, data_length / self.samplate, self.cal_time_length(data_length) + 1)
 
 
+class PitchBase(FrameAxis, Base):
+    """The body of the frame-wise pitch trackers (PitchPEF, PitchYIN, PitchNCF, PitchCEP): the constructor call,
+    cal_time_length and the batched pitch call of the C object named by _prefix.  {_prefix}_pitchBatch fills _planes
+    output planes [rows, T]; _zero: they start at 0 (in-out planes whose frames without a result keep their value);
+    _unset: trailing optional outputs passed as NULL."""
+    _prefix = ""
+    _planes, _zero, _unset = 1, False, ()
+
+    def _open(self, radix2_exp, *args):
+        """{_prefix}_new(&obj, *args) and fft_length"""
+        self._new(f"{self._prefix}_new", f"{self._prefix}_free", *args)
+        # the frame: 2**radix2_exp, or the reference's fallback 2**12 outside 1 .. 30
+        self.fft_length = 1 << (int(radix2_exp) if 1 <= radix2_exp <= 30 else 12)
+
+    def cal_time_length(self, data_length):
+        return getattr(self._lib, f"{self._prefix}_calTimeLength")(self._obj, int(data_length))
+
+    def pitch_batch(self, data):
+        """data [..., n] (numpy host | torch cuda) -> the output planes, each [..., cal_time_length(n)] float32 of the
+        same kind (a tuple when there are several).  One batched call for all channels; each row is bit-identical to a
+        legacy call."""
+        b = Batch(data)
+        t = self.cal_time_length(b.n)
+        out = [b.alloc(b.rows, t, zero=self._zero) for _ in range(self._planes)]
+        if b.rows and t:
+            self._call(f"{self._prefix}_pitchBatch", b, b.x, b.n, b.rows, *out, *self._unset)
+        out = tuple(b.shaped(o) for o in out)
+        return out if self._planes > 1 else out[0]
+
+    def pitch(self, data_arr):
+        """data_arr [..., n] -> pitch_batch's planes, each [..., time] float32"""
+        data_arr = np.asarray(data_arr, dtype=np.float32, order='C')
+        if data_arr.ndim == 0:
+            raise ValueError('Audio data must have at least one dimension')
+        if data_arr.shape[-1] == 0:
+            raise ValueError('Audio data must not be empty')
+        return self.pitch_batch(data_arr)
+
+
+def c_int(v):
+    """a pointer to the int v (the constructors' NULL-able arguments, always given here)"""
+    return C.byref(C.c_int(int(v)))
+
+
+def c_float(v):
+    return C.byref(C.c_float(float(v)))
+
+
 class SampleAxis:
     """Time axis of a per-sample transform (CWT family): one column per sample of the 2**radix2_exp window; and the
     family's batched call."""

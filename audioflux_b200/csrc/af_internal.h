@@ -93,6 +93,26 @@ int af_tail_assemble(AfTail *t, int fftLength, int slideLength, const float *dat
 void af_tail_free(AfTail *t);
 int af_sm_count(void);
 
+/* The frame-wise pitch trackers' core (host/af_pitch_frames.c), the first member of the PitchPEF, PitchYIN, PitchNCF
+ * and PitchCEP objects: frames of n = 2^log2n samples every slideLength, the streaming carry and the staging pipe. */
+typedef struct { int samplate, log2n, n, slideLength, isContinue; AfTail tail; AfPipe pipe; } AfPitchFrames;
+/* a tracker's constructor constants: its name, largest radix2Exp and what limits it, lowFre's default, highFre's
+ * default (NULL highFre) and the highFre that replaces a rejected one (lowFre then takes its default) */
+typedef struct { const char *who; int maxExp; const char *why; float lowFre, highFre, highReset; } AfPitchRules;
+/* samplate, lowFre, highFre, radix2Exp, slideLength and isContinue resolved in the reference's order into *f (no carry,
+ * no pipe) and *lf / *hf; 0, or -2 above maxExp */
+int af_pitch_frames_init(AfPitchFrames *f, float *lf, float *hf, const AfPitchRules *r, const int *samplate,
+                         const float *lowFre, const float *highFre, const int *radix2Exp, const int *slideLength,
+                         const int *isContinue);
+int af_pitch_frames(const AfPitchFrames *f, int dataLength);        /* frames in dataLength samples */
+int af_pitch_time_length(const AfPitchFrames *f, int dataLength);   /* calTimeLength: with the carry; 0 for NULL f */
+/* the batched call's argument check ("<who>: bad argument") and device; *T the frames per clip, 0 for an empty batch */
+int af_pitch_batch_begin(const AfPitchFrames *f, const char *who, const float *data, int dataLength, int batch,
+                         const float *fre, int *T);
+/* the legacy call's input in *x / *len (error cleared, carry assembled); returns its frames, 0: nothing to do */
+int af_pitch_legacy_input(AfPitchFrames *f, const float *data, int dataLength, const float **x, int *len);
+void af_pitch_frames_free(AfPitchFrames *f);                       /* the pipe and the carry */
+
 /* ---------------- setup-time tables (host/af_window.c, af_filterbank.c, ...) ---------------- */
 int af_window_symmetric(int windowType, int length, const float *value, double *out);
 int af_window_fft(int windowType, int length, float *out);

@@ -1,8 +1,9 @@
 /* af_pitch_ncf_cep.c -- PitchNCFObj and PitchCEPObj of the C ABI (host C; compute = kernels/pitch_ncf_cep.cu, one launch
  * per staging chunk).  Interface spec: include/mir/_pitch_{ncf,cep}.h, behaviour src/mir/_pitch_{ncf,cep}.c (restated in
- * include/afb200_pitch_{ncf,cep}.h).  The two objects share one core: the parameter rules, the window, the streaming
- * carry and the staging pipe; they differ in the window rule, the refusals and the kernel's mode.  The reference keeps
- * an FFT object, five 2n-float buffers and a timeLength x 2n matrix per object. */
+ * include/afb200_pitch_{ncf,cep}.h).  The parameter rules, the frame count, the streaming carry and the staging pipe are
+ * the pitch trackers' common core (af_pitch_frames.c); the two objects add the window, uploaded at the first compute
+ * call, and differ in the window rule, the refusals and the kernel's mode.  The reference keeps an FFT object, five
+ * 2n-float buffers and a timeLength x 2n matrix per object. */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -10,11 +11,9 @@
 #include "../af_internal.h"
 
 typedef struct {
-    int mode, samplate, log2n, n, slideLength, isContinue, isDebug;
-    int minIndex, maxIndex;
+    AfPitchFrames f;
+    int mode, minIndex, maxIndex;
     float *window, *dWindow;      /* host n floats, and its device copy from the first compute call */
-    AfTail tail;
-    AfPipe pipe;
 } PitchLag;
 
 struct OpaquePitchNCF { PitchLag c; };
@@ -22,34 +21,28 @@ struct OpaquePitchCEP { PitchLag c; };
 
 static void lag_free(PitchLag *c) {
     if (!c) return;
-    af_pipe_free(&c->pipe);
-    af_tail_free(&c->tail);
+    af_pitch_frames_free(&c->f);
     af_dev_free(c->dWindow);
     free(c->window);
     free(c);
 }
 
 /* pitchNCFObj_new :77-164 / pitchCEPObj_new :77-166 and their initData; the window rule is the caller's */
-static int lag_new(PitchLag **out, int mode, const char *who, int *samplate, float *lowFre, float *highFre,
-                   int *radix2Exp, int *slideLength, int winType, int *isContinue) {
+static int lag_new(PitchLag **out, int mode, int *samplate, float *lowFre, float *highFre, int *radix2Exp,
+                   int *slideLength, int winType, int *isContinue) {
     af_clear_error();
     *out = NULL;
-    /* in the reference's order: highFre is checked against the lowFre already taken, and against the integer
-     * samplate/2; a rejected highFre resets both ends to 32 / 2000 */
-    const int sr = samplate && *samplate > 0 && *samplate <= 196000 ? *samplate : 32000;
-    float lf = lowFre && *lowFre >= 27 ? *lowFre : 32, hf = 2000;
-    if (highFre) {
-        if (*highFre > lf && *highFre < sr / 2) hf = *highFre;
-        else { lf = 32; hf = 2000; }
-    }
-    const int log2n = radix2Exp && *radix2Exp >= 1 && *radix2Exp <= 30 ? *radix2Exp : 12;
-    const int maxExp = mode == AF_PITCH_NCF ? AFB200_PITCH_NCF_MAX_EXP : AFB200_PITCH_CEP_MAX_EXP;
-    if (log2n > maxExp) {
-        af_fail(-2, "%s: radix2Exp=%d; the largest supported is %d (one frame's 2n-point transform is held in shared "
-                "memory)", who, log2n, maxExp);
+    static const AfPitchRules rules[2] = {
+        {"pitchNCFObj_new", AFB200_PITCH_NCF_MAX_EXP, "one frame's 2n-point transform is held in shared memory", 32,
+         2000, 2000},
+        {"pitchCEPObj_new", AFB200_PITCH_CEP_MAX_EXP, "one frame's 2n-point transform is held in shared memory", 32,
+         2000, 2000}};
+    const char *who = rules[mode].who;
+    AfPitchFrames f;
+    float lf, hf;
+    if (af_pitch_frames_init(&f, &lf, &hf, &rules[mode], samplate, lowFre, highFre, radix2Exp, slideLength, isContinue))
         return -2;
-    }
-    const int n = 1 << log2n;
+    const int sr = f.samplate, n = f.n;
     /* initData: float quotients, rounded by roundf */
     const int minIndex = (int)roundf(sr / hf), maxIndex = (int)roundf(sr / lf);
     if (mode == AF_PITCH_NCF && maxIndex >= n) {
@@ -75,26 +68,12 @@ static int lag_new(PitchLag **out, int mode, const char *who, int *samplate, flo
     PitchLag *c = (PitchLag *)calloc(1, sizeof(PitchLag));
     if (c) c->window = (float *)malloc(sizeof(float) * (size_t)n);
     if (!c || !c->window || af_window_fft(winType, n, c->window)) { lag_free(c); return -1; }
+    c->f = f;
     c->mode = mode;
-    c->samplate = sr;
-    c->log2n = log2n;
-    c->n = n;
-    c->slideLength = slideLength && *slideLength > 0 ? *slideLength : n / 4;
-    if (c->slideLength < 1) c->slideLength = 1;                 /* n/4 at n = 2: the reference divides by zero */
-    c->isContinue = isContinue ? *isContinue : 0;
     c->minIndex = minIndex;
     c->maxIndex = maxIndex;
     *out = c;
     return 0;
-}
-
-static int frames(const PitchLag *c, int dataLength) {
-    return dataLength < c->n ? 0 : (dataLength - c->n) / c->slideLength + 1;
-}
-
-static int lag_time_length(const PitchLag *c, int dataLength) {
-    if (!c) return 0;
-    return frames(c, c->isContinue ? dataLength + c->tail.length : dataLength);
 }
 
 typedef struct { const PitchLag *c; int dataLength, timeLength; } LagCall;
@@ -105,35 +84,29 @@ static int lag_chunk(void *ctx, int nb, float *const *d, void *st) {
     const PitchLag *c = k->c;
     AfPitchLagArgs a;
     a.data = d[0]; a.window = c->dWindow; a.fre = d[1];
-    a.mode = c->mode; a.log2n = c->log2n; a.minIndex = c->minIndex; a.maxIndex = c->maxIndex; a.samplate = c->samplate;
-    a.dataLength = k->dataLength; a.hop = c->slideLength; a.timeLength = k->timeLength; a.batch = nb;
+    a.mode = c->mode; a.log2n = c->f.log2n; a.minIndex = c->minIndex; a.maxIndex = c->maxIndex;
+    a.samplate = c->f.samplate;
+    a.dataLength = k->dataLength; a.hop = c->f.slideLength; a.timeLength = k->timeLength; a.batch = nb;
     return af_launch_pitch_ncf_cep(&a, st);
 }
 
 static int lag_batch(PitchLag *c, const char *who, const float *data, int dataLength, int batch, float *freArr,
                      int memKind, void *stream) {
-    const int T = c && dataLength > 0 ? frames(c, dataLength) : 0;
-    if (!c || !data || (!freArr && T > 0 && batch > 0) || dataLength <= 0 || batch < 0)   /* freArr may be NULL when empty */
-        return af_fail(AF_ERR_ARG, "%s: bad argument", who);
-    af_clear_error();
-    int rc = af_device_ready();
-    if (rc || (!c->dWindow && (rc = af_dev_upload((void **)&c->dWindow, c->window, sizeof(float) * (size_t)c->n))))
+    int T, rc = af_pitch_batch_begin(c ? &c->f : NULL, who, data, dataLength, batch, freArr, &T);
+    if (rc || !T || (!c->dWindow && (rc = af_dev_upload((void **)&c->dWindow, c->window,
+                                                        sizeof(float) * (size_t)c->f.n))))
         return rc;
-    if (batch == 0 || T == 0) return AF_OK;
     LagCall k = {c, dataLength, T};
     const AfPlane pl[2] = {{data, (size_t)dataLength, AF_IN, 0}, {freArr, (size_t)T, AF_OUT, 0}};
-    return af_run_batch(&c->pipe, memKind, stream, lag_chunk, &k, pl, 2, batch, AF_PIPE_CHUNK_BYTES);
+    return af_run_batch(&c->f.pipe, memKind, stream, lag_chunk, &k, pl, 2, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 /* pitchNCFObj_pitch :358-378 / pitchCEPObj_pitch :360-379 */
 static void lag_pitch(PitchLag *c, const char *who, float *dataArr, int dataLength, float *freArr) {
-    if (!c) return;
-    af_clear_error();
-    if (!dataArr || dataLength <= 0) return;
-    const float *x = dataArr;
-    if (c->isContinue && !af_tail_assemble(&c->tail, c->n, c->slideLength, dataArr, dataLength, &x, &dataLength)) return;
-    if (!freArr || frames(c, dataLength) == 0) return;
-    lag_batch(c, who, x, dataLength, 1, freArr, AFB200_MEM_HOST, NULL);
+    const float *x;
+    int len;
+    if (af_pitch_legacy_input(c ? &c->f : NULL, dataArr, dataLength, &x, &len) && freArr)
+        lag_batch(c, who, x, len, 1, freArr, AFB200_MEM_HOST, NULL);
 }
 
 /* ---- PitchNCFObj: any window, Rect by default ---- */
@@ -142,17 +115,17 @@ int pitchNCFObj_new(PitchNCFObj *pitchNCFObj, int *samplate, float *lowFre, floa
                     int *slideLength, WindowType *windowType, int *isContinue) {
     if (!pitchNCFObj) return -1;
     PitchLag *c;
-    const int rc = lag_new(&c, AF_PITCH_NCF, "pitchNCFObj_new", samplate, lowFre, highFre, radix2Exp, slideLength,
+    const int rc = lag_new(&c, AF_PITCH_NCF, samplate, lowFre, highFre, radix2Exp, slideLength,
                            windowType ? (int)*windowType : Window_Rect, isContinue);
     *pitchNCFObj = (PitchNCFObj)c;
     return rc;
 }
 
-int pitchNCFObj_calTimeLength(PitchNCFObj s, int dataLength) { return lag_time_length(s ? &s->c : NULL, dataLength); }
-
-void pitchNCFObj_enableDebug(PitchNCFObj s, int isDebug) {
-    if (s) s->c.isDebug = isDebug;
+int pitchNCFObj_calTimeLength(PitchNCFObj s, int dataLength) {
+    return af_pitch_time_length(s ? &s->c.f : NULL, dataLength);
 }
+
+void pitchNCFObj_enableDebug(PitchNCFObj s, int isDebug) { (void)s; (void)isDebug; }
 
 int pitchNCFObj_pitchBatch(PitchNCFObj s, const float *data, int dataLength, int batch, float *freArr, int memKind,
                            void *stream) {
@@ -171,17 +144,17 @@ int pitchCEPObj_new(PitchCEPObj *pitchCEPObj, int *samplate, float *lowFre, floa
                     int *slideLength, WindowType *windowType, int *isContinue) {
     if (!pitchCEPObj) return -1;
     PitchLag *c;
-    const int rc = lag_new(&c, AF_PITCH_CEP, "pitchCEPObj_new", samplate, lowFre, highFre, radix2Exp, slideLength,
+    const int rc = lag_new(&c, AF_PITCH_CEP, samplate, lowFre, highFre, radix2Exp, slideLength,
                            windowType && *windowType <= Window_Hamm ? (int)*windowType : Window_Hamm, isContinue);
     *pitchCEPObj = (PitchCEPObj)c;
     return rc;
 }
 
-int pitchCEPObj_calTimeLength(PitchCEPObj s, int dataLength) { return lag_time_length(s ? &s->c : NULL, dataLength); }
-
-void pitchCEPObj_enableDebug(PitchCEPObj s, int isDebug) {
-    if (s) s->c.isDebug = isDebug;
+int pitchCEPObj_calTimeLength(PitchCEPObj s, int dataLength) {
+    return af_pitch_time_length(s ? &s->c.f : NULL, dataLength);
 }
+
+void pitchCEPObj_enableDebug(PitchCEPObj s, int isDebug) { (void)s; (void)isDebug; }
 
 int pitchCEPObj_pitchBatch(PitchCEPObj s, const float *data, int dataLength, int batch, float *freArr, int memKind,
                            void *stream) {

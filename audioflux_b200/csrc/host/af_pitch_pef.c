@@ -1,8 +1,9 @@
 /* af_pitch_pef.c -- PitchPEFObj of the C ABI (host C; compute = kernels/pitch_pef.cu, one launch per staging chunk).
  * Interface spec: include/mir/_pitch_pef.h, behaviour src/mir/_pitch_pef.c (restated in include/afb200_pitch_pef.h).
  * The object builds its tables in float as the reference does, and the filter's spectrum at the kernel's transform
- * length in double, once; they are uploaded at the first compute call.  The reference keeps two FFT objects and
- * timeLength x 8n-float matrices. */
+ * length in double, once; they are uploaded at the first compute call.  The parameter rules, the frame count, the
+ * streaming carry and the staging pipe are the pitch trackers' common core (af_pitch_frames.c).  The reference keeps
+ * two FFT objects and timeLength x 8n-float matrices. */
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -10,13 +11,14 @@
 #include "../af_internal.h"
 
 struct OpaquePitchPEF {
-    int samplate, log2n, n, slideLength, isContinue;
+    AfPitchFrames f;
     int minIndex, maxIndex, padNum, log2L;
     float *tables;        /* host, AF_PEF_TABLE_FLOATS(n, L) (af_internal.h) */
     float *dTables;
-    AfTail tail;
-    AfPipe pipe;
 };
+
+static const AfPitchRules RULES = {"pitchPEFObj_new", AFB200_PITCH_PEF_MAX_EXP,
+                                   "one frame's transforms are held in shared memory", 32, 2000, 2000};
 
 /* __vlinspace (src/vector/flux_vector.c:2145), type 0 */
 static void linspace_ref(float start, float stop, int length, float *out) {
@@ -39,7 +41,7 @@ static double dsum(const float *v, int n) {                   /* __vsum: a doubl
 /* __pitchPEFObj_initData (:428-522) and __pitchPEFObj_calEstimateFilter (:696-785); filter gets n floats */
 static int build_tables(PitchPEFObj s, int winType, float lowFre, float highFre, float cutFre, float alpha, float beta,
                         float gamma, float *filter) {
-    const int n = s->n, sr2 = s->samplate / 2;
+    const int n = s->f.n, sr2 = s->f.samplate / 2;
     float *win = s->tables, *lin = s->tables + AF_PEF_LIN(n), *lg = s->tables + AF_PEF_LOG(n);
     float *bw = s->tables + AF_PEF_BW(n);
     int *idx = (int *)(s->tables + AF_PEF_IDX(n));
@@ -108,35 +110,22 @@ int pitchPEFObj_new(PitchPEFObj *pitchPEFObj, int *samplate, float *lowFre, floa
     af_clear_error();
     if (!pitchPEFObj) return -1;
     *pitchPEFObj = NULL;
-    /* :135-204, in the reference's order: highFre is checked against the lowFre already taken */
-    const int sr = samplate && *samplate > 0 && *samplate <= 196000 ? *samplate : 32000;
-    float lf = lowFre && *lowFre >= 27 ? *lowFre : 32, hf = 2000, cf = 4000;
-    if (highFre) {
-        if (*highFre > lf && *highFre < sr / 2) hf = *highFre;
-        else { lf = 32; hf = 2000; }
-    }
-    if (cutFre) cf = *cutFre >= hf ? *cutFre : hf;
-    const int log2n = radix2Exp && *radix2Exp >= 1 && *radix2Exp <= 30 ? *radix2Exp : 12;
+    /* :135-204 */
+    AfPitchFrames f;
+    float lf, hf;
+    if (af_pitch_frames_init(&f, &lf, &hf, &RULES, samplate, lowFre, highFre, radix2Exp, slideLength, isContinue))
+        return -2;
+    const int sr = f.samplate, log2n = f.log2n, n = f.n;
+    const float cf = !cutFre ? 4000 : *cutFre >= hf ? *cutFre : hf;
     const int wt = windowType ? (int)*windowType : Window_Hamm;
     const float al = alpha && *alpha > 0 ? *alpha : 10, be = beta && *beta > 0 ? *beta : 0.5f,
                 ga = gamma && *gamma > 1 ? *gamma : 1.8f;
-    if (log2n > AFB200_PITCH_PEF_MAX_EXP) {
-        af_fail(-2, "pitchPEFObj_new: radix2Exp=%d; the largest supported is %d (one frame's transforms are held in "
-                "shared memory)", log2n, AFB200_PITCH_PEF_MAX_EXP);
-        return -2;
-    }
-    const int n = 1 << log2n;
     PitchPEFObj s = (PitchPEFObj)calloc(1, sizeof(struct OpaquePitchPEF));
     float *filter = (float *)malloc(sizeof(float) * (size_t)n);
     /* the largest table: L = 4n */
     if (s) s->tables = (float *)calloc(AF_PEF_TABLE_FLOATS(n, 4 * n), sizeof(float));
     if (!s || !filter || !s->tables) { free(filter); pitchPEFObj_free(s); return -1; }
-    s->samplate = sr;
-    s->log2n = log2n;
-    s->n = n;
-    s->slideLength = slideLength && *slideLength > 0 ? *slideLength : n / 4;
-    if (s->slideLength < 1) s->slideLength = 1;                 /* n/4 at n = 2: the reference divides by zero */
-    s->isContinue = isContinue ? *isContinue : 0;
+    s->f = f;
     if (build_tables(s, wt, lf, hf, cf, al, be, ga, filter)) { free(filter); pitchPEFObj_free(s); return -1; }
     int rc = 0;
     if (s->minIndex < 0 || s->maxIndex <= s->minIndex) {
@@ -162,13 +151,8 @@ int pitchPEFObj_new(PitchPEFObj *pitchPEFObj, int *samplate, float *lowFre, floa
     return 0;
 }
 
-static int frames(PitchPEFObj s, int dataLength) {
-    return dataLength < s->n ? 0 : (dataLength - s->n) / s->slideLength + 1;
-}
-
 int pitchPEFObj_calTimeLength(PitchPEFObj s, int dataLength) {
-    if (!s) return 0;
-    return frames(s, s->isContinue ? dataLength + s->tail.length : dataLength);
+    return af_pitch_time_length(s ? &s->f : NULL, dataLength);
 }
 
 void pitchPEFObj_setFilterParams(PitchPEFObj s, float alpha, float beta, float gamma) {
@@ -185,42 +169,33 @@ static int pef_chunk(void *ctx, int nb, float *const *d, void *st) {
     const PitchPEFObj s = c->s;
     AfPitchPefArgs a;
     a.data = d[0]; a.tables = s->dTables; a.fre = d[1];
-    a.log2n = s->log2n; a.log2L = s->log2L; a.padNum = s->padNum; a.minIndex = s->minIndex; a.maxIndex = s->maxIndex;
-    a.dataLength = c->dataLength; a.hop = s->slideLength; a.timeLength = c->timeLength; a.batch = nb;
+    a.log2n = s->f.log2n; a.log2L = s->log2L; a.padNum = s->padNum; a.minIndex = s->minIndex; a.maxIndex = s->maxIndex;
+    a.dataLength = c->dataLength; a.hop = s->f.slideLength; a.timeLength = c->timeLength; a.batch = nb;
     return af_launch_pitch_pef(&a, st);
 }
 
 int pitchPEFObj_pitchBatch(PitchPEFObj s, const float *data, int dataLength, int batch, float *freArr, int memKind,
                            void *stream) {
-    const int T = s && dataLength > 0 ? frames(s, dataLength) : 0;
-    if (!s || !data || (!freArr && T > 0 && batch > 0) || dataLength <= 0 || batch < 0)   /* freArr may be NULL when empty */
-        return af_fail(AF_ERR_ARG, "pitchPEFObj_pitchBatch: bad argument");
-    af_clear_error();
-    int rc = af_device_ready();
-    if (rc || (!s->dTables && (rc = af_dev_upload((void **)&s->dTables, s->tables,
-                                                  sizeof(float) * AF_PEF_TABLE_FLOATS(s->n, 1 << s->log2L)))))
+    int T, rc = af_pitch_batch_begin(s ? &s->f : NULL, "pitchPEFObj_pitchBatch", data, dataLength, batch, freArr, &T);
+    if (rc || !T || (!s->dTables && (rc = af_dev_upload((void **)&s->dTables, s->tables,
+                                                        sizeof(float) * AF_PEF_TABLE_FLOATS(s->f.n, 1 << s->log2L)))))
         return rc;
-    if (batch == 0 || T == 0) return AF_OK;
     PefCall c = {s, dataLength, T};
     const AfPlane pl[2] = {{data, (size_t)dataLength, AF_IN, 0}, {freArr, (size_t)T, AF_OUT, 0}};
-    return af_run_batch(&s->pipe, memKind, stream, pef_chunk, &c, pl, 2, batch, AF_PIPE_CHUNK_BYTES);
+    return af_run_batch(&s->f.pipe, memKind, stream, pef_chunk, &c, pl, 2, batch, AF_PIPE_CHUNK_BYTES);
 }
 
 /* :233-256 */
 void pitchPEFObj_pitch(PitchPEFObj s, float *dataArr, int dataLength, float *freArr) {
-    if (!s) return;
-    af_clear_error();
-    if (!dataArr || dataLength <= 0) return;
-    const float *x = dataArr;
-    if (s->isContinue && !af_tail_assemble(&s->tail, s->n, s->slideLength, dataArr, dataLength, &x, &dataLength)) return;
-    if (!freArr || frames(s, dataLength) == 0) return;
-    pitchPEFObj_pitchBatch(s, x, dataLength, 1, freArr, AFB200_MEM_HOST, NULL);
+    const float *x;
+    int len;
+    if (af_pitch_legacy_input(s ? &s->f : NULL, dataArr, dataLength, &x, &len) && freArr)
+        pitchPEFObj_pitchBatch(s, x, len, 1, freArr, AFB200_MEM_HOST, NULL);
 }
 
 void pitchPEFObj_free(PitchPEFObj s) {
     if (!s) return;
-    af_pipe_free(&s->pipe);
-    af_tail_free(&s->tail);
+    af_pitch_frames_free(&s->f);
     af_dev_free(s->dTables);
     free(s->tables);
     free(s);

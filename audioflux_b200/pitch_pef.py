@@ -11,11 +11,7 @@ grid points); and ``beta`` = 1 with ``high_fre`` nearest the top grid point, whe
 its buffer."""
 from __future__ import annotations
 
-import ctypes as C
-
-import numpy as np
-
-from .base import Base, Batch, FrameAxis
+from .base import PitchBase, c_float, c_int
 from .types import WindowType, enum_value
 
 __all__ = ["PitchPEF"]
@@ -30,9 +26,10 @@ def _check_filter(alpha, beta, gamma):
         raise ValueError('`gamma` must be greater than 1.')
 
 
-class PitchPEF(FrameAxis, Base):
+class PitchPEF(PitchBase):
     """Per frame of 2**radix2_exp samples: the log-frequency power spectrum, cross-correlated with the pitch estimation
     filter; the frequency of the largest correlation between low_fre and high_fre."""
+    _prefix = "pitchPEFObj"
 
     def __init__(self, samplate=32000, low_fre=32.0, high_fre=2000.0, cut_fre=4000.0, radix2_exp=12, slide_length=1024,
                  window_type=WindowType.HAMM, alpha=10.0, beta=0.5, gamma=1.8, _lib=None):
@@ -53,16 +50,9 @@ class PitchPEF(FrameAxis, Base):
         self.beta = beta
         self.gamma = gamma
         self.is_continue = False
-        f = lambda v: C.byref(C.c_float(float(v)))  # noqa: E731
-        i = lambda v: C.byref(C.c_int(int(v)))      # noqa: E731
-        self._new("pitchPEFObj_new", "pitchPEFObj_free", i(samplate), f(low_fre), f(high_fre), f(cut_fre),
-                  i(radix2_exp), i(slide_length), i(enum_value(window_type)), f(alpha), f(beta), f(gamma),
-                  i(self.is_continue))
-        # the frame: 2**radix2_exp, or the reference's fallback 2**12 outside 1 .. 30
-        self.fft_length = 1 << (int(radix2_exp) if 1 <= radix2_exp <= 30 else 12)
-
-    def cal_time_length(self, data_length):
-        return self._lib.pitchPEFObj_calTimeLength(self._obj, int(data_length))
+        self._open(radix2_exp, c_int(samplate), c_float(low_fre), c_float(high_fre), c_float(cut_fre),
+                   c_int(radix2_exp), c_int(slide_length), c_int(enum_value(window_type)), c_float(alpha),
+                   c_float(beta), c_float(gamma), c_int(self.is_continue))
 
     def set_filter_params(self, alpha, beta, gamma):
         _check_filter(alpha, beta, gamma)
@@ -70,22 +60,3 @@ class PitchPEF(FrameAxis, Base):
         self.alpha = alpha
         self.beta = beta
         self.gamma = gamma
-
-    def pitch_batch(self, data):
-        """data [..., n] (numpy host | torch cuda) -> [..., cal_time_length(n)] float32 of the same kind.  One
-        pitchPEFObj_pitchBatch call for all channels; each row is bit-identical to a legacy call."""
-        b = Batch(data)
-        t = self.cal_time_length(b.n)
-        out = b.alloc(b.rows, t)
-        if b.rows and t:
-            self._call("pitchPEFObj_pitchBatch", b, b.x, b.n, b.rows, out)
-        return b.shaped(out)
-
-    def pitch(self, data_arr):
-        """data_arr [..., n] -> fre_arr [..., time] float32"""
-        data_arr = np.asarray(data_arr, dtype=np.float32, order='C')
-        if data_arr.ndim == 0:
-            raise ValueError('Audio data must have at least one dimension')
-        if data_arr.shape[-1] == 0:
-            raise ValueError('Audio data must not be empty')
-        return self.pitch_batch(data_arr)

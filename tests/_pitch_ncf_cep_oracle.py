@@ -22,10 +22,9 @@ sqrt(2n) ||frame|| of |X_k|, so log |X_k|^2 lies in [2 log(|X_k| - DELTA), 2 log
 |X_k| <= DELTA), widened by the float32 rounding of the power and the log; the cepstrum interval's radius is the mean of
 those radii plus KAPPA times the l2 norm of the log spectrum over sqrt(2n), the inverse transform's own error.  A slot
 whose interval reaches the top slot's is a candidate; the frame's arg-max is undetermined when there are several."""
-import ctypes as C
-
 import numpy as np
 
+from _pitch_c import c_free, c_new, c_pitch, signal, time_length
 from oracle import af_oracle as O
 
 W_RECT, W_HANN, W_HAMM, W_BLACKMAN, W_KAISER = O.W_RECT, O.W_HANN, O.W_HAMM, O.W_BLACKMAN, O.W_KAISER
@@ -33,7 +32,6 @@ f32 = np.float32
 KAPPA = 4e-6
 U = 2.0 ** -24
 KINDS = ("ncf", "cep")
-PREFIX = {"ncf": "pitchNCFObj", "cep": "pitchCEPObj"}
 
 
 def params(kind, sr=None, lf=None, hf=None, r2=None, slide=None, wt=None):
@@ -66,10 +64,6 @@ def params(kind, sr=None, lf=None, hf=None, r2=None, slide=None, wt=None):
     if ma < mi:
         return dict(p, status=-3)
     return dict(p, status=0)
-
-
-def time_length(length, n, hop):
-    return 0 if length < n else (length - n) // hop + 1
 
 
 def _frames(x, p):
@@ -160,40 +154,7 @@ def agree(got, want, cands, p):
     return True, alt
 
 
-# ---- test signals ----
-
-def signal(kind, length, sr, seed):
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    if kind == "silence":
-        x = np.zeros(length)
-    elif kind == "dc":
-        x = np.full(length, 0.5)
-    elif kind == "alt":                         # +1, -1, ...
-        x = np.where(np.arange(length) % 2, -1.0, 1.0)
-    elif kind == "noise":
-        x = 0.1 * rng.standard_normal(length)
-    elif kind == "tones":                       # 220 Hz and five overtones, a little noise
-        x = sum(0.3 / h * np.sin(2 * np.pi * 220 * h * t + h) for h in range(1, 7)) + 0.01 * rng.standard_normal(length)
-    elif kind == "low":                         # 95 Hz and its overtones, a little noise
-        x = sum(0.4 / h * np.sin(2 * np.pi * 95 * h * t + h) for h in range(1, 9)) + 0.01 * rng.standard_normal(length)
-    elif kind == "chirp":                       # a harmonic tone gliding from 120 to 700 Hz, in noise
-        f = 120 + (700 - 120) * t / max(t[-1], 1e-9)
-        ph = 2 * np.pi * np.cumsum(f) / sr
-        x = sum(0.4 / h * np.sin(h * ph) for h in range(1, 5)) + 0.05 * rng.standard_normal(length)
-    elif kind == "gaps":                        # tones with runs of silence longer than a frame
-        x = signal("tones", length, sr, seed).astype(np.float64)
-        for a in range(length // 5, length, 2 * length // 5):
-            x[a:a + length // 6] = 0.0
-    elif kind == "nan":                         # noise with one NaN sample
-        x = 0.1 * rng.standard_normal(length)
-        x[length // 2] = np.nan
-    elif kind == "tone4638":                    # 32000 / 69 Hz: every correlation between lags 33 and 36 is negative
-        x = np.sin(2 * np.pi * (32000 / 69) * t)
-    else:
-        raise ValueError(kind)
-    return np.asarray(x, f32)
-
+# ---- cases ----
 
 def cases(kind):
     """[(name, dict(ctor=dict(...), length, kind))]: ctor arguments left out are passed as NULL"""
@@ -218,9 +179,9 @@ def cases(kind):
     add("sr_fallback", 32000, sr=0, r2=12, slide=1024)
     add("narrow", 32000, lf=150.0, hf=400.0, r2=12, slide=1024)
     add("one_lag", 32000, lf=1000.0, hf=1001.0, r2=12, slide=1024)
-    for sig in ("silence", "dc", "alt", "noise", "low", "chirp", "gaps", "nan"):
-        add(f"sig_{sig}", 48000, sig=sig, sr=32000, r2=12, slide=1024)
-    add("sig_chirp_r13", 8192 + 30 * 2048, sig="chirp", sr=44100, r2=13, slide=2048)
+    for sig in ("silence", "dc", "alt", "noise", "low", "chirp", "gaps", "nan"):       # sig_chirp: the glide
+        add(f"sig_{sig}", 48000, sig="glide" if sig == "chirp" else sig, sr=32000, r2=12, slide=1024)
+    add("sig_chirp_r13", 8192 + 30 * 2048, sig="glide", sr=44100, r2=13, slide=2048)
     add("sentinel", 32000, sig="tone4638", sr=32000, lf=900.0, hf=1000.0, r2=12, slide=1024)
     add("r5", 600, sr=8000, lf=300.0, hf=1000.0, r2=5, slide=16, sig="noise")
     return out
@@ -238,48 +199,9 @@ def oracle_case(kind, name, kw):
     return pitch(case_signal(kind, name, kw), case_params(kind, kw))
 
 
-# ---- ctypes drivers (either library) ----
-
-def c_new(lib, kind, sr=None, lf=None, hf=None, r2=None, slide=None, wt=None, cont=None):
-    def ip(v):
-        return None if v is None else C.byref(C.c_int(int(v)))
-
-    def fp(v):
-        return None if v is None else C.byref(C.c_float(float(v)))
-    obj = C.c_void_p()
-    st = getattr(lib, PREFIX[kind] + "_new")(C.byref(obj), ip(sr), fp(lf), fp(hf), ip(r2), ip(slide), ip(wt), ip(cont))
-    return st, obj
-
-
-def c_time_length(lib, kind, obj, n):
-    return getattr(lib, PREFIX[kind] + "_calTimeLength")(obj, n)
-
-
-def c_free(lib, kind, obj):
-    getattr(lib, PREFIX[kind] + "_free")(obj)
-
-
-def c_pitch(lib, kind, obj, x, fill=0.0, extra=0):
-    """pitch -> the output buffer of T + extra floats (T from calTimeLength before the call), which started as `fill`"""
-    x = np.ascontiguousarray(x, f32)
-    T = c_time_length(lib, kind, obj, x.size)
-    out = np.full(T + extra, fill, f32)
-    getattr(lib, PREFIX[kind] + "_pitch")(obj, x.ctypes.data, x.size, out.ctypes.data)
-    return out
-
-
 def c_case(lib, kind, name, kw):
     st, obj = c_new(lib, kind, **kw["ctor"])
     assert st == 0, (kind, name, st)
     out = c_pitch(lib, kind, obj, case_signal(kind, name, kw))
     c_free(lib, kind, obj)
     return out
-
-
-def c_stream(lib, kind, obj, x, pieces):
-    """pitch over consecutive pieces of x (isContinue objects) -> the frames of all calls, concatenated"""
-    outs, start = [], 0
-    for size in pieces:
-        outs.append(c_pitch(lib, kind, obj, x[start:start + size]))
-        start += size
-    return np.concatenate(outs)

@@ -28,6 +28,7 @@ import math
 
 import numpy as np
 
+from _pitch_c import c_free, c_new, c_pitch, signal, time_length
 from oracle import af_oracle as O
 
 W_RECT, W_HANN, W_HAMM = O.W_RECT, O.W_HANN, O.W_HAMM
@@ -111,10 +112,6 @@ def params(sr=None, lf=None, hf=None, cf=None, r2=None, slide=None, wt=None, alp
     return dict(p, status=0)
 
 
-def time_length(length, n, hop):
-    return 0 if length < n else (length - n) // hop + 1
-
-
 def correlations(x, p):
     """per frame, c over the lags min_index .. max_index and the Cauchy-Schwarz scale ||s|| ||filter||, float64"""
     n, hop = p["n"], p["slide"]
@@ -175,29 +172,7 @@ def agree(got, want, cands, p):
     return True, alt
 
 
-# ---- test signals ----
-
-def signal(kind, length, sr, seed):
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    if kind == "silence":
-        x = np.zeros(length)
-    elif kind == "dc":
-        x = np.full(length, 0.5)
-    elif kind == "noise":
-        x = 0.1 * rng.standard_normal(length)
-    elif kind == "tones":                       # 220 Hz and five overtones, a little noise
-        x = sum(0.3 / h * np.sin(2 * np.pi * 220 * h * t + h) for h in range(1, 7)) + 0.01 * rng.standard_normal(length)
-    elif kind == "missing":                     # overtones 2 .. 6 of 180 Hz without the fundamental
-        x = sum(0.3 / h * np.sin(2 * np.pi * 180 * h * t + h) for h in range(2, 7)) + 0.01 * rng.standard_normal(length)
-    elif kind == "glide":                       # a harmonic tone gliding from 120 to 700 Hz, in noise
-        f = 120 + (700 - 120) * t / max(t[-1], 1e-9)
-        ph = 2 * np.pi * np.cumsum(f) / sr
-        x = sum(0.4 / h * np.sin(h * ph) for h in range(1, 5)) + 0.05 * rng.standard_normal(length)
-    else:
-        raise ValueError(kind)
-    return np.asarray(x, f32)
-
+# ---- cases ----
 
 def cases():
     """[(name, dict(ctor=dict(...), length, kind))]: ctor arguments left out are passed as NULL"""
@@ -249,46 +224,9 @@ def oracle_case(name, kw):
     return pitch(case_signal(name, kw), p)
 
 
-# ---- ctypes drivers (either library) ----
-
-_INTS = ("sr", "r2", "slide", "wt", "cont")
-
-
-def c_new(lib, sr=None, lf=None, hf=None, cf=None, r2=None, slide=None, wt=None, alpha=None, beta=None, gamma=None,
-          cont=None):
-    def ip(v):
-        return None if v is None else C.byref(C.c_int(int(v)))
-
-    def fp(v):
-        return None if v is None else C.byref(C.c_float(float(v)))
-    obj = C.c_void_p()
-    st = lib.pitchPEFObj_new(C.byref(obj), ip(sr), fp(lf), fp(hf), fp(cf), ip(r2), ip(slide), ip(wt), fp(alpha),
-                             fp(beta), fp(gamma), ip(cont))
-    return st, obj
-
-
-def c_pitch(lib, obj, x, fill=0.0, extra=0):
-    """pitchPEFObj_pitch -> the output buffer of T + extra floats (T from calTimeLength before the call), which started
-    as `fill`"""
-    x = np.ascontiguousarray(x, f32)
-    T = lib.pitchPEFObj_calTimeLength(obj, x.size)
-    out = np.full(T + extra, fill, f32)
-    lib.pitchPEFObj_pitch(obj, x.ctypes.data, x.size, out.ctypes.data)
-    return out
-
-
 def c_case(lib, name, kw):
-    st, obj = c_new(lib, **kw["ctor"])
+    st, obj = c_new(lib, "pef", **kw["ctor"])
     assert st == 0, (name, st)
-    out = c_pitch(lib, obj, case_signal(name, kw))
-    lib.pitchPEFObj_free(obj)
+    out = c_pitch(lib, "pef", obj, case_signal(name, kw))
+    c_free(lib, "pef", obj)
     return out
-
-
-def c_stream(lib, obj, x, pieces):
-    """pitchPEFObj_pitch over consecutive pieces of x (isContinue objects) -> the frames of all calls, concatenated"""
-    outs, start = [], 0
-    for size in pieces:
-        outs.append(c_pitch(lib, obj, x[start:start + size]))
-        start += size
-    return np.concatenate(outs)

@@ -23,6 +23,8 @@ import ctypes as C
 
 import numpy as np
 
+from _pitch_c import c_free, c_new, c_pitch, signal, time_length
+
 f32 = np.float32
 KAPPA = 4e-6
 U = 2.0 ** -24                    # float32 unit roundoff
@@ -51,10 +53,6 @@ def params(sr=None, lf=None, hf=None, r2=None, slide=None, auto=None):
     if mi < 1 or ma < mi:
         return dict(p, status=-3)
     return dict(p, status=0)
-
-
-def time_length(length, n, hop):
-    return 0 if length < n else (length - n) // hop + 1
 
 
 def _frames(x, p):
@@ -238,33 +236,7 @@ def check_troughs(mfre, mtrough, lens, frames, p):
     return True, ""
 
 
-# ---- test signals ----
-
-def signal(kind, length, sr, seed):
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    if kind == "silence":
-        x = np.zeros(length)
-    elif kind == "noise":
-        x = 0.1 * rng.standard_normal(length)
-    elif kind == "tones":                       # 220 Hz and five overtones, a little noise
-        x = sum(0.3 / h * np.sin(2 * np.pi * 220 * h * t + h) for h in range(1, 7)) + 0.01 * rng.standard_normal(length)
-    elif kind == "missing":                     # overtones 2 .. 6 of 180 Hz without the fundamental
-        x = sum(0.3 / h * np.sin(2 * np.pi * 180 * h * t + h) for h in range(2, 7)) + 0.01 * rng.standard_normal(length)
-    elif kind == "glide":                       # a harmonic tone gliding from 120 to 700 Hz, in noise
-        f = 120 + (700 - 120) * t / max(t[-1], 1e-9)
-        ph = 2 * np.pi * np.cumsum(f) / sr
-        x = sum(0.4 / h * np.sin(h * ph) for h in range(1, 5)) + 0.05 * rng.standard_normal(length)
-    elif kind == "half":                        # the tone in the second half only
-        x = np.where(t >= t[-1] / 2, signal("tones", length, sr, seed), 0.0)
-    elif kind == "quiet":                       # near the 1e-6 clamps of r and e2
-        x = 3e-4 * signal("tones", length, sr, seed)
-    elif kind == "loud":
-        x = 3e3 * signal("tones", length, sr, seed)
-    else:
-        raise ValueError(kind)
-    return np.asarray(x, f32)
-
+# ---- cases ----
 
 def cases():
     """[(name, dict(ctor=dict(...), length, kind, thresh))]: ctor arguments left out are passed as NULL"""
@@ -318,27 +290,6 @@ def oracle_case(name, kw):
 
 # ---- ctypes drivers (either library) ----
 
-def c_new(lib, sr=None, lf=None, hf=None, r2=None, slide=None, auto=None, cont=None):
-    def ip(v):
-        return None if v is None else C.byref(C.c_int(int(v)))
-
-    def fp(v):
-        return None if v is None else C.byref(C.c_float(float(v)))
-    obj = C.c_void_p()
-    st = lib.pitchYINObj_new(C.byref(obj), ip(sr), fp(lf), fp(hf), ip(r2), ip(slide), ip(auto), ip(cont))
-    return st, obj
-
-
-def c_pitch(lib, obj, x, fill=0.0, extra=0):
-    """pitchYINObj_pitch -> (fre, value1, value2) buffers of T + extra floats (T from calTimeLength before the call),
-    which started as `fill`"""
-    x = np.ascontiguousarray(x, f32)
-    T = lib.pitchYINObj_calTimeLength(obj, x.size)
-    out = [np.full(T + extra, fill, f32) for _ in range(3)]
-    lib.pitchYINObj_pitch(obj, x.ctypes.data, x.size, *(o.ctypes.data for o in out))
-    return tuple(out)
-
-
 def c_troughs(lib, obj, T):
     """copies of getTroughData's arrays for T frames -> (mFre [T, mLen], mTrough [T, mLen], lens [T])"""
     fp, tp, lp = C.POINTER(C.c_float)(), C.POINTER(C.c_float)(), C.POINTER(C.c_int)()
@@ -351,22 +302,12 @@ def c_troughs(lib, obj, T):
 
 def c_case(lib, name, kw, fill=0.0):
     """-> (fre, value1, value2, mFre, mTrough, lens)"""
-    st, obj = c_new(lib, **kw["ctor"])
+    st, obj = c_new(lib, "yin", **kw["ctor"])
     assert st == 0, (name, st)
     if kw["thresh"] is not None:
         lib.pitchYINObj_setThresh(obj, C.c_float(kw["thresh"]))
     x = case_signal(name, kw)
-    out = c_pitch(lib, obj, x, fill)
+    out = c_pitch(lib, "yin", obj, x, fill)
     tr = c_troughs(lib, obj, len(out[0]))
-    lib.pitchYINObj_free(obj)
+    c_free(lib, "yin", obj)
     return out + tr
-
-
-def c_stream(lib, obj, x, pieces):
-    """pitchYINObj_pitch over consecutive pieces of x (isContinue objects) -> the three outputs of all calls,
-    concatenated"""
-    outs, start = [], 0
-    for size in pieces:
-        outs.append(c_pitch(lib, obj, x[start:start + size]))
-        start += size
-    return tuple(np.concatenate([o[i] for o in outs]) for i in range(3))

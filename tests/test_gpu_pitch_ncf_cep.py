@@ -8,6 +8,7 @@ libaudioflux_b200.so."""
 import numpy as np
 import pytest
 
+import _pitch_c as PC
 import _pitch_ncf_cep_oracle as PO
 from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
 from test_pitch_ncf_cep_cpu import ALL, CASES, GOLD
@@ -29,8 +30,8 @@ def _check(got, want, cands, p, what, cap=True):
 
 def _batch(lib, kind, o, x, device, fill=7.0):
     b, n = x.shape
-    T = PO.c_time_length(lib, kind, o, n)
-    return run_batch(lib, PO.PREFIX[kind] + "_pitchBatch",
+    T = PC.c_time_length(lib, kind, o, n)
+    return run_batch(lib, PC.prefix(kind) + "_pitchBatch",
                      (o, np.ascontiguousarray(x, np.float32), n, b, Out(np.full((b, T), fill, np.float32))), device)[0]
 
 
@@ -66,43 +67,33 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, kind, name)
     # the batch with host and device pointers: clip 1 is clip 0 reversed and 1000 times louder
     x = PO.case_signal(kind, name, kw)
     xs = np.stack([x, 1000 * x[::-1]])
-    st, o = PO.c_new(product_lib, kind, **kw["ctor"])
-    legacy = [PO.c_pitch(product_lib, kind, o, c) for c in xs]
+    st, o = PC.c_new(product_lib, kind, **kw["ctor"])
+    legacy = [PC.c_pitch(product_lib, kind, o, c) for c in xs]
     assert np.array_equal(legacy[0], got)
     for device in (False, True):
         out = _batch(product_lib, kind, o, xs, device)
         for k in range(2):
             assert np.array_equal(out[k], legacy[k]), (kind, name, device, k)
-    PO.c_free(product_lib, kind, o)
-
-
-def _clips(n, length, sr, seed):
-    """harmonic tones of random f0 (80 .. 600 Hz), some without their fundamental, in noise"""
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    f0 = rng.uniform(80, 600, (n, 1))
-    first = rng.integers(1, 3, (n, 1))
-    x = sum(np.where(first <= h, 0.3 / h, 0.0) * np.sin(2 * np.pi * f0 * h * t + h) for h in range(1, 6))
-    return (x + 0.05 * rng.standard_normal((n, length))).astype(np.float32)
+    PC.c_free(product_lib, kind, o)
 
 
 @gpu
 @pytest.mark.parametrize("kind", PO.KINDS)
 def test_batch_across_chunks(product_lib, cuda_device, kind):
     """200 clips of 160 000 samples: three host staging chunks; host and device batches equal the legacy call"""
-    x = _clips(200, 160000, 32000, 1)
-    st, o = PO.c_new(product_lib, kind, r2=12, slide=1024)
+    x = PC.clips(200, 160000, 32000, 1)
+    st, o = PC.c_new(product_lib, kind, r2=12, slide=1024)
     assert st == 0
     host = _batch(product_lib, kind, o, x, False)
     dev = _batch(product_lib, kind, o, x, True)
     assert np.array_equal(host, dev)
     for c in (0, 1, 95, 96, 97, 191, 192, 199):
-        assert np.array_equal(host[c], PO.c_pitch(product_lib, kind, o, x[c])), c
+        assert np.array_equal(host[c], PC.c_pitch(product_lib, kind, o, x[c])), c
     p = PO.params(kind, r2=12, slide=1024)
     for c in (0, 1):
         want, cands = PO.pitch(x[c], p)
         _check(host[c], want, cands, p, (kind, "chunks", c))
-    PO.c_free(product_lib, kind, o)
+    PC.c_free(product_lib, kind, o)
 
 
 @gpu
@@ -110,22 +101,22 @@ def test_batch_across_chunks(product_lib, cuda_device, kind):
 def test_device_calls_back_to_back(product_lib, cuda_device, kind):
     """calls with different clip counts and lengths queued on one object without a synchronise"""
     import torch
-    st, o = PO.c_new(product_lib, kind, sr=44100, r2=11, slide=512, lf=60.0)
+    st, o = PC.c_new(product_lib, kind, sr=44100, r2=11, slide=512, lf=60.0)
     assert st == 0
     calls = []
     for k, (b, n) in enumerate(((3, 30000), (17, 9000), (1, 2048), (40, 22050), (2, 60000))):
-        x = _clips(b, n, 44100, 10 + k)
+        x = PC.clips(b, n, 44100, 10 + k)
         xd = torch.from_numpy(x).cuda()
-        T = PO.c_time_length(product_lib, kind, o, n)
+        T = PC.c_time_length(product_lib, kind, o, n)
         v = torch.empty((b, T), device="cuda")
-        rc = getattr(product_lib, PO.PREFIX[kind] + "_pitchBatch")(o, dptr(xd), n, b, dptr(v), 1, stream())
+        rc = getattr(product_lib, PC.prefix(kind) + "_pitchBatch")(o, dptr(xd), n, b, dptr(v), 1, stream())
         assert rc == 0, product_lib.afb200_lastError()
         calls.append((x, xd, v))
     torch.cuda.synchronize()
     for x, _, v in calls:
         for k in (0, len(x) - 1):
-            assert np.array_equal(v[k].cpu().numpy(), PO.c_pitch(product_lib, kind, o, x[k]))
-    PO.c_free(product_lib, kind, o)
+            assert np.array_equal(v[k].cpu().numpy(), PC.c_pitch(product_lib, kind, o, x[k]))
+    PC.c_free(product_lib, kind, o)
 
 
 @gpu
@@ -133,21 +124,21 @@ def test_device_calls_back_to_back(product_lib, cuda_device, kind):
 def test_streaming_equals_one_call(product_lib, cuda_device, kind):
     """isContinue: uneven pieces (some shorter than a frame) give the frames of one call over the clip, for a slide
     below n and one above it; a batch call in between neither reads nor moves the carry"""
-    x = PO.signal("chirp", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = PO.c_new(product_lib, kind, sr=16000, r2=r2, slide=slide)
-        want = PO.c_pitch(product_lib, kind, whole, x)
-        st, o = PO.c_new(product_lib, kind, sr=16000, r2=r2, slide=slide, cont=1)
+        st, whole = PC.c_new(product_lib, kind, sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(product_lib, kind, whole, x)
+        st, o = PC.c_new(product_lib, kind, sr=16000, r2=r2, slide=slide, cont=1)
         pieces = (700, 3000, 100, 9000, 1, 27199)
         got, start = [], 0
         for k, size in enumerate(pieces):
-            got.append(PO.c_pitch(product_lib, kind, o, x[start:start + size]))
+            got.append(PC.c_pitch(product_lib, kind, o, x[start:start + size]))
             start += size
             if k == 2:
                 _batch(product_lib, kind, o, np.stack([x, x]), True)
         assert np.array_equal(np.concatenate(got), want), (r2, slide)
-        PO.c_free(product_lib, kind, o)
-        PO.c_free(product_lib, kind, whole)
+        PC.c_free(product_lib, kind, o)
+        PC.c_free(product_lib, kind, whole)
 
 
 @gpu
@@ -156,11 +147,11 @@ def test_launch_count(product_lib, cuda_device, kind):
     """one launch per staging chunk"""
     import torch
     h = CLASSES[kind](radix2_exp=11, slide_length=512)
-    x = _clips(8, 20000, 32000, 3)
+    x = PC.clips(8, 20000, 32000, 3)
     xd = torch.from_numpy(x).cuda()
     assert count_launches(product_lib, lambda: h.pitch_batch(xd), warm=True) == 1
     assert count_launches(product_lib, lambda: h.pitch(x[0]), warm=True) == 1
-    big = _clips(200, 160000, 32000, 4)                  # 64 MB staging chunks: three of them
+    big = PC.clips(200, 160000, 32000, 4)                  # 64 MB staging chunks: three of them
     assert count_launches(product_lib, lambda: h.pitch(big), warm=True) == 3
 
 
@@ -168,14 +159,14 @@ def test_launch_count(product_lib, cuda_device, kind):
 @pytest.mark.parametrize("kind", PO.KINDS)
 def test_refusals_on_device(product_lib, cuda_device, kind):
     """a refused constructor leaves no object; a call with fewer samples than the frame leaves the output untouched"""
-    st, o = PO.c_new(product_lib, kind, r2=15)
+    st, o = PC.c_new(product_lib, kind, r2=15)
     assert st == -2 and not o
-    st, o = PO.c_new(product_lib, kind, r2=8)
+    st, o = PC.c_new(product_lib, kind, r2=8)
     assert st == -3 and not o
-    st, o = PO.c_new(product_lib, kind, r2=10)
-    assert (PO.c_pitch(product_lib, kind, o, np.ones(1000, np.float32), fill=7.0, extra=3) == 7).all()
+    st, o = PC.c_new(product_lib, kind, r2=10)
+    assert (PC.c_pitch(product_lib, kind, o, np.ones(1000, np.float32), fill=7.0, extra=3) == 7).all()
     assert _batch(product_lib, kind, o, np.ones((2, 1000), np.float32), True).size == 0
-    PO.c_free(product_lib, kind, o)
+    PC.c_free(product_lib, kind, o)
 
 
 @gpu
@@ -183,7 +174,7 @@ def test_refusals_on_device(product_lib, cuda_device, kind):
 def test_reference_class_on_b200(raf, cuda_device, kind):
     """the reference's own PitchNCF / PitchCEP class, on the reference build and on libaudioflux_b200.so, per channel
     of a multi-channel array; and this package's class giving the same arrays"""
-    x = _clips(6, 48000, 32000, 7).reshape(2, 3, 48000)
+    x = PC.clips(6, 48000, 32000, 7).reshape(2, 3, 48000)
     name = {"ncf": "PitchNCF", "cep": "PitchCEP"}[kind]
     res = {}
     for which in ("ref", "b200"):

@@ -6,6 +6,7 @@ one launch per chunk; the refusals; and the reference's own PitchPEF class on li
 import numpy as np
 import pytest
 
+import _pitch_c as PC
 import _pitch_pef_oracle as PO
 from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
 from test_pitch_pef_cpu import GOLD
@@ -51,8 +52,8 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     # the batch with host and device pointers: clip 1 is clip 0 reversed and 1000 times louder
     x = PO.case_signal(name, kw)
     xs = np.stack([x, 1000 * x[::-1]])
-    st, o = PO.c_new(product_lib, **kw["ctor"])
-    legacy = [PO.c_pitch(product_lib, o, c) for c in xs]
+    st, o = PC.c_new(product_lib, "pef", **kw["ctor"])
+    legacy = [PC.c_pitch(product_lib, "pef", o, c) for c in xs]
     assert np.array_equal(legacy[0], got)
     for device in (False, True):
         out = _batch(product_lib, o, xs, device)
@@ -61,27 +62,17 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     product_lib.pitchPEFObj_free(o)
 
 
-def _clips(n, length, sr, seed):
-    """harmonic tones of random f0 (80 .. 600 Hz), some without their fundamental, in noise"""
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    f0 = rng.uniform(80, 600, (n, 1))
-    first = rng.integers(1, 3, (n, 1))
-    x = sum(np.where(first <= h, 0.3 / h, 0.0) * np.sin(2 * np.pi * f0 * h * t + h) for h in range(1, 6))
-    return (x + 0.05 * rng.standard_normal((n, length))).astype(np.float32)
-
-
 @gpu
 def test_batch_across_chunks(product_lib, cuda_device):
     """200 clips of 160 000 samples: three host staging chunks; host and device batches equal the legacy call"""
-    x = _clips(200, 160000, 32000, 1)
-    st, o = PO.c_new(product_lib, r2=12, slide=1024)
+    x = PC.clips(200, 160000, 32000, 1)
+    st, o = PC.c_new(product_lib, "pef", r2=12, slide=1024)
     assert st == 0
     host = _batch(product_lib, o, x, False)
     dev = _batch(product_lib, o, x, True)
     assert np.array_equal(host, dev)
     for c in (0, 1, 95, 96, 97, 191, 192, 199):
-        assert np.array_equal(host[c], PO.c_pitch(product_lib, o, x[c])), c
+        assert np.array_equal(host[c], PC.c_pitch(product_lib, "pef", o, x[c])), c
     p = PO.params(r2=12, slide=1024)
     for c in (0, 1):
         want, cands = PO.pitch(x[c], p)
@@ -93,10 +84,10 @@ def test_batch_across_chunks(product_lib, cuda_device):
 def test_device_calls_back_to_back(product_lib, cuda_device):
     """calls with different clip counts and lengths queued on one object without a synchronise"""
     import torch
-    st, o = PO.c_new(product_lib, sr=44100, r2=11, slide=512, beta=1.0)
+    st, o = PC.c_new(product_lib, "pef", sr=44100, r2=11, slide=512, beta=1.0)
     calls = []
     for k, (b, n) in enumerate(((3, 30000), (17, 9000), (1, 2048), (40, 22050), (2, 60000))):
-        x = _clips(b, n, 44100, 10 + k)
+        x = PC.clips(b, n, 44100, 10 + k)
         xd = torch.from_numpy(x).cuda()
         T = product_lib.pitchPEFObj_calTimeLength(o, n)
         v = torch.empty((b, T), device="cuda")
@@ -106,7 +97,7 @@ def test_device_calls_back_to_back(product_lib, cuda_device):
     torch.cuda.synchronize()
     for x, _, v in calls:
         for k in (0, len(x) - 1):
-            assert np.array_equal(v[k].cpu().numpy(), PO.c_pitch(product_lib, o, x[k]))
+            assert np.array_equal(v[k].cpu().numpy(), PC.c_pitch(product_lib, "pef", o, x[k]))
     product_lib.pitchPEFObj_free(o)
 
 
@@ -114,15 +105,15 @@ def test_device_calls_back_to_back(product_lib, cuda_device):
 def test_streaming_equals_one_call(product_lib, cuda_device):
     """isContinue: uneven pieces (some shorter than a frame) give the frames of one call over the clip, for a slide
     below n and one above it; a batch call in between neither reads nor moves the carry"""
-    x = PO.signal("glide", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = PO.c_new(product_lib, sr=16000, r2=r2, slide=slide)
-        want = PO.c_pitch(product_lib, whole, x)
-        st, o = PO.c_new(product_lib, sr=16000, r2=r2, slide=slide, cont=1)
+        st, whole = PC.c_new(product_lib, "pef", sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(product_lib, "pef", whole, x)
+        st, o = PC.c_new(product_lib, "pef", sr=16000, r2=r2, slide=slide, cont=1)
         pieces = (700, 3000, 100, 9000, 1, 27199)
         got, start = [], 0
         for k, size in enumerate(pieces):
-            got.append(PO.c_pitch(product_lib, o, x[start:start + size]))
+            got.append(PC.c_pitch(product_lib, "pef", o, x[start:start + size]))
             start += size
             if k == 2:
                 _batch(product_lib, o, np.stack([x, x]), True)
@@ -136,21 +127,21 @@ def test_launch_count(product_lib, cuda_device):
     """one launch per staging chunk"""
     import torch
     h = af.PitchPEF(radix2_exp=11, slide_length=512)
-    x = _clips(8, 20000, 32000, 3)
+    x = PC.clips(8, 20000, 32000, 3)
     xd = torch.from_numpy(x).cuda()
     assert count_launches(product_lib, lambda: h.pitch_batch(xd), warm=True) == 1
     assert count_launches(product_lib, lambda: h.pitch(x[0]), warm=True) == 1
-    big = _clips(200, 160000, 32000, 4)                  # 64 MB staging chunks: three of them
+    big = PC.clips(200, 160000, 32000, 4)                  # 64 MB staging chunks: three of them
     assert count_launches(product_lib, lambda: h.pitch(big), warm=True) == 3
 
 
 @gpu
 def test_refusals_on_device(product_lib, cuda_device):
     """a refused constructor leaves no object; a call with fewer samples than the frame leaves the output untouched"""
-    st, o = PO.c_new(product_lib, r2=14)
+    st, o = PC.c_new(product_lib, "pef", r2=14)
     assert st == -2 and not o
-    st, o = PO.c_new(product_lib, r2=10)
-    assert (PO.c_pitch(product_lib, o, np.ones(1000, np.float32), fill=7.0, extra=3) == 7).all()
+    st, o = PC.c_new(product_lib, "pef", r2=10)
+    assert (PC.c_pitch(product_lib, "pef", o, np.ones(1000, np.float32), fill=7.0, extra=3) == 7).all()
     assert _batch(product_lib, o, np.ones((2, 1000), np.float32), True).size == 0
     product_lib.pitchPEFObj_free(o)
 
@@ -159,7 +150,7 @@ def test_refusals_on_device(product_lib, cuda_device):
 def test_reference_pitch_pef_on_b200(raf, cuda_device):
     """the reference's own PitchPEF class, on the reference build and on libaudioflux_b200.so, per channel of a
     multi-channel array; and this package's class giving the same arrays"""
-    x = _clips(6, 48000, 32000, 7).reshape(2, 3, 48000)
+    x = PC.clips(6, 48000, 32000, 7).reshape(2, 3, 48000)
     res = {}
     for which in ("ref", "b200"):
         raf.fftlib.set_fft_lib(lib_ext="b200" if which == "b200" else None)

@@ -7,6 +7,7 @@ launch per chunk; the refusals; and the reference's own PitchYIN class on libaud
 import numpy as np
 import pytest
 
+import _pitch_c as PC
 import _pitch_yin_oracle as YO
 from _parity_kit import Out, count_launches, dptr, raf, run_batch, stream  # noqa: F401  (raf: a fixture)
 from test_pitch_yin_cpu import FILL, reference_outputs
@@ -68,12 +69,12 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     # the batch with host and device pointers: clip 1 is clip 0 reversed and 1000 times louder
     x = YO.case_signal(name, kw)
     xs = np.stack([x, 1000 * x[::-1]])
-    st, o = YO.c_new(product_lib, **kw["ctor"])
+    st, o = PC.c_new(product_lib, "yin", **kw["ctor"])
     if kw["thresh"] is not None:
         product_lib.pitchYINObj_setThresh(o, kw["thresh"])
     legacy = []
     for c in xs:
-        res = YO.c_pitch(product_lib, o, c, FILL)
+        res = PC.c_pitch(product_lib, "yin", o, c, FILL)
         legacy.append(res + YO.c_troughs(product_lib, o, len(res[0])))
     for a, b in zip(legacy[0], got):
         assert np.array_equal(a, b)
@@ -85,25 +86,12 @@ def test_case_matches_oracle_and_reference(product_lib, cuda_device, name):
     product_lib.pitchYINObj_free(o)
 
 
-def _clips(n, length, sr, seed):
-    """harmonic tones of random f0 (80 .. 600 Hz), some without their fundamental, in noise; every fifth clip silent
-    in its second half"""
-    rng = np.random.default_rng(seed)
-    t = np.arange(length) / sr
-    f0 = rng.uniform(80, 600, (n, 1))
-    first = rng.integers(1, 3, (n, 1))
-    x = sum(np.where(first <= h, 0.3 / h, 0.0) * np.sin(2 * np.pi * f0 * h * t + h) for h in range(1, 6))
-    x = x + 0.05 * rng.standard_normal((n, length))
-    x[::5, length // 2:] = 0
-    return x.astype(np.float32)
-
-
 @gpu
 def test_batch_across_chunks(product_lib, cuda_device):
     """200 clips of 160 000 samples: three host staging chunks; host and device batches equal the legacy call, also
     without the value outputs and without the trough rows"""
-    x = _clips(200, 160000, 32000, 1)
-    st, o = YO.c_new(product_lib, sr=32000, lf=27.0, hf=2000.0, r2=12, slide=1024, auto=2048)
+    x = PC.clips(200, 160000, 32000, 1, silent_every=5)
+    st, o = PC.c_new(product_lib, "yin", sr=32000, lf=27.0, hf=2000.0, r2=12, slide=1024, auto=2048)
     assert st == 0
     host = _batch(product_lib, o, x, False)
     dev = _batch(product_lib, o, x, True)
@@ -115,7 +103,7 @@ def test_batch_across_chunks(product_lib, cuda_device):
     assert np.array_equal(bare[0], host[0][:40]) and all(np.array_equal(bare[i], host[i][:40]) for i in (3, 4, 5))
     assert (host[0] == FILL).any()                     # silent halves: frames without a trough keep the fill
     for c in (0, 1, 95, 96, 97, 191, 192, 199):
-        res = YO.c_pitch(product_lib, o, x[c], FILL)
+        res = PC.c_pitch(product_lib, "yin", o, x[c], FILL)
         for i in range(3):
             assert np.array_equal(host[i][c], res[i]), (c, i)
     p = YO.params(sr=32000, lf=27.0, hf=2000.0, r2=12, slide=1024, auto=2048)
@@ -128,11 +116,11 @@ def test_batch_across_chunks(product_lib, cuda_device):
 def test_device_calls_back_to_back(product_lib, cuda_device):
     """calls with different clip counts and lengths queued on one object without a synchronise"""
     import torch
-    st, o = YO.c_new(product_lib, sr=44100, r2=11, slide=512, auto=1024)
+    st, o = PC.c_new(product_lib, "yin", sr=44100, r2=11, slide=512, auto=1024)
     m = product_lib.pitchYINObj_getTroughData(o, None, None, None)
     calls = []
     for k, (b, n) in enumerate(((3, 30000), (17, 9000), (1, 2048), (40, 22050), (2, 60000))):
-        x = _clips(b, n, 44100, 10 + k)
+        x = PC.clips(b, n, 44100, 10 + k, silent_every=5)
         xd = torch.from_numpy(x).cuda()
         T = product_lib.pitchYINObj_calTimeLength(o, n)
         outs = [torch.full((b, T), FILL, device="cuda") for _ in range(3)]
@@ -144,7 +132,7 @@ def test_device_calls_back_to_back(product_lib, cuda_device):
     torch.cuda.synchronize()
     for x, _, outs, rows, lens in calls:
         for k in (0, len(x) - 1):
-            res = YO.c_pitch(product_lib, o, x[k], FILL)
+            res = PC.c_pitch(product_lib, "yin", o, x[k], FILL)
             res = res + YO.c_troughs(product_lib, o, len(res[0]))
             for i, v in enumerate(outs + rows + [lens]):
                 assert np.array_equal(v[k].cpu().numpy(), res[i]), (len(x), k, i)
@@ -155,15 +143,15 @@ def test_device_calls_back_to_back(product_lib, cuda_device):
 def test_streaming_equals_one_call(product_lib, cuda_device):
     """isContinue: uneven pieces (some shorter than a frame) give the frames of one call over the clip, for a slide
     below n and one above it; a batch call in between neither reads nor moves the carry"""
-    x = YO.signal("glide", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = YO.c_new(product_lib, sr=16000, r2=r2, slide=slide)
-        want = YO.c_pitch(product_lib, whole, x)
-        st, o = YO.c_new(product_lib, sr=16000, r2=r2, slide=slide, cont=1)
+        st, whole = PC.c_new(product_lib, "yin", sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(product_lib, "yin", whole, x)
+        st, o = PC.c_new(product_lib, "yin", sr=16000, r2=r2, slide=slide, cont=1)
         pieces = (700, 3000, 100, 9000, 1, 27199)
         got, start = [], 0
         for k, size in enumerate(pieces):
-            got.append(YO.c_pitch(product_lib, o, x[start:start + size]))
+            got.append(PC.c_pitch(product_lib, "yin", o, x[start:start + size]))
             start += size
             if k == 2:
                 _batch(product_lib, o, np.stack([x, x]), True)
@@ -178,11 +166,11 @@ def test_launch_count(product_lib, cuda_device):
     """one launch per staging chunk"""
     import torch
     h = af.PitchYIN(radix2_exp=11, slide_length=512, auto_length=1024)
-    x = _clips(8, 20000, 32000, 3)
+    x = PC.clips(8, 20000, 32000, 3, silent_every=5)
     xd = torch.from_numpy(x).cuda()
     assert count_launches(product_lib, lambda: h.pitch_batch(xd), warm=True) == 1
     assert count_launches(product_lib, lambda: h.pitch(x[0]), warm=True) == 1
-    big = _clips(200, 160000, 32000, 4)                  # 64 MB staging chunks: three of them
+    big = PC.clips(200, 160000, 32000, 4, silent_every=5)                  # 64 MB staging chunks: three of them
     assert count_launches(product_lib, lambda: h.pitch(big), warm=True) == 3
 
 
@@ -190,10 +178,10 @@ def test_launch_count(product_lib, cuda_device):
 def test_refusals_on_device(product_lib, cuda_device):
     """a refused constructor leaves no object; a call with fewer samples than the frame leaves the outputs untouched"""
     for kw, want in ((dict(r2=15), -2), (dict(sr=2000), -3), (dict(sr=8000, r2=10, auto=1021), -3)):
-        st, o = YO.c_new(product_lib, **kw)
+        st, o = PC.c_new(product_lib, "yin", **kw)
         assert st == want and not o
-    st, o = YO.c_new(product_lib, r2=10)
-    assert all((v == 7).all() for v in YO.c_pitch(product_lib, o, np.ones(1000, np.float32), fill=7.0, extra=3))
+    st, o = PC.c_new(product_lib, "yin", r2=10)
+    assert all((v == 7).all() for v in PC.c_pitch(product_lib, "yin", o, np.ones(1000, np.float32), fill=7.0, extra=3))
     assert _batch(product_lib, o, np.ones((2, 1000), np.float32), True)[0].size == 0
     product_lib.pitchYINObj_free(o)
 
@@ -202,7 +190,7 @@ def test_refusals_on_device(product_lib, cuda_device):
 def test_reference_pitch_yin_on_b200(raf, cuda_device):
     """the reference's own PitchYIN class (with set_thresh), on the reference build and on libaudioflux_b200.so, per
     channel of a multi-channel array; and this package's class giving the same arrays"""
-    x = _clips(6, 48000, 32000, 7).reshape(2, 3, 48000)
+    x = PC.clips(6, 48000, 32000, 7, silent_every=5).reshape(2, 3, 48000)
     res = {}
     for which in ("ref", "b200"):
         raf.fftlib.set_fft_lib(lib_ext="b200" if which == "b200" else None)

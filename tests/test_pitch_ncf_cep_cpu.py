@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none      # first: conftest puts the root on sys.path
+import _pitch_c as PC
 import _pitch_ncf_cep_oracle as PO
 
 CASES = {k: dict(PO.cases(k)) for k in PO.KINDS}
@@ -88,19 +89,19 @@ def test_statuses_match_reference(product_lib, ref_lib, kind):
     for kw in _grid():
         for slide in (None, 700):
             p = PO.params(kind, **kw, slide=slide)
-            st_p, o_p = PO.c_new(product_lib, kind, **kw, slide=slide)
+            st_p, o_p = PC.c_new(product_lib, kind, **kw, slide=slide)
             assert st_p == p["status"], (kw, slide, st_p, p["status"])
             seen.add(st_p)
             if st_p:
                 assert not o_p
                 continue
-            st_r, o_r = PO.c_new(ref_lib, kind, **kw, slide=slide)
+            st_r, o_r = PC.c_new(ref_lib, kind, **kw, slide=slide)
             assert st_r == 0
             for n in (0, 1, p["n"] - 1, p["n"], p["n"] + 1, p["n"] + p["slide"], 5 * p["n"] + 3, 100000):
-                got = PO.c_time_length(product_lib, kind, o_p, n)
-                assert got == PO.time_length(n, p["n"], p["slide"]) == PO.c_time_length(ref_lib, kind, o_r, n)
-            PO.c_free(product_lib, kind, o_p)
-            PO.c_free(ref_lib, kind, o_r)
+                got = PC.c_time_length(product_lib, kind, o_p, n)
+                assert got == PC.time_length(n, p["n"], p["slide"]) == PC.c_time_length(ref_lib, kind, o_r, n)
+            PC.c_free(product_lib, kind, o_p)
+            PC.c_free(ref_lib, kind, o_r)
     assert seen == {0, -2, -3}, seen
 
 
@@ -111,15 +112,15 @@ def test_streaming_in_the_reference(kind):
     lib = ref_lib_or_none()
     if lib is None:
         pytest.skip("needs the reference build")
-    x = PO.signal("chirp", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = PO.c_new(lib, kind, sr=16000, r2=r2, slide=slide)
-        want = PO.c_pitch(lib, kind, whole, x)
-        st, o = PO.c_new(lib, kind, sr=16000, r2=r2, slide=slide, cont=1)
-        got = PO.c_stream(lib, kind, o, x, (700, 3000, 100, 9000, 1, 27199))
+        st, whole = PC.c_new(lib, kind, sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(lib, kind, whole, x)
+        st, o = PC.c_new(lib, kind, sr=16000, r2=r2, slide=slide, cont=1)
+        got = PC.c_stream(lib, kind, o, x, (700, 3000, 100, 9000, 1, 27199))
         assert np.array_equal(got, want), (r2, slide)
-        PO.c_free(lib, kind, o)
-        PO.c_free(lib, kind, whole)
+        PC.c_free(lib, kind, o)
+        PC.c_free(lib, kind, whole)
 
 
 def test_cep_window_rule():
@@ -127,12 +128,12 @@ def test_cep_window_rule():
     lib = ref_lib_or_none()
     if lib is None:
         pytest.skip("needs the reference build")
-    x = PO.signal("tones", 20000, 32000, 3)
+    x = PC.signal("tones", 20000, 32000, 3)
     outs = []
     for wt in (PO.W_HAMM, PO.W_BLACKMAN, PO.W_HANN):
-        st, o = PO.c_new(lib, "cep", r2=12, slide=1024, wt=wt)
-        outs.append(PO.c_pitch(lib, "cep", o, x))
-        PO.c_free(lib, "cep", o)
+        st, o = PC.c_new(lib, "cep", r2=12, slide=1024, wt=wt)
+        outs.append(PC.c_pitch(lib, "cep", o, x))
+        PC.c_free(lib, "cep", o)
     assert np.array_equal(outs[0], outs[1]) and not np.array_equal(outs[0], outs[2])
     assert PO.params("cep", wt=PO.W_BLACKMAN)["wt"] == PO.W_HAMM
 
@@ -151,34 +152,34 @@ def test_refusals(product_lib):
                                ("cep", dict(lf=3000.0), -3, b"is empty")):
         p = PO.params(kind, **kw)
         assert p["status"] == st, (kind, kw, p["status"])
-        s, o = PO.c_new(L, kind, **kw)
+        s, o = PC.c_new(L, kind, **kw)
         assert s == st and not o, (kind, kw, s)
         assert what in L.afb200_lastError(), L.afb200_lastError()
     for kind, r2 in (("ncf", 10), ("cep", 9)):                          # just inside the bounds: 1000 < 1024
-        s, o = PO.c_new(L, kind, r2=r2)
+        s, o = PC.c_new(L, kind, r2=r2)
         assert s == 0
-        PO.c_free(L, kind, o)
-    s, o = PO.c_new(L, "cep", r2=1, sr=8000, lf=3000.0, hf=3500.0)       # n = 2: the default slide n/4 = 0 becomes 1
-    assert s == 0 and PO.c_time_length(L, "cep", o, 10) == 9
-    PO.c_free(L, "cep", o)
+        PC.c_free(L, kind, o)
+    s, o = PC.c_new(L, "cep", r2=1, sr=8000, lf=3000.0, hf=3500.0)       # n = 2: the default slide n/4 = 0 becomes 1
+    assert s == 0 and PC.c_time_length(L, "cep", o, 10) == 9
+    PC.c_free(L, "cep", o)
     for kind in PO.KINDS:
-        s, o = PO.c_new(L, kind, r2=12)
-        assert (PO.c_pitch(L, kind, o, np.ones(4095, np.float32), fill=7.0, extra=4) == 7).all()
+        s, o = PC.c_new(L, kind, r2=12)
+        assert (PC.c_pitch(L, kind, o, np.ones(4095, np.float32), fill=7.0, extra=4) == 7).all()
         v = np.zeros(4, np.float32)
-        batch = getattr(L, PO.PREFIX[kind] + "_pitchBatch")
+        batch = getattr(L, PC.prefix(kind) + "_pitchBatch")
         assert batch(o, None, 8192, 1, v.ctypes.data, 0, None) != 0
         assert b"bad argument" in L.afb200_lastError()
         assert batch(o, v.ctypes.data, 4, -1, v.ctypes.data, 0, None) != 0
-        PO.c_free(L, kind, o)
-        PO.c_free(L, kind, None)
-        getattr(L, PO.PREFIX[kind] + "_pitch")(None, None, 0, None)
-        assert PO.c_time_length(L, kind, None, 100000) == 0
+        PC.c_free(L, kind, o)
+        PC.c_free(L, kind, None)
+        getattr(L, PC.prefix(kind) + "_pitch")(None, None, 0, None)
+        assert PC.c_time_length(L, kind, None, 100000) == 0
 
 
 @pytest.mark.parametrize("kind", PO.KINDS)
 def test_pitch_symbols_exported_and_bound(product_lib, kind):
     from audioflux_b200 import capi
-    pre = PO.PREFIX[kind]
+    pre = PC.prefix(kind)
     check_symbols(product_lib, f"afb200_pitch_{kind}.h", pre + "_",
                   capi.PITCH_NCF_API if kind == "ncf" else capi.PITCH_CEP_API,
                   {pre + s for s in ("_new", "_calTimeLength", "_pitch", "_enableDebug", "_free")}, {pre + "_pitchBatch"})

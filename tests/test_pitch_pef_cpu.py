@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none      # first: conftest puts the root on sys.path
+import _pitch_c as PC
 import _pitch_pef_oracle as PO
 
 CASES = dict(PO.cases())
@@ -69,17 +70,17 @@ def test_statuses_match_reference(product_lib, ref_lib):
     for kw in _grid():
         for slide in (None, 700):
             p = PO.params(**kw, slide=slide)
-            st_p, o_p = PO.c_new(product_lib, **kw, slide=slide)
+            st_p, o_p = PC.c_new(product_lib, "pef", **kw, slide=slide)
             assert st_p == p["status"], (kw, slide, st_p, p["status"])
             seen.add(st_p)
             if st_p:
                 assert not o_p
                 continue
-            st_r, o_r = PO.c_new(ref_lib, **kw, slide=slide)
+            st_r, o_r = PC.c_new(ref_lib, "pef", **kw, slide=slide)
             assert st_r == 0
             for n in (0, 1, p["n"] - 1, p["n"], p["n"] + 1, p["n"] + p["slide"], 5 * p["n"] + 3, 100000):
                 got = product_lib.pitchPEFObj_calTimeLength(o_p, n)
-                assert got == PO.time_length(n, p["n"], p["slide"]) == ref_lib.pitchPEFObj_calTimeLength(o_r, n)
+                assert got == PC.time_length(n, p["n"], p["slide"]) == ref_lib.pitchPEFObj_calTimeLength(o_r, n)
             product_lib.pitchPEFObj_free(o_p)
             ref_lib.pitchPEFObj_free(o_r)
     assert seen == {0, -2, -3}, seen
@@ -91,12 +92,12 @@ def test_streaming_in_the_reference():
     lib = ref_lib_or_none()
     if lib is None:
         pytest.skip("needs the reference build")
-    x = PO.signal("glide", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = PO.c_new(lib, sr=16000, r2=r2, slide=slide)
-        want = PO.c_pitch(lib, whole, x)
-        st, o = PO.c_new(lib, sr=16000, r2=r2, slide=slide, cont=1)
-        got = PO.c_stream(lib, o, x, (700, 3000, 100, 9000, 1, 27199))
+        st, whole = PC.c_new(lib, "pef", sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(lib, "pef", whole, x)
+        st, o = PC.c_new(lib, "pef", sr=16000, r2=r2, slide=slide, cont=1)
+        got = PC.c_stream(lib, "pef", o, x, (700, 3000, 100, 9000, 1, 27199))
         assert np.array_equal(got, want), (r2, slide)
         lib.pitchPEFObj_free(o)
         lib.pitchPEFObj_free(whole)
@@ -114,14 +115,14 @@ def test_refusals(product_lib):
                          (dict(r2=11, beta=1.0, hf=hf_top, cf=4000.0), -4, b"reads past")):
         p = PO.params(**kw)
         assert p["status"] == st, (kw, p["status"])
-        s, o = PO.c_new(L, **kw)
+        s, o = PC.c_new(L, "pef", **kw)
         assert s == st and not o, (kw, s)
         assert what in L.afb200_lastError(), L.afb200_lastError()
-    s, o = PO.c_new(L, r2=1)                         # n = 2: the default slide n/4 = 0 becomes 1
+    s, o = PC.c_new(L, "pef", r2=1)                         # n = 2: the default slide n/4 = 0 becomes 1
     assert s == 0 and L.pitchPEFObj_calTimeLength(o, 10) == 9
     L.pitchPEFObj_free(o)
-    s, o = PO.c_new(L, r2=10)
-    assert (PO.c_pitch(L, o, np.ones(1023, np.float32), fill=7.0, extra=4) == 7).all()
+    s, o = PC.c_new(L, "pef", r2=10)
+    assert (PC.c_pitch(L, "pef", o, np.ones(1023, np.float32), fill=7.0, extra=4) == 7).all()
     v = np.zeros(4, np.float32)
     assert L.pitchPEFObj_pitchBatch(o, None, 2048, 1, v.ctypes.data, 0, None) != 0
     assert b"bad argument" in L.afb200_lastError()
@@ -136,14 +137,14 @@ def test_set_filter_params_changes_nothing():
     lib = ref_lib_or_none()
     if lib is None:
         pytest.skip("needs the reference build")
-    x = PO.signal("missing", 30000, 32000, 3)
-    st, o = PO.c_new(lib, r2=12, slide=1024)
-    before = PO.c_pitch(lib, o, x)
+    x = PC.signal("missing", 30000, 32000, 3)
+    st, o = PC.c_new(lib, "pef", r2=12, slide=1024)
+    before = PC.c_pitch(lib, "pef", o, x)
     lib.pitchPEFObj_setFilterParams(o, 3.0, 0.9, 1.2)
-    after = PO.c_pitch(lib, o, x)
+    after = PC.c_pitch(lib, "pef", o, x)
     lib.pitchPEFObj_free(o)
-    st, o = PO.c_new(lib, r2=12, slide=1024, alpha=3.0, beta=0.9, gamma=1.2)
-    other = PO.c_pitch(lib, o, x)
+    st, o = PC.c_new(lib, "pef", r2=12, slide=1024, alpha=3.0, beta=0.9, gamma=1.2)
+    other = PC.c_pitch(lib, "pef", o, x)
     lib.pitchPEFObj_free(o)
     assert np.array_equal(before, after) and not np.array_equal(before, other)
 

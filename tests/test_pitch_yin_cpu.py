@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from _parity_kit import GoldenStore, check_symbols, ref_lib_or_none      # first: conftest puts the root on sys.path
+import _pitch_c as PC
 import _pitch_yin_oracle as YO
 
 CASES = dict(YO.cases())
@@ -92,17 +93,17 @@ def test_statuses_match_reference(product_lib, ref_lib):
     for kw in _grid():
         for slide in (None, 700):
             p = YO.params(**kw, slide=slide)
-            st_p, o_p = YO.c_new(product_lib, **kw, slide=slide)
+            st_p, o_p = PC.c_new(product_lib, "yin", **kw, slide=slide)
             assert st_p == p["status"], (kw, slide, st_p, p["status"])
             seen.add(st_p)
             if st_p:
                 assert not o_p
                 continue
-            st_r, o_r = YO.c_new(ref_lib, **kw, slide=slide)
+            st_r, o_r = PC.c_new(ref_lib, "yin", **kw, slide=slide)
             assert st_r == 0
             for n in (0, 1, p["n"] - 1, p["n"], p["n"] + 1, p["n"] + p["slide"], 5 * p["n"] + 3, 100000):
                 got = product_lib.pitchYINObj_calTimeLength(o_p, n)
-                assert got == YO.time_length(n, p["n"], p["slide"]) == ref_lib.pitchYINObj_calTimeLength(o_r, n)
+                assert got == PC.time_length(n, p["n"], p["slide"]) == ref_lib.pitchYINObj_calTimeLength(o_r, n)
             assert product_lib.pitchYINObj_getTroughData(o_p, None, None, None) == p["m_len"]
             product_lib.pitchYINObj_free(o_p)
             ref_lib.pitchYINObj_free(o_r)
@@ -115,12 +116,12 @@ def test_streaming_in_the_reference():
     lib = ref_lib_or_none()
     if lib is None:
         pytest.skip("needs the reference build")
-    x = YO.signal("glide", 40000, 16000, 5)
+    x = PC.signal("glide", 40000, 16000, 5)
     for r2, slide in ((11, 512), (10, 1500)):
-        st, whole = YO.c_new(lib, sr=16000, r2=r2, slide=slide)
-        want = YO.c_pitch(lib, whole, x)
-        st, o = YO.c_new(lib, sr=16000, r2=r2, slide=slide, cont=1)
-        got = YO.c_stream(lib, o, x, (700, 3000, 100, 9000, 1, 27199))
+        st, whole = PC.c_new(lib, "yin", sr=16000, r2=r2, slide=slide)
+        want = PC.c_pitch(lib, "yin", whole, x)
+        st, o = PC.c_new(lib, "yin", sr=16000, r2=r2, slide=slide, cont=1)
+        got = PC.c_stream(lib, "yin", o, x, (700, 3000, 100, 9000, 1, 27199))
         for g, w in zip(got, want):
             assert np.array_equal(g, w), (r2, slide)
         lib.pitchYINObj_free(o)
@@ -138,14 +139,14 @@ def test_refusals(product_lib):
                          (dict(sr=8000, r2=10, auto=1021), -3, b"yinLength=0 is empty")):
         p = YO.params(**kw)
         assert p["status"] == st, (kw, p["status"])
-        s, o = YO.c_new(L, **kw)
+        s, o = PC.c_new(L, "yin", **kw)
         assert s == st and not o, (kw, s)
         assert what in L.afb200_lastError(), L.afb200_lastError()
-    s, o = YO.c_new(L, sr=4000, r2=1, auto=0)          # n = 2: the default slide n/4 = 0 becomes 1
+    s, o = PC.c_new(L, "yin", sr=4000, r2=1, auto=0)          # n = 2: the default slide n/4 = 0 becomes 1
     assert s == 0 and L.pitchYINObj_calTimeLength(o, 10) == 9
     L.pitchYINObj_free(o)
-    s, o = YO.c_new(L, r2=10)
-    assert all((v == 7).all() for v in YO.c_pitch(L, o, np.ones(1023, np.float32), fill=7.0, extra=4))
+    s, o = PC.c_new(L, "yin", r2=10)
+    assert all((v == 7).all() for v in PC.c_pitch(L, "yin", o, np.ones(1023, np.float32), fill=7.0, extra=4))
     assert L.pitchYINObj_getTroughData(o, None, None, None) == YO.params(r2=10)["m_len"]
     v = np.zeros(4, np.float32)
     assert L.pitchYINObj_pitchBatch(o, None, 2048, 1, v.ctypes.data, None, None, None, None, None, 0, None) != 0

@@ -48,6 +48,8 @@ BUDGETS = [
     Budget("pitch_pef.cu", {"k_pitch_pef": "k_pitch_pef"}, 32, 0, 0, ("-fmad=false",)),
     # CTAs of up to 1024 threads; the launcher sizes them for 1536 threads per SM (65 536 registers / 40, rounded down)
     Budget("pitch_yin.cu", {"k_pitch_yin": "k_pitch_yin"}, 40, 0, 0, ("-fmad=false",)),
+    # CTAs of up to 1024 threads; the launcher sizes them for 2048 threads per SM (65 536 registers / 32)
+    Budget("pitch_ncf_cep.cu", {"k_pitch_ncf": "k_pitch_ncf", "k_pitch_cep": "k_pitch_cep"}, 32, 0, 0, ("-fmad=false",)),
 ]
 
 
